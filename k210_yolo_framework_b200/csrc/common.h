@@ -65,10 +65,6 @@ struct DwArgs {
     int B, H, W, C, OH, OW, stride, pad_t, pad_l;
     int act;
     float alpha;
-    // [11][cpad] = 9 tap rows, scale, shift, zero-padded to cpad = ceil(C / 64) * 64 channels: the fused depthwise->pointwise
-    // kernel brings it into shared memory with one bulk copy (null: the kernel gathers it from w / scale / shift)
-    const float *pack = nullptr;
-    int cpad = 0;
 };
 
 struct PoolArgs {

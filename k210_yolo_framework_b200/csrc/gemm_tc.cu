@@ -5,16 +5,15 @@
 // One persistent CTA per SM walks the (k-slice, m-tile, n-tile) work list; a tile is 128 GEMM rows x BN columns.
 //   warpgroup 0  producers   one elected lane of warp 0 issues the TMA loads of the weight tile (hi/lo planes) every
 //                            k-block, and of the A tile too when the conv is a plain 1x1 (A is then the [M,K] row-major
-//                            activation matrix).  Otherwise all 128 threads fill the A tile: 3x3 / strided / concat /
-//                            nearest-upsample inputs are gathered with cp.async (zero-fill = padding), and a fused
-//                            depthwise 3x3 layer (DWFUSE) is computed straight into it.  A is stored as fp32 in the
+//                            activation matrix).  Otherwise all 128 threads gather the A tile of a 3x3 / strided / concat /
+//                            nearest-upsample input with cp.async (zero-fill = padding).  A is stored as fp32 in the
 //                            128B-swizzled K-major layout, 128 rows x 128 bytes per 16 KB sub-tile.
 //   warpgroups 1-2  consumers  64 rows each: read their A rows from shared memory into the wgmma A register fragment,
 //                            split them into hi/lo planes (3xTF32: hi = tf32(a), lo = tf32(a - hi); bf16x3: hi = bf16(a),
 //                            mid = bf16(a - hi); the weights were split on the host), so that lo*hi + hi*lo + hi*hi
 //                            recovers fp32-class accuracy from the tensor cores; B comes from shared memory.  After the
 //                            last k-block of a tile they apply folded BN, activation and residual and store to HBM.
-// mbarrier ring per stage: full_b (TMA tx) / full_a (cp.async or st.shared arrivals) -> [consumers] -> empty.
+// mbarrier ring per stage: full_b (TMA tx) / full_a (cp.async arrivals) -> [consumers] -> empty.
 //
 // Replaces the TF Conv2D + FusedBatchNorm + LeakyRelu/Relu6 (+ ResizeNearestNeighbor/ConcatV2/Add) ops that
 // models/yolonet.py:244-260 and models/keras_mobilenet*.py compose.
@@ -59,10 +58,6 @@ struct TcParams {
     int a_boxes;                    // 16 KB sub-tiles of raw fp32 A per stage (k per k-block / 32)
     int half_taps;                  // gather: Cin is half a k-block (16 with tf32, 32 with bf16 k-blocks), a k-block holds TWO consecutive taps
     float act_slope, act_clamp;     // branch-free activation parameters
-    // fused depthwise producer (DWFUSE): A = act(BN(depthwise3x3(src0))), channels of k-block kb = [kb * KBK, kb * KBK + KBK)
-    const float *dw_pack;           // [11][dw_cpad]: 9 tap rows, scale, shift (zero beyond C0)
-    int dw_cpad, dw_act;
-    float dw_alpha;
 };
 
 struct __align__(8) Barriers {
@@ -78,7 +73,7 @@ __device__ __forceinline__ uint32_t a_addr(uint32_t box, int r, int k) {
 
 // BNT = the tile width p.BN, a compile-time constant so that every accumulator register and every wgmma of the consumers is
 // fixed at compile time (a runtime-sliced accumulator made ptxas serialise the wgmma pipeline)
-template <bool GATHER, bool DWFUSE, int BNT>
+template <bool GATHER, int BNT>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_bhi,
                const __grid_constant__ CUtensorMap map_blo, const TcParams p) {
@@ -129,7 +124,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             const int kb0 = ks * p.kb_per_split, kb1 = min(p.nkb, kb0 + p.kb_per_split);
             const int m = mt * BM + r;
             int b = -1, iy0 = 0, ix0 = 0;
-            if (GATHER && !DWFUSE && m < p.M) {
+            if (GATHER && m < p.M) {
                 const int ox = m % p.OW;
                 const int q = m / p.OW;
                 const int oy = q % p.OH;
@@ -152,50 +147,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                     }
                     __syncwarp();
                 }
-                if (DWFUSE) {
-                    // the A tile is computed, not copied: item = (GEMM row, channel quad), lanes run over the quads of a row
-                    // first so that a load instruction reads whole pixels' channel runs.  Tap order (ky, kx) ascending with
-                    // fmaf and BN as one fmaf, like the stand-alone depthwise kernel.
-                    const int qpk = KBK / 4;
-                    const uint32_t stg = stage_a(s);
-                    for (int it = r; it < BM * qpk; it += 128) {
-                        const int qd = it % qpk, row = it / qpk;
-                        const int c = kb * KBK + qd * 4;
-                        const int mm = mt * BM + row;
-                        float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (mm < p.M && c < p.C0) {
-                            const int ox = mm % p.OW;
-                            const int q = mm / p.OW;
-                            const int oy = q % p.OH, bb = q / p.OH;
-                            float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                            for (int ky = 0; ky < 3; ++ky) {
-                                const int iy = oy * p.stride - p.pad_t + ky;
-#pragma unroll
-                                for (int kx = 0; kx < 3; ++kx) {
-                                    const int ix = ox * p.stride - p.pad_l + kx;
-                                    if (iy < 0 || iy >= p.H || ix < 0 || ix >= p.W) continue;
-                                    const float4 x = __ldg(reinterpret_cast<const float4 *>(p.src0 + ((size_t)(bb * p.H + iy) * p.W + ix) * p.C0 + c));
-                                    const float4 w = __ldg(reinterpret_cast<const float4 *>(p.dw_pack + (size_t)(ky * 3 + kx) * p.dw_cpad + c));
-                                    acc.x = fmaf(x.x, w.x, acc.x);
-                                    acc.y = fmaf(x.y, w.y, acc.y);
-                                    acc.z = fmaf(x.z, w.z, acc.z);
-                                    acc.w = fmaf(x.w, w.w, acc.w);
-                                }
-                            }
-                            const float4 sc = __ldg(reinterpret_cast<const float4 *>(p.dw_pack + (size_t)9 * p.dw_cpad + c));
-                            const float4 sh = __ldg(reinterpret_cast<const float4 *>(p.dw_pack + (size_t)10 * p.dw_cpad + c));
-                            o.x = apply_act(fmaf(acc.x, sc.x, sh.x), p.dw_act, p.dw_alpha);
-                            o.y = apply_act(fmaf(acc.y, sc.y, sh.y), p.dw_act, p.dw_alpha);
-                            o.z = apply_act(fmaf(acc.z, sc.z, sh.z), p.dw_act, p.dw_alpha);
-                            o.w = apply_act(fmaf(acc.w, sc.w, sh.w), p.dw_act, p.dw_alpha);
-                        }
-                        const uint32_t box = stg + (uint32_t)(qd >> 3) * A_TILE_BYTES;
-                        st_shared_v4(box + (uint32_t)row * 128u + ((uint32_t)((qd & 7) ^ (row & 7)) << 4), __float_as_uint(o.x),
-                                     __float_as_uint(o.y), __float_as_uint(o.z), __float_as_uint(o.w));
-                    }
-                    mbar_arrive(smem_u32(&bars->full_a[s]));
-                } else if (GATHER) {
+                if (GATHER) {
                     // Each k-block is KBK consecutive channels of one filter tap, i.e. one contiguous run per output pixel.
                     // Thread r computes the source address of GEMM row r; the addresses are exchanged with warp shuffles so
                     // that 8 (tf32) or 16 (bf16) consecutive lanes copy one row's run with 16-byte cp.async.
@@ -564,12 +516,10 @@ void pick_tile(int M, int N, int nkb, bool three_x, bool bf16, bool gather, size
     const int n16 = (N + 15) / 16 * 16;
     const int m_tiles = (M + BM - 1) / BM;
     const char *force = getenv("K2Y_TC_SPLITK");
-    const char *force_bn = getenv("K2Y_TC_BN");
     int best = 16, best_s = 1;
     double best_cost = 1e30;
     for (int bn = 16; bn <= MAX_BN; bn += 16) {
         if (bn > n16) break;
-        if (force_bn && bn != atoi(force_bn)) continue;
         const int stages = stages_for(bn, three_x, bf16);
         if (stages < 2) continue;
         const int n_tiles = (n16 + bn - 1) / bn;
@@ -604,21 +554,21 @@ void pick_tile(int M, int N, int nkb, bool three_x, bool bf16, bool gather, size
     *splits_out = best_s;
 }
 
-template <bool G, bool D>
-using ConvKernel = decltype(&conv_tc_kernel<G, D, 16>);
+template <bool G>
+using ConvKernel = decltype(&conv_tc_kernel<G, 16>);
 
 // the instantiation for tile width bn (a multiple of 16 up to MAX_BN)
-template <bool G, bool D>
-ConvKernel<G, D> conv_kernel_for(int bn) {
+template <bool G>
+ConvKernel<G> conv_kernel_for(int bn) {
     switch (bn) {
-        case 16: return conv_tc_kernel<G, D, 16>;
-        case 32: return conv_tc_kernel<G, D, 32>;
-        case 48: return conv_tc_kernel<G, D, 48>;
-        case 64: return conv_tc_kernel<G, D, 64>;
-        case 80: return conv_tc_kernel<G, D, 80>;
-        case 96: return conv_tc_kernel<G, D, 96>;
-        case 112: return conv_tc_kernel<G, D, 112>;
-        case 128: return conv_tc_kernel<G, D, 128>;
+        case 16: return conv_tc_kernel<G, 16>;
+        case 32: return conv_tc_kernel<G, 32>;
+        case 48: return conv_tc_kernel<G, 48>;
+        case 64: return conv_tc_kernel<G, 64>;
+        case 80: return conv_tc_kernel<G, 80>;
+        case 96: return conv_tc_kernel<G, 96>;
+        case 112: return conv_tc_kernel<G, 112>;
+        case 128: return conv_tc_kernel<G, 128>;
         default: return nullptr;
     }
 }
@@ -635,11 +585,9 @@ int tc_init() {
     cudaDeviceProp prop;
     K2Y_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
     for (int bn = 16; bn <= MAX_BN; bn += 16) {
-        K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<false, false>(bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
+        K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<false>(bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                             (int)prop.sharedMemPerBlockOptin));
-        K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<true, false>(bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)prop.sharedMemPerBlockOptin));
-        K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<true, true>(bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
+        K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<true>(bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                             (int)prop.sharedMemPerBlockOptin));
     }
     if (g_num_sms == 0) {
@@ -728,27 +676,35 @@ bool tc_supported(const ConvArgs &a, const TcWeights &w) {
     return is_half_taps(a, 16) && (((uintptr_t)a.src0) & 15) == 0;
 }
 
-// Fused MobileNet block: depthwise 3x3 stride 1 (SAME) + BN + act, then the plain 1x1 conv that reads it.  The producer
-// warpgroup computes the depthwise result straight into the A stage of the tensor-core kernel, so it never reaches HBM.
-bool dwpw_supported(const DwArgs &dw, const ConvArgs &pw, const TcWeights &w, int math_mode) {
-    if (math_mode != K2Y_MATH_TC_BF16X3 || !is_plain_1x1(pw) || !tc_supported(pw, w) || pw.residual) return false;
-    if (dw.stride != 1 || dw.pad_t != 1 || dw.pad_l != 1 || dw.OH != dw.H || dw.OW != dw.W) return false;
-    if (pw.src0 != dw.dst || pw.C0 != dw.C || pw.C1 != 0 || pw.OH != dw.OH || pw.OW != dw.OW || pw.B != dw.B) return false;
-    if ((dw.C & 3) || dw.C > 512 || pw.N > 384 || !dw.pack || dw.cpad < dw.C || (dw.cpad & 3)) return false;
-    return (((uintptr_t)dw.src) & 15) == 0 && (((uintptr_t)dw.pack) & 15) == 0;
-}
+// The tile plan of one conv with K = kh*kw*Cin: what the launch, the launch count and the host-only planner view all read.
+struct TcPlan {
+    int mode;                   // effective math mode (effective_mode)
+    bool gather;                // A gathered by the producer warpgroup; false: TMA loads of a plain 1x1 conv's [M,K] rows
+    int nkb;                    // k-blocks: 64 k each with bf16x3, 32 k otherwise
+    int bn, stages;
+    int k_splits, kb_per_split;
+    int m_tiles, n_tiles, grid;  // grid: persistent CTAs, at most the SM budget
+};
 
-static cudaError_t launch_conv(const ConvArgs &a, const TcWeights &w, int math_mode, cudaStream_t st, const DwArgs *dw);
-
-cudaError_t launch_dwpw_tc(const DwArgs &dw, const ConvArgs &pw, const TcWeights &w, cudaStream_t st) {
-    return launch_conv(pw, w, K2Y_MATH_TC_BF16X3, st, &dw);
+static TcPlan plan_conv(const ConvArgs &a, int K, int math_mode) {
+    TcPlan pl;
+    pl.mode = effective_mode(a, math_mode);
+    const bool bf = pl.mode == K2Y_MATH_TC_BF16X3, three_x = pl.mode != K2Y_MATH_TC_TF32;
+    pl.gather = !is_plain_1x1(a);
+    pl.nkb = bf ? (K + 63) / 64 : (K + BK - 1) / BK;
+    const int M = a.B * a.OH * a.OW, sms = budget_sms(a.sm_limit);
+    pick_tile(M, a.N, pl.nkb, three_x, bf, pl.gather, a.tc_scratch ? a.tc_scratch_bytes : 0, sms, &pl.bn, &pl.k_splits);
+    pl.kb_per_split = (pl.nkb + pl.k_splits - 1) / pl.k_splits;
+    pl.k_splits = (pl.nkb + pl.kb_per_split - 1) / pl.kb_per_split;  // no empty slices
+    pl.stages = stages_for(pl.bn, three_x, bf);
+    pl.m_tiles = (M + BM - 1) / BM;
+    pl.n_tiles = ((a.N + 15) / 16 * 16 + pl.bn - 1) / pl.bn;
+    const int tiles = pl.m_tiles * pl.n_tiles * pl.k_splits;
+    pl.grid = tiles < sms ? tiles : sms;
+    return pl;
 }
 
 cudaError_t launch_conv_tc(const ConvArgs &a, const TcWeights &w, int math_mode, cudaStream_t st) {
-    return launch_conv(a, w, math_mode, st, nullptr);
-}
-
-static cudaError_t launch_conv(const ConvArgs &a, const TcWeights &w, int math_mode, cudaStream_t st, const DwArgs *dw) {
     DevState *ds = cur_dev();
     if (!ds) return cudaErrorInvalidDevice;
     if (!ds->init && tc_init() != K2Y_OK) return cudaErrorNotReady;  // first launch on this device: attributes
@@ -777,32 +733,18 @@ static cudaError_t launch_conv(const ConvArgs &a, const TcWeights &w, int math_m
     p.M = a.B * a.OH * a.OW;
     p.N = a.N;
     p.K = w.K;
-    if (dw) {  // fused depthwise producer: the producer warpgroup reads the depthwise INPUT
-        p.src0 = dw->src;
-        p.H = dw->H;
-        p.W = dw->W;
-        p.stride = dw->stride;
-        p.pad_t = dw->pad_t;
-        p.pad_l = dw->pad_l;
-        p.dw_pack = dw->pack;
-        p.dw_cpad = dw->cpad;
-        p.dw_act = dw->act;
-        p.dw_alpha = dw->alpha;
-    }
-    math_mode = effective_mode(a, math_mode);
-    p.bf16 = (math_mode == K2Y_MATH_TC_BF16X3) ? 1 : 0;
-    p.three_x = (math_mode == K2Y_MATH_TC_TF32) ? 0 : 1;
+    const TcPlan pl = plan_conv(a, w.K, math_mode);
+    p.bf16 = (pl.mode == K2Y_MATH_TC_BF16X3) ? 1 : 0;
+    p.three_x = (pl.mode == K2Y_MATH_TC_TF32) ? 0 : 1;
     p.a_boxes = p.bf16 ? 2 : 1;
-    p.half_taps = (!dw && is_half_taps(a, p.bf16 ? 32 : 16)) ? 1 : 0;
-    p.nkb = p.bf16 ? w.Kpad64 / 64 : w.Kpad / BK;
-    const bool gather = !is_plain_1x1(a) || dw != nullptr;
-    const int sms = budget_sms(a.sm_limit);
-    pick_tile(p.M, a.N, p.nkb, p.three_x != 0, p.bf16 != 0, gather, a.tc_scratch ? a.tc_scratch_bytes : 0, sms, &p.BN, &p.k_splits);
-    p.n_tiles = (w.Npad + p.BN - 1) / p.BN;
-    p.m_tiles = (p.M + BM - 1) / BM;
-    p.kb_per_split = (p.nkb + p.k_splits - 1) / p.k_splits;
-    p.k_splits = (p.nkb + p.kb_per_split - 1) / p.kb_per_split;  // no empty slices
-    p.stages = stages_for(p.BN, p.three_x != 0, p.bf16 != 0);
+    p.half_taps = is_half_taps(a, p.bf16 ? 32 : 16) ? 1 : 0;
+    p.nkb = pl.nkb;
+    p.BN = pl.bn;
+    p.n_tiles = pl.n_tiles;
+    p.m_tiles = pl.m_tiles;
+    p.kb_per_split = pl.kb_per_split;
+    p.k_splits = pl.k_splits;
+    p.stages = pl.stages;
     if (p.stages < 2) return cudaErrorInvalidConfiguration;
     const size_t smem = FIXED_SMEM + (size_t)p.stages * stage_bytes_of(p.BN, p.three_x != 0, p.bf16 != 0);
 
@@ -824,7 +766,7 @@ static cudaError_t launch_conv(const ConvArgs &a, const TcWeights &w, int math_m
         p.dst = scratch;
         p.residual = nullptr;
     }
-    if (!gather && !make_map_2d(&map_a, a.src0, (uint64_t)p.M, (uint64_t)(a.C0 + a.C1), BM)) return cudaErrorInvalidValue;
+    if (!pl.gather && !make_map_2d(&map_a, a.src0, (uint64_t)p.M, (uint64_t)(a.C0 + a.C1), BM)) return cudaErrorInvalidValue;
     if (p.bf16) {
         if (!make_map_2d(&map_bhi, w.d_bh, (uint64_t)w.Npad, (uint64_t)w.Kpad64, (uint32_t)p.BN, 0, true)) return cudaErrorInvalidValue;
         if (!make_map_2d(&map_blo, w.d_bm, (uint64_t)w.Npad, (uint64_t)w.Kpad64, (uint32_t)p.BN, 0, true)) return cudaErrorInvalidValue;
@@ -833,13 +775,10 @@ static cudaError_t launch_conv(const ConvArgs &a, const TcWeights &w, int math_m
         if (!make_map_2d(&map_blo, w.d_lo, (uint64_t)w.Npad, (uint64_t)w.Kpad, (uint32_t)p.BN)) return cudaErrorInvalidValue;
     }
 
-    const int tiles = p.m_tiles * p.n_tiles * p.k_splits;
-    const int grid = tiles < sms ? tiles : sms;
     if (p.BN % 16 != 0 || p.BN > MAX_BN) return cudaErrorInvalidConfiguration;
-    const dim3 g((unsigned)grid), b(NUM_THREADS);
-    cudaError_t le = dw       ? launch_k(conv_kernel_for<true, true>(p.BN), g, b, smem, st, map_a, map_bhi, map_blo, p)
-                     : gather ? launch_k(conv_kernel_for<true, false>(p.BN), g, b, smem, st, map_a, map_bhi, map_blo, p)
-                              : launch_k(conv_kernel_for<false, false>(p.BN), g, b, smem, st, map_a, map_bhi, map_blo, p);
+    const dim3 g((unsigned)pl.grid), b(NUM_THREADS);
+    cudaError_t le = pl.gather ? launch_k(conv_kernel_for<true>(p.BN), g, b, smem, st, map_a, map_bhi, map_blo, p)
+                               : launch_k(conv_kernel_for<false>(p.BN), g, b, smem, st, map_a, map_bhi, map_blo, p);
     if (le != cudaSuccess) return le;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
@@ -853,13 +792,7 @@ static cudaError_t launch_conv(const ConvArgs &a, const TcWeights &w, int math_m
 }
 
 int tc_launch_count(const ConvArgs &a, const TcWeights &w, int math_mode) {
-    int bn = 0, splits = 1;
-    const int mode = effective_mode(a, math_mode);
-    const bool bf = mode == K2Y_MATH_TC_BF16X3;
-    const int M = a.B * a.OH * a.OW, nkb = bf ? w.Kpad64 / 64 : w.Kpad / BK;
-    pick_tile(M, a.N, nkb, mode != K2Y_MATH_TC_TF32, bf, !is_plain_1x1(a), a.tc_scratch ? a.tc_scratch_bytes : 0,
-              budget_sms(a.sm_limit), &bn, &splits);
-    return splits > 1 ? 2 : 1;
+    return plan_conv(a, w.K, math_mode).k_splits > 1 ? 2 : 1;
 }
 
 // Upper bound of the split-K scratch a conv of this shape can ask for (8 slices of [m_tiles*128][N] partials, capped at the
@@ -894,26 +827,21 @@ extern "C" int k2y_tc_plan_budget(int M, int N, int K, int ksize, int math_mode,
         set_error("k2y_tc_plan: bad arguments");
         return K2Y_ERR_INVALID;
     }
-    const bool gather = ksize == 3;
-    int mode = math_mode;
-    if (mode == K2Y_MATH_TC_BF16X3) {  // effective_mode(): same rules, expressed on (K, ksize)
-        const int cin = gather ? K / 9 : K;
-        if (!gather) mode = cin <= 32 ? K2Y_MATH_TC_3XTF32 : mode;
-        else if ((cin % 64) != 0 && cin != 32) mode = K2Y_MATH_TC_3XTF32;   // 32 channels: two taps per bf16 k-block
-    }
-    const bool bf = mode == K2Y_MATH_TC_BF16X3, three_x = mode != K2Y_MATH_TC_TF32;
-    const int nkb = bf ? (K + 63) / 64 : (K + BK - 1) / BK;
+    // the GEMM as a conv: M output pixels in one row, ksize x ksize taps over K / ksize^2 channels of one plain source
+    ConvArgs a{};
+    a.B = a.H = a.OH = 1;
+    a.W = a.OW = M;
+    a.kh = a.kw = ksize;
+    a.stride = 1;
+    a.C0 = K / (ksize * ksize);
+    a.N = N;
+    a.sm_limit = sm_limit;
+    const TcPlan pl = plan_conv(a, K, math_mode);
+    *bn = pl.bn;
+    *k_splits = pl.k_splits;
+    *stages = pl.stages;
     *cluster = 1;
-    const int sms = budget_sms(sm_limit);
-    pick_tile(M, N, nkb, three_x, bf, gather, 0, sms, bn, k_splits);
-    *stages = stages_for(*bn, three_x, bf);
-    const int kb_per_split = (nkb + *k_splits - 1) / *k_splits;
-    *k_splits = (nkb + kb_per_split - 1) / kb_per_split;
-    *effective_math = mode;
-    {
-        const int n16 = (N + 15) / 16 * 16, n_tiles = (n16 + *bn - 1) / *bn, m_tiles = (M + BM - 1) / BM;
-        const int items = m_tiles * n_tiles * *k_splits;
-        *grid = items < sms ? items : sms;
-    }
+    *effective_math = pl.mode;
+    *grid = pl.grid;
     return K2Y_OK;
 }

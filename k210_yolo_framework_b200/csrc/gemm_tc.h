@@ -21,9 +21,4 @@ size_t tc_scratch_bound(const ConvArgs &a, const TcWeights &w);           // spl
 int tc_launch_count(const ConvArgs &a, const TcWeights &w, int math_mode);  // kernels one launch_conv_tc issues
 cudaError_t launch_conv_tc(const ConvArgs &a, const TcWeights &w, int math_mode, cudaStream_t st);
 
-// Fused MobileNet block: depthwise 3x3 stride 1 + BN + act computed by the producer warps straight into the A stage of the
-// tensor-core kernel, then the 1x1 conv on the tensor cores — the depthwise output never reaches HBM.
-bool dwpw_supported(const DwArgs &dw, const ConvArgs &pw, const TcWeights &w, int math_mode);
-cudaError_t launch_dwpw_tc(const DwArgs &dw, const ConvArgs &pw, const TcWeights &w, cudaStream_t st);
-
 }  // namespace k2y

@@ -63,9 +63,6 @@ struct Layer {
     TcWeights tc2;
     float *d_scale2 = nullptr, *d_shift2 = nullptr;
     TcWeights tc;  // tensor-core packing (gemm_tc.cu)
-    float *d_dwpack = nullptr;  // depthwise layers: [11][cpad] taps + folded BN, zero-padded (DwArgs::pack)
-    int dw_cpad = 0;
-    int fused = 0;  // last issue_layers(): 1 = this depthwise ran fused with the next 1x1 conv, 2 = this conv ran inside the previous launch
 };
 
 }  // namespace
@@ -372,22 +369,12 @@ void plan_arena(k2y_net *n) {
                 top += need;
             }
         }
-        // release inputs whose last use is this layer.  A depthwise layer followed by the conv that reads its output may run
-        // fused with it (one kernel reads the depthwise input while it writes the conv output), so its inputs are released
-        // one layer later, after the conv's output has been placed.
-        const auto fusable_dw = [&](size_t j) {
-            return n->layers[j].kind == L_DW && j + 1 < n->layers.size() && n->layers[j + 1].src0 == n->layers[j].dst;
-        };
-        std::vector<std::pair<int, int>> release;  // (tensor, layer whose use ends it)
-        if (!fusable_dw(i))
-            for (int s : {L.src0, L.src1, L.res}) release.push_back({s, (int)i});
-        if (i > 0 && fusable_dw(i - 1))
-            for (int s : {n->layers[i - 1].src0, n->layers[i - 1].src1, n->layers[i - 1].res}) release.push_back({s, (int)i - 1});
-        for (const auto &rel : release) {
-            const int s = rel.first;
+        // release inputs whose last use is this layer (each layer is its own kernel, and every kernel waits for its
+        // predecessor to complete before it touches activations)
+        for (int s : {L.src0, L.src1, L.res}) {
             if (s < 0) continue;
             Tensor &t = T[s];
-            if (t.last_use == rel.second && !t.is_input && t.out_index < 0 && !n->keep_all) {
+            if (t.last_use == (int)i && !t.is_input && t.out_index < 0 && !n->keep_all) {
                 bool dup = false;
                 for (auto &fb : free_list) dup |= (fb.off == t.off);
                 if (dup) continue;
@@ -424,7 +411,6 @@ int check_net(const k2y_net *n, const char *fn) {
 }
 
 int issue_layers(k2y_net *n, int batch, cudaStream_t st, cudaEvent_t *ev = nullptr) {
-    int li = 0;
     n->launches = 0;
     if (ev) cudaEventRecord(ev[0], st);
     if (n->x_u8) {  // np.max(img) per image, consumed by the first conv's u8 -> f32 look-up table
@@ -470,7 +456,6 @@ int issue_layers(k2y_net *n, int batch, cudaStream_t st, cudaEvent_t *ev = nullp
         a.sm_limit = n->sm_limit;
         return a;
     };
-    int dw_ordinal = 0;
     // one NVTX range per layer (header-only NVTX 3: a no-op unless a tool is attached); under graph capture the ranges
     // bracket the capture-time issue of each node, in eager mode (k2y_net_set_use_graph(0), k2y_net_profile) the launches
     struct NvtxRange {
@@ -478,9 +463,8 @@ int issue_layers(k2y_net *n, int batch, cudaStream_t st, cudaEvent_t *ev = nullp
         ~NvtxRange() { nvtxRangePop(); }
     };
     for (size_t idx = 0; idx < n->layers.size(); ++idx) {
-        Layer &L = n->layers[idx];
+        const Layer &L = n->layers[idx];
         NvtxRange range(L.name.c_str());
-        L.fused = 0;
         const Tensor &s0 = n->tensors[L.src0];
         const Tensor &d = n->tensors[L.dst];
         cudaError_t e = cudaSuccess;
@@ -496,7 +480,7 @@ int issue_layers(k2y_net *n, int batch, cudaStream_t st, cudaEvent_t *ev = nullp
             }
             const long long Mrows = (long long)batch * d.h * d.w;
             ConvArgs pa = a;  // pixel-pair form (see Layer::tc2)
-            const bool pair = n->math != K2Y_MATH_FP32_SIMT && L.tc2.d_hi && L.d_scale2 && (Mrows % 2) == 0 && !getenv("K2Y_NO_PAIR");
+            const bool pair = n->math != K2Y_MATH_FP32_SIMT && L.tc2.d_hi && L.d_scale2 && (Mrows % 2) == 0;
             if (pair) {
                 pa.B = 1;
                 pa.H = pa.OH = 1;
@@ -534,42 +518,8 @@ int issue_layers(k2y_net *n, int batch, cudaStream_t st, cudaEvent_t *ev = nullp
             a.pad_l = L.pad_l;
             a.act = L.act;
             a.alpha = L.alpha;
-            a.pack = L.d_dwpack;
-            a.cpad = L.dw_cpad;
-            // depthwise + the following 1x1 conv as one tensor-core launch, the depthwise output goes straight into the GEMM's
-            // A stage (skipped when every layer output must be readable)
-            bool fused = false;
-            ++dw_ordinal;
-            if (!n->keep_all && n->math != K2Y_MATH_FP32_SIMT && idx + 1 < n->layers.size()) {
-                const Layer &P = n->layers[idx + 1];
-                const Tensor &dt = n->tensors[L.dst];
-                if (P.kind == L_CONV && P.src0 == L.dst && dt.last_use == (int)idx + 1 && dt.out_index < 0) {
-                    const ConvArgs pa = conv_args(P);
-                    // opt-in (K2Y_DWPW=1): stride-1 blocks run as ONE launch (dwpw_supported).  Off by default: the fused kernel
-                    // computes the depthwise layer in the GEMM's producer warpgroup, and cfg 2 ran 2.3x slower with it on an
-                    // H100 (9.8 k vs 22.8 k images/s).  K2Y_NO_DWPW=1 overrides K2Y_DWPW, K2Y_DWPW_MASK=<bitmask over the
-                    // depthwise layers in schedule order> restricts it.
-                    const char *no = getenv("K2Y_NO_DWPW"), *yes = getenv("K2Y_DWPW"), *mask = getenv("K2Y_DWPW_MASK");
-                    const bool on = yes && yes[0] == '1' && !(no && no[0] == '1');
-                    const bool allowed = on && (!mask || ((strtoul(mask, nullptr, 0) >> (dw_ordinal - 1)) & 1ul));
-                    if (allowed && dwpw_supported(a, pa, P.tc, n->math)) {
-                        e = launch_dwpw_tc(a, pa, P.tc, st);
-                        n->launches += 1;
-                        fused = true;
-                        if (e == cudaSuccess) {
-                            ++li;
-                            if (ev) cudaEventRecord(ev[li], st);
-                            L.fused = 1;
-                            n->layers[idx + 1].fused = 2;
-                            ++idx;  // the pointwise layer is done
-                        }
-                    }
-                }
-            }
-            if (!fused) {
-                e = launch_dwconv(a, st);
-                n->launches += 1;
-            }
+            e = launch_dwconv(a, st);
+            n->launches += 1;
         } else {
             PoolArgs a;
             a.src = tensor_ptr(n, L.src0);
@@ -588,8 +538,7 @@ int issue_layers(k2y_net *n, int batch, cudaStream_t st, cudaEvent_t *ev = nullp
             set_error("layer %s: launch failed: %s", L.name.c_str(), cudaGetErrorString(e));
             return K2Y_ERR_CUDA;
         }
-        ++li;
-        if (ev) cudaEventRecord(ev[li], st);
+        if (ev) cudaEventRecord(ev[idx + 1], st);
     }
     return K2Y_OK;
 }
@@ -664,8 +613,7 @@ extern "C" int k2y_net_destroy(k2y_net *net) {
         tc_free(L.tc2);
         cudaFree(L.d_scale2);
         cudaFree(L.d_shift2);
-        cudaFree(L.d_dwpack);
-        L.d_scale2 = L.d_shift2 = L.d_dwpack = nullptr;
+        L.d_scale2 = L.d_shift2 = nullptr;
     }
     delete net;
     return K2Y_OK;
@@ -799,20 +747,6 @@ extern "C" int k2y_net_finalize(k2y_net *net) {
         K2Y_CUDA_CHECK(cudaMemcpy(L.d_shift, shift.data(), L.cout * sizeof(float), cudaMemcpyHostToDevice));
         L.h_scale = scale;
         L.h_shift = shift;
-        if (L.kind == L_DW) {
-            const int C = L.cout, cpad = (C + 63) / 64 * 64;
-            std::vector<float> pack((size_t)11 * cpad, 0.f);
-            for (int c = 0; c < C; ++c) {
-                for (int t = 0; t < 9; ++t) pack[(size_t)t * cpad + c] = L.kernel[(size_t)t * C + c];
-                pack[(size_t)9 * cpad + c] = scale[c];
-                pack[(size_t)10 * cpad + c] = shift[c];
-            }
-            cudaFree(L.d_dwpack);
-            L.d_dwpack = nullptr;
-            K2Y_CUDA_CHECK(cudaMalloc(&L.d_dwpack, pack.size() * sizeof(float)));
-            K2Y_CUDA_CHECK(cudaMemcpy(L.d_dwpack, pack.data(), pack.size() * sizeof(float), cudaMemcpyHostToDevice));
-            L.dw_cpad = cpad;
-        }
         if (L.kind == L_CONV) {
             int rc = tc_pack(L.tc, L.kernel.data(), L.kh * L.kw * L.cin, L.cout);
             if (rc != K2Y_OK) return rc;
@@ -1163,18 +1097,7 @@ extern "C" int k2y_net_launch_info(const k2y_net *net, int i, char *name, int na
     double macs = 0;
     if (L.kind == L_CONV) macs = out_elems * L.kh * L.kw * L.cin;
     else if (L.kind == L_DW) macs = out_elems * 9;
-    double bytes = 4.0 * (in_elems + out_elems);  // algorithmic: activations read once + written once
-    if (L.fused == 1) {  // depthwise + next 1x1 in one launch: reads the depthwise input, writes the pointwise output
-        const Layer &P = net->layers[i + 1];
-        const Tensor &pd = net->tensors[P.dst];
-        const double p_out = (double)pd.h * pd.w * pd.c;
-        if (name && name_len > 0) snprintf(name, name_len, "%s+%s", L.name.c_str(), P.name.c_str());
-        macs += p_out * P.cin;
-        bytes = 4.0 * (in_elems + p_out);
-    } else if (L.fused == 2) {  // ran inside the previous launch
-        macs = 0;
-        bytes = 0;
-    }
+    const double bytes = 4.0 * (in_elems + out_elems);  // algorithmic: activations read once + written once
     if (flops_per_image) *flops_per_image = 2.0 * macs;
     if (bytes_per_image) *bytes_per_image = bytes;
     return K2Y_OK;

@@ -61,9 +61,6 @@ __device__ __forceinline__ void cp_async_16(uint32_t dst, const void *src, uint3
 __device__ __forceinline__ void cp_async_mbar_arrive_noinc(uint32_t bar) {
     asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
 __device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
     float v;
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");

@@ -61,7 +61,8 @@ def test_mobilev1_real_weights_layerwise(golden_weights, dog_u8, dog_heads, math
 
 CASES = [("yolo_mobilev1", 0.75, 20, (224, 320), 3), ("yolo_mobilev1", 1.0, 20, (96, 128), 2),
          ("yolo_mobilev2", 1.0, 20, (224, 320), 2), ("yolo_mobilev2", 0.5, 20, (96, 96), 2),
-         ("tiny_yolo", 1.0, 20, (160, 160), 2), ("yolo", 1.0, 80, (96, 96), 2)]
+         ("tiny_yolo", 1.0, 20, (160, 160), 2), ("yolo", 1.0, 80, (96, 96), 2),
+         ("yolo_mobilev1", 0.5, 20, (96, 160), 2)]   # partial tiles on the 48x80 ... 6x10 maps, C = 16..512
 
 
 @pytest.mark.parametrize("math", MODES)
@@ -111,59 +112,6 @@ def test_device_api_graph_replay_and_batching():
     for p, q in zip(a, host):
         np.testing.assert_array_equal(p.cpu().numpy(), q)
     assert m.engine.launches_per_run() >= 32   # + split-K reducers
-
-
-def test_fused_depthwise_pointwise_blocks(monkeypatch):
-    """K2Y_DWPW=1: every stride-1 MobileNet block (depthwise 3x3 + 1x1) is ONE launch of the tensor-core kernel — the
-    depthwise result is computed straight into the GEMM's shared-memory A stage.  Same heads as the unfused schedule
-    (K2Y_NO_DWPW=1), fewer launches, and the oracle on extents where tiles are partial."""
-    monkeypatch.setenv("K2Y_DWPW", "1")
-    monkeypatch.delenv("K2Y_NO_DWPW", raising=False)
-    m, _ = yolonet.yolo_mobilev1([224, 320, 3], 3, 20, alpha=0.75, max_batch=3)
-    weights = random_weights(m.engine.expected_variables(), seed=9, detection_rich=True)
-    m.set_weights_dict(weights)
-    m.engine.set_use_graph(False)
-    x = torch.rand((3, 224, 320, 3), device="cuda")
-    fused = [t.clone() for t in m.predict_device(x)]
-    n_fused = m.engine.launches_per_run()
-    names = [p["name"] for p in m.engine.profile(3)]
-    for blk in (1, 3, 5, 7, 8, 9, 10, 11):
-        assert f"conv_dw_{blk}+conv_pw_{blk}" in names, names
-    monkeypatch.setenv("K2Y_NO_DWPW", "1")
-    monkeypatch.setenv("K2Y_DWPW", "0")
-    plain = [t.clone() for t in m.predict_device(x)]
-    assert m.engine.launches_per_run() == n_fused + 8
-    assert not any("+" in p["name"] for p in m.engine.profile(3))
-    monkeypatch.delenv("K2Y_NO_DWPW")
-    monkeypatch.setenv("K2Y_DWPW", "1")
-    for p, q in zip(fused, plain):
-        assert torch.allclose(p, q, atol=3e-4, rtol=1e-4), float((p - q).abs().max())
-    # one block at a time (K2Y_DWPW_MASK selects depthwise layers by schedule order): localises a failure to a layer shape
-    for blk in (1, 3, 5, 7):
-        monkeypatch.setenv("K2Y_DWPW_MASK", hex(1 << (blk - 1)))
-        one = m.predict_device(x)
-        assert m.engine.launches_per_run() == n_fused + 7
-        for p, q in zip(one, plain):
-            assert torch.allclose(p, q, atol=3e-4, rtol=1e-4), (blk, float((p - q).abs().max()))
-    monkeypatch.delenv("K2Y_DWPW_MASK")
-    # the default schedule fuses no block (the fused launch is slower than the pair on an H100)
-    monkeypatch.delenv("K2Y_DWPW")
-    m.predict_device(x)
-    dflt = [p["name"] for p in m.engine.profile(3) if "+" in p["name"]]
-    assert dflt == [], dflt
-    assert m.engine.launches_per_run() == n_fused + 8
-    monkeypatch.setenv("K2Y_DWPW", "1")
-    # against the oracle, on extents where tiles are partial (96x160 -> 48x80, 24x40, 12x20, 6x10 maps) and C = 16..512
-    for alpha, hw in ((0.5, (96, 160)), (1.0, (64, 96))):
-        m2, _ = yolonet.yolo_mobilev1([hw[0], hw[1], 3], 3, 20, alpha=alpha, max_batch=2)
-        w2 = random_weights(m2.engine.expected_variables(), seed=10, detection_rich=True)
-        m2.set_weights_dict(w2)
-        x2 = np.random.default_rng(3).random((2, hw[0], hw[1], 3), dtype=np.float32)
-        got = m2.predict(x2)
-        assert any("+" in p["name"] for p in m2.engine.profile(2))
-        ref = keras_ref.forward("yolo_mobilev1", w2, x2.astype(np.float64), alpha=alpha, dtype=torch.float64)
-        for g, r in zip(got, ref):
-            assert _maxerr(g, r) / max(1.0, float(np.abs(r).max())) < LAYER_TOL[_lib.MATH_TC_BF16X3]
 
 
 def test_predict_after_uint8_input_uses_the_float_input():
