@@ -11,8 +11,10 @@
 //   warpgroups 1-2  consumers  64 rows each: read their A rows from shared memory into the wgmma A register fragment,
 //                            split them into hi/lo planes (3xTF32: hi = tf32(a), lo = tf32(a - hi); bf16x3: hi = bf16(a),
 //                            mid = bf16(a - hi); the weights were split on the host), so that lo*hi + hi*lo + hi*hi
-//                            recovers fp32-class accuracy from the tensor cores; B comes from shared memory.  After the
-//                            last k-block of a tile they apply folded BN, activation and residual and store to HBM.
+//                            recovers fp32-class accuracy from the tensor cores; B comes from shared memory.  A k-block's
+//                            MMAs are one committed wgmma group; while it runs, the next k-block's A is read and split
+//                            into a second fragment buffer, and a stage is released once its group has completed.  After
+//                            the last k-block of a tile they apply folded BN, activation and residual and store to HBM.
 // mbarrier ring per stage: full_b (TMA tx) / full_a (cp.async arrivals) -> [consumers] -> empty.
 //
 // Replaces the TF Conv2D + FusedBatchNorm + LeakyRelu/Relu6 (+ ResizeNearestNeighbor/ConcatV2/Add) ops that
@@ -53,9 +55,6 @@ struct TcParams {
     int BN, n_tiles, m_tiles, nkb, stages;
     int k_splits, kb_per_split;     // split-K: work item = (m-tile, n-tile, k-slice); partials go to a scratch buffer
     int partial;                    // 1: raw accumulators to dst (split-K scratch, row pitch N, rows of slice ks at ks * m_tiles * 128)
-    int three_x;                    // 1 = split scheme (3 MMAs per k-step: lo*hi + hi*lo + hi*hi), 0 = single tf32 pass
-    int bf16;                       // 1 = bf16x3: operands are bf16 (hi, mid) planes, 64 k per k-block; 0 = tf32, 32 k per k-block
-    int a_boxes;                    // 16 KB sub-tiles of raw fp32 A per stage (k per k-block / 32)
     int half_taps;                  // gather: Cin is half a k-block (16 with tf32, 32 with bf16 k-blocks), a k-block holds TWO consecutive taps
     float act_slope, act_clamp;     // branch-free activation parameters
 };
@@ -71,19 +70,83 @@ __device__ __forceinline__ uint32_t a_addr(uint32_t box, int r, int k) {
     return box + (uint32_t)r * 128u + ((uint32_t)((k >> 2) ^ (r & 7)) << 4) + (uint32_t)(k & 3) * 4u;
 }
 
-// BNT = the tile width p.BN, a compile-time constant so that every accumulator register and every wgmma of the consumers is
-// fixed at compile time (a runtime-sliced accumulator made ptxas serialise the wgmma pipeline)
-template <bool GATHER, int BNT>
+// Register budget of the warp-specialised kernel: the consumers, which hold the accumulators and two k-blocks of A fragments,
+// rise to CONSUMER_REGS (the least with no spills in every instantiation) and the producers give up the difference
+// (128 x 152 + 256 x 176 = 384 x 168, the launch's share).  The gather producers run measurably slower at smaller budgets.
+constexpr int PRODUCER_REGS = 152;
+constexpr int CONSUMER_REGS = 176;
+
+template <int I>
+struct Buf {
+    static constexpr int value = I;
+};
+
+// The MMAs of one k-block for one consumer warpgroup, NKS k-steps of it (the rest of the k-block is K padding), as one batch:
+// a fence, the wgmmas, one commit.  Per k-step and tile column the split schemes issue lo*hi, hi*lo, hi*hi.
+template <int MODE, int BNT, int NKS>
+__device__ __forceinline__ void mma_ksteps(float (&acc)[BNT / 2], const uint32_t (&ahi)[4][4], const uint32_t (&alo)[4][4],
+                                           uint64_t dhi, uint64_t dlo, uint32_t accumulate) {
+    constexpr int nb64 = BNT / 64;  // 64-column MMAs first, then 16-column ones for the rest
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < NKS; ++kk) {
+        const uint64_t adv = (uint64_t)((kk * 32) >> 4);  // 32 bytes of B per k-step inside the 128 B swizzle row
+        const uint32_t first = kk == 0 ? accumulate : 1u;
+#pragma unroll
+        for (int j = 0; j < nb64; ++j) {
+            const uint64_t o = adv + (uint64_t)((j * 64 * 128) >> 4);
+            float *d = acc + j * 32;
+            if constexpr (MODE == K2Y_MATH_TC_BF16X3) {
+                wgmma_bf16_n64(d, alo[kk], dhi + o, first);
+                wgmma_bf16_n64(d, ahi[kk], dlo + o, 1u);
+                wgmma_bf16_n64(d, ahi[kk], dhi + o, 1u);
+            } else if constexpr (MODE == K2Y_MATH_TC_3XTF32) {
+                wgmma_tf32_n64(d, alo[kk], dhi + o, first);
+                wgmma_tf32_n64(d, ahi[kk], dlo + o, 1u);
+                wgmma_tf32_n64(d, ahi[kk], dhi + o, 1u);
+            } else {
+                wgmma_tf32_n64(d, ahi[kk], dhi + o, first);
+            }
+        }
+#pragma unroll
+        for (int j = nb64 * 4; j < BNT / 16; ++j) {
+            const uint64_t o = adv + (uint64_t)((j * 16 * 128) >> 4);
+            float *d = acc + j * 8;
+            if constexpr (MODE == K2Y_MATH_TC_BF16X3) {
+                wgmma_bf16_n16(d, alo[kk], dhi + o, first);
+                wgmma_bf16_n16(d, ahi[kk], dlo + o, 1u);
+                wgmma_bf16_n16(d, ahi[kk], dhi + o, 1u);
+            } else if constexpr (MODE == K2Y_MATH_TC_3XTF32) {
+                wgmma_tf32_n16(d, alo[kk], dhi + o, first);
+                wgmma_tf32_n16(d, ahi[kk], dlo + o, 1u);
+                wgmma_tf32_n16(d, ahi[kk], dhi + o, 1u);
+            } else {
+                wgmma_tf32_n16(d, ahi[kk], dhi + o, first);
+            }
+        }
+    }
+    wgmma_commit();
+}
+
+// BNT = the tile width p.BN and MODE = the math mode (K2Y_MATH_TC_*), compile-time constants so that every accumulator
+// register and every wgmma of the consumers is fixed at compile time and a k-block's MMAs are one branch-free batch (a
+// runtime-sliced accumulator made ptxas serialise the wgmma pipeline; a runtime mode test split the batch into groups)
+template <bool GATHER, int BNT, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_bhi,
                const __grid_constant__ CUtensorMap map_blo, const TcParams p) {
+    constexpr bool BF16 = MODE == K2Y_MATH_TC_BF16X3;       // operands are bf16 (hi, mid) planes, 64 k per k-block
+    constexpr bool THREE_X = MODE != K2Y_MATH_TC_TF32;      // split scheme: 3 MMAs per k-step; else one tf32 pass, 32 k per k-block
+    constexpr int A_BOXES = BF16 ? 2 : 1;                   // 16 KB sub-tiles of raw fp32 A per stage
+    constexpr int KBK = A_BOXES * BK;                       // k values per k-block
+    constexpr int KSTEP = BF16 ? 16 : 8;                    // k values per wgmma
+    static_assert(KBK / KSTEP == 4, "a k-block is four k-steps");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [stages] x { A (raw fp32) a_boxes x 16K | B_hi BN*128 | B_lo BN*128 (3x) }, then barriers
+    // carve: [stages] x { A (raw fp32) A_BOXES x 16K | B_hi BN*128 | B_lo BN*128 (3x) }, then barriers
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t b_bytes = (uint32_t)p.BN * 128u;
-    const uint32_t a_bytes = (uint32_t)A_TILE_BYTES * (uint32_t)p.a_boxes;
-    const uint32_t stage_bytes = a_bytes + b_bytes * (p.three_x ? 2u : 1u);
-    const int KBK = p.a_boxes * BK;  // k values per k-block
+    const uint32_t a_bytes = (uint32_t)A_TILE_BYTES * (uint32_t)A_BOXES;
+    const uint32_t stage_bytes = a_bytes + b_bytes * (THREE_X ? 2u : 1u);
     uint8_t *smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
     Barriers *bars = reinterpret_cast<Barriers *>(smem_gen + (size_t)p.stages * stage_bytes);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -98,7 +161,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         fence_barrier_init();
         if (!GATHER) prefetch_tmap(&map_a);
         prefetch_tmap(&map_bhi);
-        if (p.three_x) prefetch_tmap(&map_blo);
+        if (THREE_X) prefetch_tmap(&map_blo);
     }
     __syncthreads();
     pdl_wait();  // barrier set-up and descriptor prefetch overlap the previous kernel's tail; activations do not
@@ -110,11 +173,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 
     if (warp < 4) {
         // ================= producers =================
+        setmaxnreg_dec<PRODUCER_REGS>();
         const int r = threadIdx.x;  // GEMM row inside the tile (gather), or producer thread index
         int s = 0;
         uint32_t ph = 0;
-        const uint32_t tx = b_bytes * (p.three_x ? 2u : 1u) + (GATHER ? 0u : a_bytes);
-        const int bk_elems = p.bf16 ? 64 : 32;  // k-block extent in elements of the weight map (bf16 or fp32)
+        const uint32_t tx = b_bytes * (THREE_X ? 2u : 1u) + (GATHER ? 0u : a_bytes);
+        constexpr int bk_elems = BF16 ? 64 : 32;  // k-block extent in elements of the weight map (bf16 or fp32)
         if (!GATHER && warp != 0) return;
         const int Cin = p.C0 + p.C1;
         const int wrow0 = warp * 32;  // first tile row of this warp
@@ -139,11 +203,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         const uint32_t fb = smem_u32(&bars->full_b[s]);
                         mbar_arrive_expect_tx(fb, tx);
                         if (!GATHER) {
-                            for (int bx = 0; bx < p.a_boxes; ++bx)
+                            for (int bx = 0; bx < A_BOXES; ++bx)
                                 tma_load_2d(stage_a(s) + (uint32_t)bx * A_TILE_BYTES, &map_a, fb, kb * KBK + bx * BK, mt * BM);
                         }
                         tma_load_2d(stage_b_hi(s), &map_bhi, fb, kb * bk_elems, nt * p.BN);
-                        if (p.three_x) tma_load_2d(stage_b_lo(s), &map_blo, fb, kb * bk_elems, nt * p.BN);
+                        if (THREE_X) tma_load_2d(stage_b_lo(s), &map_blo, fb, kb * bk_elems, nt * p.BN);
                     }
                     __syncwarp();
                 }
@@ -185,7 +249,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                         pr = (unsigned long long)src;
                     }
                     const uint32_t stg_a = stage_a(s);
-                    if (p.a_boxes == 2) {
+                    if constexpr (A_BOXES == 2) {
                         const int cjj = lane & 15;
                         const uint32_t dcol = (uint32_t)(cjj >> 3) * A_TILE_BYTES;
 #pragma unroll
@@ -227,13 +291,57 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     }
 
     // ================= consumers: warpgroup cg owns tile rows [64 cg, 64 cg + 64) =================
+    setmaxnreg_inc<CONSUMER_REGS>();
     const int cw = warp - 4;                 // 0..7
     const int cg = cw >> 2, wq = cw & 3;     // warpgroup, warp inside it
     const int g = lane >> 2, tq = lane & 3;  // fragment row / column group
     const int r0 = cg * 64 + wq * 16 + g;    // this thread's two tile rows: r0, r0 + 8
-    constexpr int nb64 = BNT / 64;              // 64-column MMAs first, then 16-column ones for the rest
     int s = 0;
     uint32_t ph = 0;
+    // A fragments of two k-blocks (4 k-steps x 4 registers, hi and lo planes): the MMAs of one k-block read their buffer
+    // while the next k-block's A is read from shared memory and split into the other
+    uint32_t ahi[2][4][4], alo[2][4][4];
+    // wait for stage s, read this thread's A elements of it and split them into the (hi, lo) planes
+    auto load_a = [&](uint32_t (&hi)[4][4], uint32_t (&lo)[4][4]) {
+        mbar_wait(smem_u32(&bars->full_b[s]), ph);
+        if (GATHER) mbar_wait(smem_u32(&bars->full_a[s]), ph);
+        const uint32_t sa = stage_a(s);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            if constexpr (BF16) {
+                // k-step kk = 16 bf16 columns: sub-tile kk/2, columns (kk&1)*16 + {2tq, 2tq+1} and + 8
+                float v[4][2];  // fragment element j: row r0 + 8*(j&1), columns (lo, hi) of the pair
+                const uint32_t box = sa + (uint32_t)(kk >> 1) * A_TILE_BYTES;
+                const int c0 = (kk & 1) * 16 + 2 * tq;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int row = r0 + 8 * (j & 1), col = c0 + 8 * (j >> 1);
+                    const float2 x = ld_shared_v2(a_addr(box, row, col));
+                    v[j][0] = x.x;
+                    v[j][1] = x.y;
+                }
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const uint32_t h = pack_bf16x2(v[j][0], v[j][1]);
+                    hi[kk][j] = h;
+                    lo[kk][j] = pack_bf16x2(v[j][0] - __uint_as_float(h << 16), v[j][1] - __uint_as_float(h & 0xffff0000u));
+                }
+            } else {
+                // k-step kk = 8 tf32 columns: (row r0 / r0+8) x (column 8kk + tq / 8kk + tq + 4)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float x = ld_shared_f32(a_addr(sa, r0 + 8 * (j & 1), kk * 8 + tq + 4 * (j >> 1)));
+                    const float h = to_tf32_rna(x);
+                    hi[kk][j] = __float_as_uint(THREE_X ? h : x);
+                    if (THREE_X) lo[kk][j] = __float_as_uint(to_tf32_rna(x - h));
+                }
+            }
+        }
+    };
+    auto release = [&](int stage) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&bars->empty[stage]));
+    };
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const int ks = t % p.k_splits, tt = t / p.k_splits;
         const int mt = tt / p.n_tiles, nt = tt - mt * p.n_tiles;
@@ -241,119 +349,73 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         float acc[BNT / 2];
 #pragma unroll
         for (int i = 0; i < BNT / 2; ++i) acc[i] = 0.f;
-        for (int kb = kb0; kb < kb1; ++kb) {
-            mbar_wait(smem_u32(&bars->full_b[s]), ph);
-            if (GATHER) mbar_wait(smem_u32(&bars->full_a[s]), ph);
-            const uint32_t sa = stage_a(s);
-            uint32_t ahi[4][4], alo[4][4];
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                float v[4][2];  // fragment element j: row r0 + 8*(j&1), columns (lo, hi) of the pair / the tf32 column
-                if (p.bf16) {
-                    // k-step kk = 16 bf16 columns: sub-tile kk/2, columns (kk&1)*16 + {2tq, 2tq+1} and + 8
-                    const uint32_t box = sa + (uint32_t)(kk >> 1) * A_TILE_BYTES;
-                    const int c0 = (kk & 1) * 16 + 2 * tq;
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const int row = r0 + 8 * (j & 1), col = c0 + 8 * (j >> 1);
-                        const float2 x = ld_shared_v2(a_addr(box, row, col));
-                        v[j][0] = x.x;
-                        v[j][1] = x.y;
-                    }
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const uint32_t h = pack_bf16x2(v[j][0], v[j][1]);
-                        ahi[kk][j] = h;
-                        alo[kk][j] = pack_bf16x2(v[j][0] - __uint_as_float(h << 16), v[j][1] - __uint_as_float(h & 0xffff0000u));
-                    }
-                } else {
-                    // k-step kk = 8 tf32 columns: (row r0 / r0+8) x (column 8kk + tq / 8kk + tq + 4)
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float x = ld_shared_f32(a_addr(sa, r0 + 8 * (j & 1), kk * 8 + tq + 4 * (j >> 1)));
-                        const float h = to_tf32_rna(x);
-                        ahi[kk][j] = __float_as_uint(p.three_x ? h : x);
-                        alo[kk][j] = __float_as_uint(to_tf32_rna(x - h));
-                    }
-                }
-            }
+        load_a(ahi[0], alo[0]);
+        int kb = kb0, prev = 0;
+        // k-block kb from fragment buffer B: issue its MMAs, retire the previous k-block's (freeing its stage and the other
+        // buffer), then load the next k-block into the other buffer while these run.  false after the tile's last k-block.
+        auto kblock = [&](auto buf) -> bool {
+            constexpr int B = decltype(buf)::value;
             const uint64_t dhi = make_desc_sw128(stage_b_hi(s)), dlo = make_desc_sw128(stage_b_lo(s));
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                const uint64_t adv = (uint64_t)((kk * 32) >> 4);  // 32 bytes of B per k-step inside the 128 B swizzle row
-                const uint32_t first = ((kb - kb0) | kk) == 0 ? 0u : 1u;
-#pragma unroll
-                for (int j = 0; j < BNT / 64; ++j) {
-                    if (j >= nb64) continue;
-                    const uint64_t o = adv + (uint64_t)((j * 64 * 128) >> 4);
-                    float *d = acc + j * 32;
-                    if (p.bf16) {
-                        wgmma_bf16_n64(d, alo[kk], dhi + o, first);
-                        wgmma_bf16_n64(d, ahi[kk], dlo + o, 1u);
-                        wgmma_bf16_n64(d, ahi[kk], dhi + o, 1u);
-                    } else if (p.three_x) {
-                        wgmma_tf32_n64(d, alo[kk], dhi + o, first);
-                        wgmma_tf32_n64(d, ahi[kk], dlo + o, 1u);
-                        wgmma_tf32_n64(d, ahi[kk], dhi + o, 1u);
-                    } else {
-                        wgmma_tf32_n64(d, ahi[kk], dhi + o, first);
-                    }
-                }
-#pragma unroll
-                for (int j = 0; j < BNT / 16; ++j) {
-                    if (j < nb64 * 4 || j * 16 >= BNT) continue;
-                    const uint64_t o = adv + (uint64_t)((j * 16 * 128) >> 4);
-                    float *d = acc + j * 8;
-                    if (p.bf16) {
-                        wgmma_bf16_n16(d, alo[kk], dhi + o, first);
-                        wgmma_bf16_n16(d, ahi[kk], dlo + o, 1u);
-                        wgmma_bf16_n16(d, ahi[kk], dhi + o, 1u);
-                    } else if (p.three_x) {
-                        wgmma_tf32_n16(d, alo[kk], dhi + o, first);
-                        wgmma_tf32_n16(d, ahi[kk], dlo + o, 1u);
-                        wgmma_tf32_n16(d, ahi[kk], dhi + o, 1u);
-                    } else {
-                        wgmma_tf32_n16(d, ahi[kk], dhi + o, first);
-                    }
-                }
-            }
-            wgmma_commit();
-            wgmma_wait_all();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&bars->empty[s]));
+            const uint32_t accumulate = kb == kb0 ? 0u : 1u;
+            // only the k-steps that hold real K: past it A and B are zero-filled
+            const int k_left = p.K - kb * KBK;
+            if (k_left > 3 * KSTEP) mma_ksteps<MODE, BNT, 4>(acc, ahi[B], alo[B], dhi, dlo, accumulate);
+            else if (k_left > 2 * KSTEP) mma_ksteps<MODE, BNT, 3>(acc, ahi[B], alo[B], dhi, dlo, accumulate);
+            else if (k_left > KSTEP) mma_ksteps<MODE, BNT, 2>(acc, ahi[B], alo[B], dhi, dlo, accumulate);
+            else mma_ksteps<MODE, BNT, 1>(acc, ahi[B], alo[B], dhi, dlo, accumulate);
+            wgmma_wait<1>();
+            if (kb > kb0) release(prev);
+            prev = s;
             if (++s == p.stages) {
                 s = 0;
                 ph ^= 1u;
             }
+            if (++kb < kb1) {
+                load_a(ahi[B ^ 1], alo[B ^ 1]);
+                return true;
+            }
+            wgmma_wait<0>();
+            release(prev);
+            return false;
+        };
+        while (kblock(Buf<0>{}) && kblock(Buf<1>{})) {
         }
+#pragma unroll
+        for (int i = 0; i < BNT / 2; ++i) reg_fence(acc[i]);
         // ---- epilogue: folded BN + activation (+ residual) straight from the accumulator registers ----
         const int n_base = nt * BNT + 2 * tq;
+        if (p.partial) {
+            // split-K partial of slice ks: raw sums, rows [ks * m_tiles * 128, ...) of the scratch tensor (N % 4 == 0)
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int mloc = mt * BM + r0 + 8 * h;
-            if (p.partial) {
-                // split-K partial of slice ks: raw sums, rows [ks * m_tiles * 128, ...) of the scratch tensor (N % 4 == 0)
-                float *out = p.dst + ((size_t)ks * p.m_tiles * BM + mloc) * p.N;
+            for (int h = 0; h < 2; ++h) {
+                float *out = p.dst + ((size_t)ks * p.m_tiles * BM + mt * BM + r0 + 8 * h) * p.N;
 #pragma unroll
                 for (int c = 0; c < BNT / 8; ++c) {
                     const int n = n_base + 8 * c;
-                    if (c * 8 >= BNT || n >= p.N) continue;
+                    if (n >= p.N) continue;
                     *reinterpret_cast<float2 *>(out + n) = make_float2(acc[4 * c + 2 * h], acc[4 * c + 2 * h + 1]);
                 }
-                continue;
             }
-            if (mloc >= p.M) continue;
-            float *out = p.dst + (size_t)mloc * p.N;
-            const float *res = p.residual ? p.residual + (size_t)mloc * p.N : nullptr;
-            const bool vec = (p.N & 1) == 0;
+            continue;
+        }
+        const bool vec = (p.N & 1) == 0;
 #pragma unroll
-            for (int c = 0; c < BNT / 8; ++c) {
-                const int n = n_base + 8 * c;
-                if (c * 8 >= BNT || n >= p.N) continue;
-                float o0 = act_bf(fmaf(acc[4 * c + 2 * h], __ldg(p.scale + n), __ldg(p.shift + n)), p.act_slope, p.act_clamp);
+        for (int c = 0; c < BNT / 8; ++c) {
+            const int n = n_base + 8 * c;
+            if (n >= p.N) continue;
+            // the column pair's BN constants, once for both row halves (n + 1 < N whenever N is even)
+            const bool two = n + 1 < p.N;
+            const float sc0 = __ldg(p.scale + n), sh0 = __ldg(p.shift + n);
+            const float sc1 = two ? __ldg(p.scale + n + 1) : 0.f, sh1 = two ? __ldg(p.shift + n + 1) : 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int mloc = mt * BM + r0 + 8 * h;
+                if (mloc >= p.M) continue;
+                float *out = p.dst + (size_t)mloc * p.N;
+                const float *res = p.residual ? p.residual + (size_t)mloc * p.N : nullptr;
+                float o0 = act_bf(fmaf(acc[4 * c + 2 * h], sc0, sh0), p.act_slope, p.act_clamp);
                 if (vec) {
-                    float o1 = act_bf(fmaf(acc[4 * c + 2 * h + 1], __ldg(p.scale + n + 1), __ldg(p.shift + n + 1)), p.act_slope, p.act_clamp);
+                    float o1 = act_bf(fmaf(acc[4 * c + 2 * h + 1], sc1, sh1), p.act_slope, p.act_clamp);
                     if (res) {
                         const float2 rr = __ldg(reinterpret_cast<const float2 *>(res + n));
                         o0 += rr.x, o1 += rr.y;
@@ -362,8 +424,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 } else {
                     if (res) o0 += __ldg(res + n);
                     out[n] = o0;
-                    if (n + 1 < p.N) {
-                        float o1 = act_bf(fmaf(acc[4 * c + 2 * h + 1], __ldg(p.scale + n + 1), __ldg(p.shift + n + 1)), p.act_slope, p.act_clamp);
+                    if (two) {
+                        float o1 = act_bf(fmaf(acc[4 * c + 2 * h + 1], sc1, sh1), p.act_slope, p.act_clamp);
                         if (res) o1 += __ldg(res + n + 1);
                         out[n + 1] = o1;
                     }
@@ -554,24 +616,34 @@ void pick_tile(int M, int N, int nkb, bool three_x, bool bf16, bool gather, size
     *splits_out = best_s;
 }
 
-template <bool G>
-using ConvKernel = decltype(&conv_tc_kernel<G, 16>);
+using ConvKernel = decltype(&conv_tc_kernel<false, 16, K2Y_MATH_TC_TF32>);
 
 // the instantiation for tile width bn (a multiple of 16 up to MAX_BN)
-template <bool G>
-ConvKernel<G> conv_kernel_for(int bn) {
+template <bool G, int MODE>
+ConvKernel conv_kernel_bn(int bn) {
     switch (bn) {
-        case 16: return conv_tc_kernel<G, 16>;
-        case 32: return conv_tc_kernel<G, 32>;
-        case 48: return conv_tc_kernel<G, 48>;
-        case 64: return conv_tc_kernel<G, 64>;
-        case 80: return conv_tc_kernel<G, 80>;
-        case 96: return conv_tc_kernel<G, 96>;
-        case 112: return conv_tc_kernel<G, 112>;
-        case 128: return conv_tc_kernel<G, 128>;
+        case 16: return conv_tc_kernel<G, 16, MODE>;
+        case 32: return conv_tc_kernel<G, 32, MODE>;
+        case 48: return conv_tc_kernel<G, 48, MODE>;
+        case 64: return conv_tc_kernel<G, 64, MODE>;
+        case 80: return conv_tc_kernel<G, 80, MODE>;
+        case 96: return conv_tc_kernel<G, 96, MODE>;
+        case 112: return conv_tc_kernel<G, 112, MODE>;
+        case 128: return conv_tc_kernel<G, 128, MODE>;
         default: return nullptr;
     }
 }
+// the instantiation for a gather / TMA A operand, a tensor-core math mode (K2Y_MATH_TC_*) and tile width bn
+template <bool G>
+ConvKernel conv_kernel_for(int mode, int bn) {
+    switch (mode) {
+        case K2Y_MATH_TC_TF32: return conv_kernel_bn<G, K2Y_MATH_TC_TF32>(bn);
+        case K2Y_MATH_TC_3XTF32: return conv_kernel_bn<G, K2Y_MATH_TC_3XTF32>(bn);
+        case K2Y_MATH_TC_BF16X3: return conv_kernel_bn<G, K2Y_MATH_TC_BF16X3>(bn);
+        default: return nullptr;
+    }
+}
+constexpr int TC_MODES[] = {K2Y_MATH_TC_TF32, K2Y_MATH_TC_3XTF32, K2Y_MATH_TC_BF16X3};
 
 int tc_init() {
     int dev = 0;
@@ -584,12 +656,13 @@ int tc_init() {
     if (ds.init) return K2Y_OK;
     cudaDeviceProp prop;
     K2Y_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
-    for (int bn = 16; bn <= MAX_BN; bn += 16) {
-        K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<false>(bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)prop.sharedMemPerBlockOptin));
-        K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<true>(bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                            (int)prop.sharedMemPerBlockOptin));
-    }
+    for (int mode : TC_MODES)
+        for (int bn = 16; bn <= MAX_BN; bn += 16) {
+            K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<false>(mode, bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                (int)prop.sharedMemPerBlockOptin));
+            K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<true>(mode, bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                (int)prop.sharedMemPerBlockOptin));
+        }
     if (g_num_sms == 0) {
         g_max_smem = prop.sharedMemPerBlockOptin;
         g_num_sms = prop.multiProcessorCount;
@@ -734,10 +807,8 @@ cudaError_t launch_conv_tc(const ConvArgs &a, const TcWeights &w, int math_mode,
     p.N = a.N;
     p.K = w.K;
     const TcPlan pl = plan_conv(a, w.K, math_mode);
-    p.bf16 = (pl.mode == K2Y_MATH_TC_BF16X3) ? 1 : 0;
-    p.three_x = (pl.mode == K2Y_MATH_TC_TF32) ? 0 : 1;
-    p.a_boxes = p.bf16 ? 2 : 1;
-    p.half_taps = is_half_taps(a, p.bf16 ? 32 : 16) ? 1 : 0;
+    const bool bf16 = pl.mode == K2Y_MATH_TC_BF16X3, three_x = pl.mode != K2Y_MATH_TC_TF32;
+    p.half_taps = is_half_taps(a, bf16 ? 32 : 16) ? 1 : 0;
     p.nkb = pl.nkb;
     p.BN = pl.bn;
     p.n_tiles = pl.n_tiles;
@@ -746,7 +817,7 @@ cudaError_t launch_conv_tc(const ConvArgs &a, const TcWeights &w, int math_mode,
     p.k_splits = pl.k_splits;
     p.stages = pl.stages;
     if (p.stages < 2) return cudaErrorInvalidConfiguration;
-    const size_t smem = FIXED_SMEM + (size_t)p.stages * stage_bytes_of(p.BN, p.three_x != 0, p.bf16 != 0);
+    const size_t smem = FIXED_SMEM + (size_t)p.stages * stage_bytes_of(p.BN, three_x, bf16);
 
     CUtensorMap map_a, map_bhi, map_blo;
     memset(&map_a, 0, sizeof(map_a));
@@ -767,7 +838,7 @@ cudaError_t launch_conv_tc(const ConvArgs &a, const TcWeights &w, int math_mode,
         p.residual = nullptr;
     }
     if (!pl.gather && !make_map_2d(&map_a, a.src0, (uint64_t)p.M, (uint64_t)(a.C0 + a.C1), BM)) return cudaErrorInvalidValue;
-    if (p.bf16) {
+    if (bf16) {
         if (!make_map_2d(&map_bhi, w.d_bh, (uint64_t)w.Npad, (uint64_t)w.Kpad64, (uint32_t)p.BN, 0, true)) return cudaErrorInvalidValue;
         if (!make_map_2d(&map_blo, w.d_bm, (uint64_t)w.Npad, (uint64_t)w.Kpad64, (uint32_t)p.BN, 0, true)) return cudaErrorInvalidValue;
     } else {
@@ -775,10 +846,11 @@ cudaError_t launch_conv_tc(const ConvArgs &a, const TcWeights &w, int math_mode,
         if (!make_map_2d(&map_blo, w.d_lo, (uint64_t)w.Npad, (uint64_t)w.Kpad, (uint32_t)p.BN)) return cudaErrorInvalidValue;
     }
 
-    if (p.BN % 16 != 0 || p.BN > MAX_BN) return cudaErrorInvalidConfiguration;
+    // null for a tile width or math mode that has no instantiation
+    const ConvKernel kern = pl.gather ? conv_kernel_for<true>(pl.mode, p.BN) : conv_kernel_for<false>(pl.mode, p.BN);
+    if (!kern) return cudaErrorInvalidConfiguration;
     const dim3 g((unsigned)pl.grid), b(NUM_THREADS);
-    cudaError_t le = pl.gather ? launch_k(conv_kernel_for<true>(p.BN), g, b, smem, st, map_a, map_bhi, map_blo, p)
-                               : launch_k(conv_kernel_for<false>(p.BN), g, b, smem, st, map_a, map_bhi, map_blo, p);
+    cudaError_t le = launch_k(kern, g, b, smem, st, map_a, map_bhi, map_blo, p);
     if (le != cudaSuccess) return le;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;

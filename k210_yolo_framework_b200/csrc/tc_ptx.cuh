@@ -102,9 +102,26 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
     return d;
 }
 
+// per-thread register budget of the calling warpgroup (all 128 threads execute it): dec hands registers back to the CTA's
+// pool, inc waits until the pool has them
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// wait until at most N committed wgmma groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving reads or writes of a wgmma operand register across the wgmma fence / wait next to it
+__device__ __forceinline__ void reg_fence(float &r) { asm volatile("" : "+f"(r)::"memory"); }
 
 // D[64 x N] (+)= A[64 x K] * B[N x K]^T for one warpgroup: A from registers (the fragment layout of mma.m16n8k8 tf32 /
 // m16n8k16 bf16 per warp, rows 16w..16w+15), B from shared memory through a descriptor, fp32 accumulators in registers
