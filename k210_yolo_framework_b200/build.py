@@ -28,7 +28,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not needs_build():
         return OUT
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    extra = os.environ.get("K2Y_NVCC_EXTRA", "").split()   # development builds only (e.g. -DK2Y_NMS_TRACE)
+    extra = os.environ.get("K2Y_NVCC_EXTRA", "").split()   # extra nvcc flags, for development builds only
     cmd = [nvcc] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-o", OUT] + \
           [os.path.join(CSRC, s) for s in SOURCES] + ["-ldl"]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)

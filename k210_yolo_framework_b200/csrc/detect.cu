@@ -7,9 +7,13 @@
 //                       sigmoid(conf) is evaluated once per box, every box is decoded once (tf_xywh_to_all + correct_box)
 //                       into a per-image box table, and every (box, class) with score >= obj_thresh appends its sort key
 //                       (score bits << 32 | ~index) to the class's candidate list.
-//   detect_nms_kernel   CTA = one (image, class): candidate keys and boxes (gathered from the box table) in shared memory,
-//                       then the greedy selection as <= max_per_class rounds of "best candidate still alive (CTA-wide
-//                       arg-max, no sort) -> keep -> every thread tests its candidates against it".
+//   detect_nms_kernel   CTA = one (image, class), 512 threads: the class's greedy NMS in one of three tiers, chosen from its
+//                       candidate count (the rule is stated above the kernel):
+//                         chunked  <= 256 candidates: rank sort, then 32-candidate chunks resolved warp by warp;
+//                         rounds   keys in registers, decoded boxes in shared memory (4 or 8 slots per thread), then
+//                                  <= max_per_class rounds of "best live candidate (CTA-wide arg-max, no sort) -> keep ->
+//                                  every thread tests its candidates against it";
+//                         global   the same rounds with keys, boxes and liveness bits in global memory.
 // REGION_C: one CTA per image (softmax + decode by all threads, then one warp per class).
 //
 // Arithmetic is float32 in the reference's operation order with explicit round-to-nearest intrinsics where FMA
@@ -73,6 +77,15 @@ __device__ __forceinline__ unsigned long long pack_key(float score, int idx) {
 __device__ __forceinline__ int key_index(unsigned long long k) { return (int)(0xffffffffu - (unsigned)(k & 0xffffffffull)); }
 __device__ __forceinline__ float key_score(unsigned long long k) { return __uint_as_float((unsigned)(k >> 32)); }
 
+// The rounds tier's key also carries the candidate's position in shared memory: (score bits << 32) | ((0xFFFFF - index) << 12)
+// | position.  The low 12 bits never decide a comparison (the (score, index) pair is unique), so ONE 64-bit maximum yields the
+// winner AND where its decoded box sits.  Needs index < 2^20 - 1 and position < 4096.
+__device__ __forceinline__ unsigned long long pack_pos_key(unsigned long long key, int pos) {
+    return (key & 0xffffffff00000000ull) | ((unsigned long long)(0xFFFFFu - (unsigned)key_index(key)) << 12) | (unsigned long long)pos;
+}
+__device__ __forceinline__ int pos_key_index(unsigned long long k) { return (int)(0xFFFFFu - (unsigned)((k >> 12) & 0xFFFFFull)); }
+__device__ __forceinline__ int pos_key_position(unsigned long long k) { return (int)(k & 0xFFFull); }
+
 // Sort (descending) n <= 32 keys held one per lane (lanes >= n hold 0).
 __device__ __forceinline__ unsigned long long warp_sort_desc(unsigned long long key, int lane) {
 #pragma unroll
@@ -113,7 +126,14 @@ __device__ __forceinline__ void warp_sort_desc_mem(unsigned long long *keys, int
 // the division in the common case: inter/uni > thr  <=>  inter > thr*uni (uni > 0).  The product form is only trusted
 // outside a 1e-6 relative margin (>> the 3 roundings involved); inside it the exact IEEE division decides, so the
 // boolean is bit-identical to the reference's `iou > iou_threshold`.  Boxes are (min,max)-normalised with their areas
-// cached (once per box instead of once per pair).
+// cached (once per box instead of once per pair).  One body computes the intersection and union; two control-flow forms decide
+// the same boolean from them:
+//   iou_norm_gt     straight-line (selects, the exact division only under a rarely-taken branch).  The chunked tier tests up to
+//                   eight independent pairs per thread in a row, and with early-outs the compiler serialises those chains
+//                   (~190 cycles each) instead of interleaving them.
+//   iou_norm_gt_eo  early returns.  The rounds tiers and the operator NMS test one pair per live candidate under its own liveness
+//                   branch; there the early-out form measured faster (on an H100 at 700 W the 8-slot rounds tier ran ~9 %
+//                   slower with the straight-line form).
 __device__ __forceinline__ float4 norm_box(const float4 a, float &area) {
     float4 n;
     n.x = fminf(a.x, a.z);
@@ -123,28 +143,15 @@ __device__ __forceinline__ float4 norm_box(const float4 a, float &area) {
     area = __fmul_rn(__fsub_rn(n.z, n.x), __fsub_rn(n.w, n.y));
     return n;
 }
-__device__ __forceinline__ bool iou_norm_gt(const float4 a, float area_a, const float4 b, float area_b, float thr) {
-    if (area_a <= 0.f || area_b <= 0.f) return 0.f > thr;
+__device__ __forceinline__ float2 iou_terms(const float4 a, float area_a, const float4 b, float area_b) {
     const float iy = fmaxf(__fsub_rn(fminf(a.z, b.z), fmaxf(a.x, b.x)), 0.f);
     const float ix = fmaxf(__fsub_rn(fminf(a.w, b.w), fmaxf(a.y, b.y)), 0.f);
     const float inter = __fmul_rn(iy, ix);
-    const float uni = __fsub_rn(__fadd_rn(area_a, area_b), inter);
-    if (thr >= 0.f && uni > 0.f) {
-        const float t = __fmul_rn(thr, uni);
-        if (inter > __fmul_rn(t, 1.000001f)) return true;
-        if (inter < __fmul_rn(t, 0.999999f)) return false;
-    }
-    return __fdiv_rn(inter, uni) > thr;
+    return make_float2(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
 }
-
-// The same predicate as straight-line code (selects instead of early returns; the exact division only under a rarely-taken
-// branch): the register-resident NMS tests up to 8 candidates per thread per round, and with early-outs the compiler serialises
-// them (~190 cycles each) instead of interleaving the independent chains.
-__device__ __forceinline__ bool iou_norm_gt_sl(const float4 a, float area_a, const float4 b, float area_b, float thr) {
-    const float iy = fmaxf(__fsub_rn(fminf(a.z, b.z), fmaxf(a.x, b.x)), 0.f);
-    const float ix = fmaxf(__fsub_rn(fminf(a.w, b.w), fmaxf(a.y, b.y)), 0.f);
-    const float inter = __fmul_rn(iy, ix);
-    const float uni = __fsub_rn(__fadd_rn(area_a, area_b), inter);
+__device__ __forceinline__ bool iou_norm_gt(const float4 a, float area_a, const float4 b, float area_b, float thr) {
+    const float2 iu = iou_terms(a, area_a, b, area_b);
+    const float inter = iu.x, uni = iu.y;
     const float t = __fmul_rn(thr, uni);
     const bool usable = thr >= 0.f && uni > 0.f;                       // the product form is only trusted then
     const bool gt = usable && inter > __fmul_rn(t, 1.000001f);
@@ -153,6 +160,17 @@ __device__ __forceinline__ bool iou_norm_gt_sl(const float4 a, float area_a, con
     if (!(gt || lt)) res = __fdiv_rn(inter, uni) > thr;                 // inside the margin (or degenerate): exact IEEE division
     const bool degenerate = area_a <= 0.f || area_b <= 0.f;             // zero-area boxes: IoU 0
     return degenerate ? (0.f > thr) : res;
+}
+__device__ __forceinline__ bool iou_norm_gt_eo(const float4 a, float area_a, const float4 b, float area_b, float thr) {
+    if (area_a <= 0.f || area_b <= 0.f) return 0.f > thr;
+    const float2 iu = iou_terms(a, area_a, b, area_b);
+    const float inter = iu.x, uni = iu.y;
+    if (thr >= 0.f && uni > 0.f) {
+        const float t = __fmul_rn(thr, uni);
+        if (inter > __fmul_rn(t, 1.000001f)) return true;
+        if (inter < __fmul_rn(t, 0.999999f)) return false;
+    }
+    return __fdiv_rn(inter, uni) > thr;
 }
 
 // region_layer.c box_iou on centre-form (x,y,w,h) boxes (:228-254).
@@ -196,16 +214,15 @@ struct KerasParams {
     int cap;                          // candidates the NMS kernel can hold in shared memory (key 8 B + decoded box 16 B each)
 };
 
-// Collects the candidates of one class (score passes `pred`) in index order, sorts them.
+// Collects the candidates of one class (score > thr) in index order, sorts them.
 // Returns n; on return either `rkey` holds the sorted keys (n <= 32) or keys[0..n) does.
-template <bool GE>
 __device__ __forceinline__ int gather_sorted(const float *sc, int nbox, float thr, unsigned long long *keys, int lane,
                                              unsigned long long &rkey) {
     int n = 0;
     for (int base = 0; base < nbox; base += 32) {
         const int i = base + lane;
         const float s = (i < nbox) ? sc[i] : -1.f;
-        const bool pass = (i < nbox) && (GE ? (s >= thr) : (s > thr));
+        const bool pass = (i < nbox) && s > thr;
         const unsigned m = __ballot_sync(FULL, pass);
         if (pass) keys[n + __popc(m & ((1u << lane) - 1u))] = pack_key(s, i);
         n += __popc(m);
@@ -225,40 +242,43 @@ __device__ __forceinline__ int gather_sorted(const float *sc, int nbox, float th
     return n;
 }
 
-struct BoxXform {  // correct_box constants of one image (keras_inference.py:53-58)
+// The box decode, shared by the fused scan kernel and the operator kernels (xywh_to_all_kernel, correct_box_kernel), so
+// that both give the same bits.
+
+// correct_box's letterbox constants of one image (keras_inference.py:53-58)
+struct BoxXform {
     float img_h, img_w, off_y, off_x, sc_y, sc_x;
 };
-
-__device__ __forceinline__ BoxXform make_xform(const KerasParams &p, int b) {
+__device__ __forceinline__ BoxXform letterbox(float in_h, float in_w, float img_h, float img_w) {
     BoxXform x;
-    x.img_h = p.image_hw[2 * b];
-    x.img_w = p.image_hw[2 * b + 1];
-    const float r = fminf(__fdiv_rn(p.in_h, x.img_h), __fdiv_rn(p.in_w, x.img_w));
-    const float new_h = rintf(__fmul_rn(x.img_h, r)), new_w = rintf(__fmul_rn(x.img_w, r));
-    x.off_y = __fdiv_rn(__fdiv_rn(__fsub_rn(p.in_h, new_h), 2.0f), p.in_h);
-    x.off_x = __fdiv_rn(__fdiv_rn(__fsub_rn(p.in_w, new_w), 2.0f), p.in_w);
-    x.sc_y = __fdiv_rn(p.in_h, new_h);
-    x.sc_x = __fdiv_rn(p.in_w, new_w);
+    x.img_h = img_h;
+    x.img_w = img_w;
+    const float r = fminf(__fdiv_rn(in_h, img_h), __fdiv_rn(in_w, img_w));
+    const float new_h = rintf(__fmul_rn(img_h, r)), new_w = rintf(__fmul_rn(img_w, r));
+    x.off_y = __fdiv_rn(__fdiv_rn(__fsub_rn(in_h, new_h), 2.0f), in_h);
+    x.off_x = __fdiv_rn(__fdiv_rn(__fsub_rn(in_w, new_w), 2.0f), in_w);
+    x.sc_y = __fdiv_rn(in_h, new_h);
+    x.sc_x = __fdiv_rn(in_w, new_w);
     return x;
 }
 
-// tf_xywh_to_all (tools/utils.py:545-546) + correct_box (keras_inference.py:59-71) for one box, on a record whose first four entries
-// already hold sigmoid(tx), sigmoid(ty), exp(tw), exp(th) (the scan kernel spreads those over all of its threads).
-__device__ __forceinline__ float4 assemble_box(const KerasParams &p, const BoxXform &x, int box, const float *e) {
-    int l = 0;
-    if (p.n_layers > 1 && box >= p.loff[1]) l = 1;
-    if (p.n_layers > 2 && box >= p.loff[2]) l = 2;
-    const int local = box - p.loff[l];
-    const int a = local % p.A;
-    const int cell = local / p.A;
-    const int W = p.lw[l];
-    const int col = cell % W, row = cell / W;
-    const float bx = __fdiv_rn(__fadd_rn(e[0], (float)col), (float)W);
-    const float by = __fdiv_rn(__fadd_rn(e[1], (float)row), (float)p.lh[l]);
-    const float bw = __fmul_rn(e[2], p.anchors[(l * p.A + a) * 2]);
-    const float bh = __fmul_rn(e[3], p.anchors[(l * p.A + a) * 2 + 1]);
-    const float cy = __fmul_rn(__fsub_rn(by, x.off_y), x.sc_y), cx = __fmul_rn(__fsub_rn(bx, x.off_x), x.sc_x);
-    const float hh2 = __fdiv_rn(__fmul_rn(bh, x.sc_y), 2.0f), ww2 = __fdiv_rn(__fmul_rn(bw, x.sc_x), 2.0f);
+// tf_xywh_to_all (tools/utils.py:545-546) for one box, given sigmoid(tx), sigmoid(ty), exp(tw), exp(th), its cell (col, row)
+// of a W x H layer and its anchor (aw, ah): (x, y, w, h) as fractions of the network input
+__device__ __forceinline__ float4 xywh_to_all(float sx, float sy, float ew, float eh, int col, int row, int W, int H, float aw,
+                                              float ah) {
+    float4 r;
+    r.x = __fdiv_rn(__fadd_rn(sx, (float)col), (float)W);
+    r.y = __fdiv_rn(__fadd_rn(sy, (float)row), (float)H);
+    r.z = __fmul_rn(ew, aw);
+    r.w = __fmul_rn(eh, ah);
+    return r;
+}
+
+// correct_box (keras_inference.py:59-71) for one box: (x, y, w, h) relative to the letterboxed input -> (ymin, xmin, ymax, xmax)
+// in pixels of the original image
+__device__ __forceinline__ float4 to_corners(const BoxXform &x, const float4 b) {
+    const float cy = __fmul_rn(__fsub_rn(b.y, x.off_y), x.sc_y), cx = __fmul_rn(__fsub_rn(b.x, x.off_x), x.sc_x);
+    const float hh2 = __fdiv_rn(__fmul_rn(b.w, x.sc_y), 2.0f), ww2 = __fdiv_rn(__fmul_rn(b.z, x.sc_x), 2.0f);
     float4 r;
     r.x = __fmul_rn(__fsub_rn(cy, hh2), x.img_h);
     r.y = __fmul_rn(__fsub_rn(cx, ww2), x.img_w);
@@ -335,9 +355,20 @@ __global__ void __launch_bounds__(SCAN_THREADS) detect_scan_kernel(const KerasPa
         }
         s_thr[tid] = thr;
     } else if (tid >= SCAN_BOXES && tid < SCAN_BOXES + nb) {
+        // the record's first four entries hold sigmoid(tx), sigmoid(ty), exp(tw), exp(th) now
         const int i = tid - SCAN_BOXES;
-        const BoxXform x = make_xform(p, b);
-        p.boxes[(size_t)b * p.nbox + box0 + i] = assemble_box(p, x, box0 + i, s_rec + i * E);
+        const BoxXform x = letterbox(p.in_h, p.in_w, p.image_hw[2 * b], p.image_hw[2 * b + 1]);
+        const float *e = s_rec + i * E;
+        const int box = box0 + i;
+        int l = 0;
+        if (p.n_layers > 1 && box >= p.loff[1]) l = 1;
+        if (p.n_layers > 2 && box >= p.loff[2]) l = 2;
+        const int local = box - p.loff[l];
+        const int a = local % p.A, cell = local / p.A;
+        const int W = p.lw[l];
+        const float4 xywh = xywh_to_all(e[0], e[1], e[2], e[3], cell % W, cell / W, W, p.lh[l], p.anchors[(l * p.A + a) * 2],
+                                        p.anchors[(l * p.A + a) * 2 + 1]);
+        p.boxes[(size_t)b * p.nbox + box0 + i] = to_corners(x, xywh);
     }
     __syncthreads();
     const bool shortcut = p.logit_min > -__int_as_float(0x7f800000);
@@ -378,50 +409,45 @@ __global__ void __launch_bounds__(SCAN_THREADS) detect_scan_kernel(const KerasPa
     }
 }
 
-// ---- pass 2: greedy NMS by repeated selection.  grid = (C, B), one CTA per (image, class) ------------------------------
+// ---- pass 2: greedy NMS.  grid = (C, B), one CTA of NMS_THREADS per (image, class) ---------------------------------------
 // tf.image.non_max_suppression visits candidates in descending score and keeps one iff no box kept earlier overlaps it by
-// more than the threshold.  Equivalently: repeat { take the best candidate still alive, keep it, kill everything it
-// overlaps } — at most max_per_class rounds, with NO sort: a round is an arg-max over the live candidates (three
-// warp-reduce instructions on the (score bits, ~index, position) triple + one shared-memory exchange) followed by one
-// IoU test per live candidate, all candidates spread over the CTA's threads.  The selection order is exactly the order of
-// the sorted keys (score descending, index ascending), so the records equal the sequential algorithm's.
-constexpr int NMS_MAX_WARPS = 16;   // the kernel runs with 256 (cap <= 2048) or 512 threads
+// more than the threshold.  The rounds tiers restate this as: repeat { take the best candidate still alive, keep it, kill
+// everything it overlaps } — at most max_per_class rounds, with NO sort: a round is an arg-max over the live candidates
+// (warp-reduce instructions on the key + one shared-memory exchange) followed by one IoU test per live candidate, all
+// candidates spread over the CTA's threads.  The selection order is exactly the order of the sorted keys (score descending,
+// index ascending), so the records equal the sequential algorithm's.
+constexpr int NMS_THREADS = 512;
+constexpr int NMS_WARPS = NMS_THREADS / 32;
 
-__device__ __forceinline__ void write_det(k2y_det *out, int slot, unsigned long long key, const float4 kb) {
+__device__ __forceinline__ void write_det(k2y_det *out, int slot, const float4 box, float score, int index) {
     k2y_det d;
-    d.ymin = kb.x;
-    d.xmin = kb.y;
-    d.ymax = kb.z;
-    d.xmax = kb.w;
-    d.score = key_score(key);
-    d.index = key_index(key);
+    d.ymin = box.x;
+    d.xmin = box.y;
+    d.ymax = box.z;
+    d.xmax = box.w;
+    d.score = score;
+    d.index = index;
     out[slot] = d;
 }
 
-template <bool SMEM, int NMS_THREADS>
-__device__ __forceinline__ int nms_rounds(const KerasParams &p, int n, const unsigned long long *keys, const float4 *s_box, const float *s_area,
-                                          const float4 *gboxes, unsigned *alive_g, k2y_det *out, int (*s_red)[NMS_MAX_WARPS][3]) {
-    constexpr int NMS_WARPS = NMS_THREADS / 32;
+// Global-memory rounds (n > cap): keys and decoded boxes are read from the global candidate lists, the liveness bits live in
+// global memory.  Candidate `pos` belongs to thread pos % NMS_THREADS; its liveness is bit (pos / NMS_THREADS) % 32 of the
+// thread's word (pos / NMS_THREADS) / 32.
+__device__ __forceinline__ int nms_rounds(const KerasParams &p, int n, const unsigned long long *keys, const float4 *gboxes,
+                                          unsigned *alive_g, k2y_det *out, int (*s_red)[NMS_WARPS][3]) {
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    // candidate `pos` belongs to thread pos % NMS_THREADS; its liveness is bit (pos / NMS_THREADS) % 32 of the thread's mask word
-    // (pos / NMS_THREADS) / 32 — one register in the shared-memory path (cap <= 32 * NMS_THREADS), global words otherwise
     const int slots = n > tid ? (n - tid + NMS_THREADS - 1) / NMS_THREADS : 0;
     const int nwords = (slots + 31) >> 5;
-    unsigned mask0 = 0u;
-    if (SMEM) {
-        mask0 = slots >= 32 ? 0xffffffffu : ((1u << slots) - 1u);
-    } else {
-        for (int w = 0; w < nwords; ++w) {
-            const int left = slots - w * 32;
-            alive_g[(size_t)w * NMS_THREADS + tid] = left >= 32 ? 0xffffffffu : ((1u << left) - 1u);
-        }
+    for (int w = 0; w < nwords; ++w) {
+        const int left = slots - w * 32;
+        alive_g[(size_t)w * NMS_THREADS + tid] = left >= 32 ? 0xffffffffu : ((1u << left) - 1u);
     }
     int nsel = 0, par = 0;
     // best live candidate of this thread; afterwards maintained by the kill pass of each round
     unsigned long long best = 0ull;
     int bpos = -1;
-    for (int w = 0; w < (SMEM ? 1 : nwords); ++w) {
-        for (unsigned m = SMEM ? mask0 : alive_g[(size_t)w * NMS_THREADS + tid]; m;) {
+    for (int w = 0; w < nwords; ++w) {
+        for (unsigned m = alive_g[(size_t)w * NMS_THREADS + tid]; m;) {
             const int q = __ffs(m) - 1;
             m &= m - 1u;
             const int pos = tid + (w * 32 + q) * NMS_THREADS;
@@ -461,20 +487,15 @@ __device__ __forceinline__ int nms_rounds(const KerasParams &p, int n, const uns
         par ^= 1;
         if (wpos == 0x7fffffff) break;   // nothing alive
         const unsigned long long wkey = ((unsigned long long)whi << 32) | wlo;
-        float4 kb;
+        const float4 ob = gboxes[key_index(wkey)];
         float ka;
-        if (SMEM) {
-            kb = s_box[wpos];
-            ka = s_area[wpos];
-        } else {
-            kb = norm_box(gboxes[key_index(wkey)], ka);
-        }
-        if (tid == 0) write_det(out, nsel, wkey, gboxes[key_index(wkey)]);
+        const float4 kb = norm_box(ob, ka);
+        if (tid == 0) write_det(out, nsel, ob, key_score(wkey), key_index(wkey));
         // ---- the kept box kills what it overlaps (and itself); the same pass finds this thread's best survivor ----
         best = 0ull;
         bpos = -1;
-        for (int w = 0; w < (SMEM ? 1 : nwords); ++w) {
-            unsigned word = SMEM ? mask0 : alive_g[(size_t)w * NMS_THREADS + tid];
+        for (int w = 0; w < nwords; ++w) {
+            unsigned word = alive_g[(size_t)w * NMS_THREADS + tid];
             for (unsigned m = word; m;) {
                 const int q = __ffs(m) - 1;
                 m &= m - 1u;
@@ -482,13 +503,9 @@ __device__ __forceinline__ int nms_rounds(const KerasParams &p, int n, const uns
                 bool kill = pos == wpos;
                 const unsigned long long k = keys[pos];
                 if (!kill) {
-                    if (SMEM) {
-                        kill = iou_norm_gt(kb, ka, s_box[pos], s_area[pos], p.iou);
-                    } else {
-                        float ar;
-                        const float4 cb = norm_box(gboxes[key_index(k)], ar);
-                        kill = iou_norm_gt(kb, ka, cb, ar, p.iou);
-                    }
+                    float ar;
+                    const float4 cb = norm_box(gboxes[key_index(k)], ar);
+                    kill = iou_norm_gt_eo(kb, ka, cb, ar, p.iou);
                 }
                 if (kill) {
                     word &= ~(1u << q);
@@ -497,24 +514,21 @@ __device__ __forceinline__ int nms_rounds(const KerasParams &p, int n, const uns
                     bpos = pos;
                 }
             }
-            if (SMEM) mask0 = word;
-            else alive_g[(size_t)w * NMS_THREADS + tid] = word;
+            alive_g[(size_t)w * NMS_THREADS + tid] = word;
         }
         ++nsel;
     }
     return nsel;
 }
 
-// Shared-memory rounds (CHUNK_MAX < n <= cap <= 4096): every thread keeps the packed keys of its candidates in registers —
-// position t + s * NMS_THREADS in slot s; their boxes stay in shared memory (the register budget decides how many CTAs fit an SM).  The packed key is (score bits << 32) | ((0xFFFFF - index)
-// << 12) | position: the low 12 bits never decide a comparison (the (score, index) pair is unique), so ONE 64-bit maximum yields
-// the winner AND where its decoded box sits in shared memory.  A round: per-warp maximum (two warp-reduce instructions) ->
-// shared memory -> barrier -> every warp reduces the per-warp maxima again -> winner's box from shared memory -> IoU tests of
-// the thread's own live candidates.  Work-efficient (maxk x n IoU tests), but maxk barrier-separated rounds.
-template <int NMS_THREADS, int SLOTS>
+// Shared-memory rounds (n <= cap <= 4096): every thread keeps the position-carrying keys (pack_pos_key) of its candidates in
+// registers — position t + s * NMS_THREADS in slot s; their boxes stay in shared memory (the register budget decides how many
+// CTAs fit an SM).  A round: per-warp maximum (two warp-reduce instructions) -> shared memory -> barrier -> every warp reduces
+// the per-warp maxima again -> winner's box from shared memory -> IoU tests of the thread's own live candidates.
+// Work-efficient (maxk x n IoU tests), but maxk barrier-separated rounds.
+template <int SLOTS>
 __device__ __forceinline__ int nms_rounds_smem(const KerasParams &p, int n, const unsigned long long *s_keys, const float4 *s_box,
                                                k2y_det *out, unsigned long long *s_best) {
-    constexpr int NMS_WARPS = NMS_THREADS / 32;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     unsigned long long pk[SLOTS];
     unsigned alive = 0u;
@@ -524,8 +538,7 @@ __device__ __forceinline__ int nms_rounds_smem(const KerasParams &p, int n, cons
         const int pos = tid + s * NMS_THREADS;
         pk[s] = 0ull;
         if (pos < n) {
-            const unsigned long long k = s_keys[pos];
-            pk[s] = (k & 0xffffffff00000000ull) | ((unsigned long long)(0xFFFFFu - (unsigned)key_index(k)) << 12) | (unsigned long long)pos;
+            pk[s] = pack_pos_key(s_keys[pos], pos);
             alive |= 1u << s;
             tbest = pk[s] > tbest ? pk[s] : tbest;
         }
@@ -548,26 +561,17 @@ __device__ __forceinline__ int nms_rounds_smem(const KerasParams &p, int n, cons
         const unsigned wlo = __reduce_max_sync(FULL, (unsigned)(mine >> 32) == whi ? (unsigned)mine : 0u);
         const unsigned long long w = ((unsigned long long)whi << 32) | wlo;
         if (w == 0ull) break;   // nothing alive (a live key is never 0: its index field is non-zero)
-        const float4 ob = s_box[(int)(w & 0xFFFull)];   // as decoded (the record keeps these); every thread normalises its own copy
+        const float4 ob = s_box[pos_key_position(w)];   // as decoded (the record keeps these); every thread normalises its own copy
         float ka;
         const float4 kb = norm_box(ob, ka);
-        if (tid == 0) {
-            k2y_det d;
-            d.ymin = ob.x;
-            d.xmin = ob.y;
-            d.ymax = ob.z;
-            d.xmax = ob.w;
-            d.score = __uint_as_float((unsigned)(w >> 32));
-            d.index = (int)(0xFFFFFu - (unsigned)((w >> 12) & 0xFFFFFull));
-            out[nsel] = d;
-        }
+        if (tid == 0) write_det(out, nsel, ob, key_score(w), pos_key_index(w));
         tbest = 0ull;
 #pragma unroll
         for (int s = 0; s < SLOTS; ++s) {
             if ((alive >> s) & 1u) {
                 float ar;
                 const float4 bx = norm_box(s_box[tid + s * NMS_THREADS], ar);   // from shared memory: 2 registers per slot, not 7
-                if (pk[s] == w || iou_norm_gt(kb, ka, bx, ar, p.iou)) alive &= ~(1u << s);
+                if (pk[s] == w || iou_norm_gt_eo(kb, ka, bx, ar, p.iou)) alive &= ~(1u << s);
                 else tbest = pk[s] > tbest ? pk[s] : tbest;
             }
         }
@@ -576,7 +580,7 @@ __device__ __forceinline__ int nms_rounds_smem(const KerasParams &p, int n, cons
     return nsel;
 }
 
-// Chunked path (n <= CHUNK_MAX = 256 candidates, maxk <= CHUNK_MAXK): the usual case.  Greedy NMS keeps a candidate iff no
+// Chunked tier (n <= CHUNK_MAX = 256 candidates, maxk <= CHUNK_MAXK): the usual case.  Greedy NMS keeps a candidate iff no
 // EARLIER KEPT candidate (in (score desc, index asc) order) overlaps it by more than the threshold, so with the candidates in
 // that order the serial dependence is between 32-candidate chunks, not between survivors:
 //   1. rank sort: two lanes per candidate (l, l ^ 16 of one warp) count the keys <= its own, half of the list each — broadcast
@@ -594,14 +598,10 @@ __device__ __forceinline__ int nms_rounds_smem(const KerasParams &p, int n, cons
 //      later warps wait on it and test their candidate against the newly kept boxes only (four independent tests at a time).
 //      Every candidate still meets each survivor at most once (work n x maxk + 16 n tests), but the barrier count drops from
 //      maxk (30) to n/32 (<= 8) and finished warps stop paying.
-// The IoU predicate is that of the rounds path, so the decisions are the same bits.  Needs blockDim.x == 2 * CHUNK_MAX.
+// Its IoU test (iou_norm_gt) decides the same booleans as the rounds tiers' (iou_norm_gt_eo): same terms, same decision rule.
 constexpr int CHUNK_MAX = 256;
 constexpr int CHUNK_MAXK = 64;
-#ifdef K2Y_NMS_TRACE   // development aid: phase clocks of the dense classes of image 0, printed per warp
-#define NMS_T(i) do { if (lane == 0) tr[i] = clock64(); } while (0)
-#else
-#define NMS_T(i) do { } while (0)
-#endif
+static_assert(NMS_THREADS == 2 * CHUNK_MAX, "the chunked tier runs two lanes per candidate");
 struct __align__(16) ChunkShared {
     unsigned long long skey[CHUNK_MAX];   // sorted keys
     float4 sobox[CHUNK_MAX];              // sorted boxes as decoded
@@ -612,7 +612,7 @@ struct __align__(16) ChunkShared {
     float karea[CHUNK_MAXK];
     int cnt[CHUNK_MAX / 32];              // survivors after chunk c
 };
-constexpr size_t CHUNK_SMEM = (CHUNK_MAX + 4) * sizeof(unsigned long long) + sizeof(ChunkShared);   // arrival keys (padded to x4), tables
+constexpr size_t CHUNK_SMEM_BYTES = (CHUNK_MAX + 4) * sizeof(unsigned long long) + sizeof(ChunkShared);   // arrival keys (padded to x4), tables
 
 // r += (a >= b) for 64-bit keys given as 32-bit halves: the borrow chain of a - b, its final carry added to r
 __device__ __forceinline__ void count_ge(unsigned &r, unsigned alo, unsigned ahi, unsigned blo, unsigned bhi) {
@@ -635,11 +635,6 @@ __device__ __forceinline__ void nms_chunked(const KerasParams &p, int n, const u
     constexpr int HW = CHUNK_MAX / 32;   // warps 0..7 own the chunks, warps 8..15 help with the pair tests
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int nchunks = (n + 31) >> 5;
-#ifdef K2Y_NMS_TRACE
-    long long tr[16];
-    for (int i = 0; i < 16; ++i) tr[i] = 0;
-#endif
-    NMS_T(0);
     // phase 1: warp w, lanes l and l ^ 16 <-> candidate 16 w + (l & 15)
     const int half = lane >> 4, ci = warp * 16 + (lane & 15);
     const bool cvalid = ci < n;
@@ -653,7 +648,6 @@ __device__ __forceinline__ void nms_chunked(const KerasParams &p, int n, const u
         }
         if (!half && ci < L) s_arrival[ci] = kt;
         __syncthreads();
-        NMS_T(1);
         const bool ranks = warp * 16 < n, pairs_too = (warp < HW ? warp : warp - HW) < nchunks;
         if (!ranks && !pairs_too) return;   // (warp-uniform) the named barrier below counts the warps that stay
         if (ranks) {
@@ -682,11 +676,9 @@ __device__ __forceinline__ void nms_chunked(const KerasParams &p, int n, const u
                 }
             }
         }
-        NMS_T(2);
         int staying = 0;
         for (int w = 0; w < 2 * HW; ++w) staying += (w * 16 < n || (w < HW ? w : w - HW) < nchunks) ? 32 : 0;
         named_sync(1, staying);
-        NMS_T(3);
     }
     // phase 2: warps c and 8+c, lane q <-> sorted candidate 32 c + q
     const int c_own = warp < HW ? warp : warp - HW;
@@ -705,7 +697,7 @@ __device__ __forceinline__ void nms_chunked(const KerasParams &p, int n, const u
 #pragma unroll
         for (int u = 1; u <= 8; ++u) {
             const int d = d0 + u, b = (lane + d) & 31;
-            bool hit = iou_norm_gt_sl(cs.snbox[32 * c_own + b], cs.sarea[32 * c_own + b], nb, ar, p.iou);
+            bool hit = iou_norm_gt(cs.snbox[32 * c_own + b], cs.sarea[32 * c_own + b], nb, ar, p.iou);
             hit = hit && valid && 32 * c_own + b < n && !(d == 16 && lane >= 16);   // distance 16: from the lower member only
             const unsigned T = __ballot_sync(FULL, hit);   // bit q: members q and (q + d) & 31 overlap
             if (lane + d < 32) myrow |= ((T >> lane) & 1u) << (lane + d);   // my own test, partner above me
@@ -718,7 +710,6 @@ __device__ __forceinline__ void nms_chunked(const KerasParams &p, int n, const u
         named_arrive(4 + c_own, 64);
         return;
     }
-    NMS_T(4);
     named_sync(4 + c_own, 64);
     myrow |= cs.rows[si];
     // phase 3
@@ -727,7 +718,6 @@ __device__ __forceinline__ void nms_chunked(const KerasParams &p, int n, const u
     for (int c = 0; c < nchunks; ++c) {
         const int nthr = (nchunks - c) * 32;   // warps c .. nchunks-1 meet at this step's barrier (ids alternate: the count changes)
         if (warp == c) {
-            NMS_T(5);
             unsigned R = __ballot_sync(FULL, removed), K = 0u;
             const int room = p.maxk - base;
             int count = 0;
@@ -751,24 +741,9 @@ __device__ __forceinline__ void nms_chunked(const KerasParams &p, int n, const u
             }
             if (kept) {
                 const unsigned long long k = cs.skey[si];
-                const float4 o = cs.sobox[si];
-                k2y_det d;
-                d.ymin = o.x;
-                d.xmin = o.y;
-                d.ymax = o.z;
-                d.xmax = o.w;
-                d.score = __uint_as_float((unsigned)(k >> 32));
-                d.index = key_index(k);
-                out[base + slot] = d;
+                write_det(out, base + slot, cs.sobox[si], key_score(k), key_index(k));
             }
             if (lane == 0 && (c == nchunks - 1 || total >= p.maxk)) *count_out = total;
-            NMS_T(6);
-#ifdef K2Y_NMS_TRACE
-            if (lane == 0 && blockIdx.y == 0 && n > 128)
-                printf("nms-trace class %d n %d chunk %d/%d base %d: load %lld rank %lld bar %lld pairs %lld wait %lld resolve %lld total %lld\n",
-                       (int)blockIdx.x, n, c, nchunks, base, tr[1] - tr[0], tr[2] - tr[1], tr[3] - tr[2], tr[4] - tr[3], tr[5] - tr[4],
-                       tr[6] - tr[5], tr[6] - tr[0]);
-#endif
             return;
         }
         named_sync(2 + (c & 1), nthr);
@@ -781,7 +756,7 @@ __device__ __forceinline__ void nms_chunked(const KerasParams &p, int n, const u
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
                     const int kk = min(k + u, total - 1);
-                    hit |= iou_norm_gt_sl(cs.kbox[kk], cs.karea[kk], nb, ar, p.iou);
+                    hit |= iou_norm_gt(cs.kbox[kk], cs.karea[kk], nb, ar, p.iou);
                 }
                 if (hit) {
                     removed = true;
@@ -794,17 +769,21 @@ __device__ __forceinline__ void nms_chunked(const KerasParams &p, int n, const u
     }
 }
 
-// 512 threads: two lanes per candidate in the chunked path's sort / mask phases, NMS_THREADS x SLOTS >= cap candidates in the
-// rounds path (4 slots up to 2048 candidates, 8 beyond: one instantiation each, so that the common grids are not compiled at
-// the register count of the largest).
-template <int NMS_THREADS, int SLOTS>
+// The tier of one (image, class) follows from its candidate count n, max_per_class (maxk) and cap = min(round_up(nbox, 256),
+// 4096), the number of candidates whose keys and decoded boxes the shared memory holds (0 when nbox >= 2^20 - 1):
+//   - chunked:                       n <= 256 (CHUNK_MAX) and maxk <= 64 (CHUNK_MAXK);
+//   - shared-memory rounds, 4 slots: not chunked, n <= cap and cap <= 2048;
+//   - shared-memory rounds, 8 slots: not chunked, n <= cap and cap > 2048;
+//   - global-memory rounds:          not chunked and n > cap.
+// SLOTS is chosen on the host from cap (NMS_THREADS x SLOTS >= cap), one instantiation each, so that the common grids are not
+// compiled at the register count of the largest.
+template <int SLOTS>
 __global__ void __launch_bounds__(NMS_THREADS, 2) detect_nms_kernel(const KerasParams p) {
-    constexpr int NMS_WARPS = NMS_THREADS / 32;
     extern __shared__ __align__(16) unsigned char s_nms[];
-    __shared__ int s_red[2][NMS_MAX_WARPS][3];
-    __shared__ unsigned long long s_best[2 * NMS_MAX_WARPS];
+    __shared__ int s_red[2][NMS_WARPS][3];
+    __shared__ unsigned long long s_best[2 * NMS_WARPS];
     pdl_trigger();
-    const int c = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int c = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     pdl_wait();
     const int n = p.ncand[b * p.C + c];
     k2y_det *out = reinterpret_cast<k2y_det *>(reinterpret_cast<int *>(p.dets) + (size_t)b * p.det_stride) + (size_t)c * p.maxk;
@@ -817,8 +796,8 @@ __global__ void __launch_bounds__(NMS_THREADS, 2) detect_nms_kernel(const KerasP
     const float4 *gboxes = p.boxes + (size_t)b * p.nbox;
 
     int nsel;
-    if (NMS_THREADS == 2 * CHUNK_MAX && n <= CHUNK_MAX && p.maxk <= CHUNK_MAXK) {
-        // dynamic region = [CHUNK_MAX + 4] arrival-order keys, then the chunk tables (the launch provides at least CHUNK_SMEM bytes)
+    if (n <= CHUNK_MAX && p.maxk <= CHUNK_MAXK) {
+        // dynamic region = [CHUNK_MAX + 4] arrival-order keys, then the chunk tables (the launch provides at least CHUNK_SMEM_BYTES)
         nms_chunked(p, n, gkeys, gboxes, out, count_out, reinterpret_cast<unsigned long long *>(s_nms),
                     *reinterpret_cast<ChunkShared *>(s_nms + (CHUNK_MAX + 4) * sizeof(unsigned long long)));
         return;
@@ -833,10 +812,10 @@ __global__ void __launch_bounds__(NMS_THREADS, 2) detect_nms_kernel(const KerasP
             s_box[i] = gboxes[key_index(k)];
         }
         __syncthreads();
-        nsel = nms_rounds_smem<NMS_THREADS, SLOTS>(p, n, s_keys, s_box, out, s_best);
+        nsel = nms_rounds_smem<SLOTS>(p, n, s_keys, s_box, out, s_best);
     } else {
         unsigned *alive_g = p.alive + ((size_t)b * p.C + c) * (size_t)p.alive_stride;
-        nsel = nms_rounds<false, NMS_THREADS>(p, n, gkeys, nullptr, nullptr, gboxes, alive_g, out, s_red);
+        nsel = nms_rounds(p, n, gkeys, gboxes, alive_g, out, s_red);
     }
     if (tid == 0) *count_out = nsel;
 }
@@ -915,7 +894,7 @@ __global__ void __launch_bounds__(DET_THREADS) region_kernel(const RegionParams 
         unsigned long long *keys = p.keys + ((size_t)b * p.C + k) * p.P;
         int *kept = p.kept + ((size_t)b * p.C + k) * p.N;
         unsigned long long rkey;
-        const int n = gather_sorted<false>(scores + (size_t)k * p.N, p.N, 0.f, keys, lane, rkey);
+        const int n = gather_sorted(scores + (size_t)k * p.N, p.N, 0.f, keys, lane, rkey);
         float4 mybox = make_float4(0.f, 0.f, 0.f, 0.f);
         int nsel = 0;
         for (int i = 0; i < n; ++i) {
@@ -944,7 +923,7 @@ __global__ void __launch_bounds__(DET_THREADS) region_kernel(const RegionParams 
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Operator-level entry points of the reference's decode loop (keras_inference.py:94-135), for callers that keep that loop
-// and replace one operator at a time.  Same arithmetic (intrinsics, operation order) as the fused kernel above.
+// and replace one operator at a time.  They call the fused path's decode helpers and IoU terms, so they give its bits.
 // ---------------------------------------------------------------------------------------------------------------------
 struct OpsAnchors {
     float wh[16];  // (w, h) pairs of one layer, A <= 8
@@ -958,15 +937,11 @@ __global__ void __launch_bounds__(256) xywh_to_all_kernel(const float2 *__restri
     if (i >= total) return;
     const int a = (int)(i % A);
     const int cell = (int)((i / A) % ((long long)H * W));
-    const int col = cell % W, row = cell / W;
     const float2 t = pred_xy[i], u = pred_wh[i];
-    float2 o;
-    o.x = __fdiv_rn(__fadd_rn(sigmoidf_ref(t.x), (float)col), (float)W);
-    o.y = __fdiv_rn(__fadd_rn(sigmoidf_ref(t.y), (float)row), (float)H);
-    xy[i] = o;
-    o.x = __fmul_rn(exp_cr(u.x), anc.wh[2 * a]);
-    o.y = __fmul_rn(exp_cr(u.y), anc.wh[2 * a + 1]);
-    wh[i] = o;
+    const float4 o = xywh_to_all(sigmoidf_ref(t.x), sigmoidf_ref(t.y), exp_cr(u.x), exp_cr(u.y), cell % W, cell / W, W, H,
+                                 anc.wh[2 * a], anc.wh[2 * a + 1]);
+    xy[i] = make_float2(o.x, o.y);
+    wh[i] = make_float2(o.z, o.w);
 }
 
 // correct_box (keras_inference.py:32-72): (xy, wh) relative to the letterboxed input -> (ymin, xmin, ymax, xmax) in pixels
@@ -976,20 +951,8 @@ __global__ void __launch_bounds__(256) correct_box_kernel(const float2 *__restri
                                                           float img_h, float img_w) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return;
-    const float r = fminf(__fdiv_rn(in_h, img_h), __fdiv_rn(in_w, img_w));
-    const float new_h = rintf(__fmul_rn(img_h, r)), new_w = rintf(__fmul_rn(img_w, r));
-    const float off_y = __fdiv_rn(__fdiv_rn(__fsub_rn(in_h, new_h), 2.0f), in_h);
-    const float off_x = __fdiv_rn(__fdiv_rn(__fsub_rn(in_w, new_w), 2.0f), in_w);
-    const float sc_y = __fdiv_rn(in_h, new_h), sc_x = __fdiv_rn(in_w, new_w);
-    const float2 c = xy[i], s2 = wh[i];
-    const float cy = __fmul_rn(__fsub_rn(c.y, off_y), sc_y), cx = __fmul_rn(__fsub_rn(c.x, off_x), sc_x);
-    const float hh2 = __fdiv_rn(__fmul_rn(s2.y, sc_y), 2.0f), ww2 = __fdiv_rn(__fmul_rn(s2.x, sc_x), 2.0f);
-    float4 o;
-    o.x = __fmul_rn(__fsub_rn(cy, hh2), img_h);
-    o.y = __fmul_rn(__fsub_rn(cx, ww2), img_w);
-    o.z = __fmul_rn(__fadd_rn(cy, hh2), img_h);
-    o.w = __fmul_rn(__fadd_rn(cx, ww2), img_w);
-    boxes[i] = o;
+    const float2 c = xy[i], s = wh[i];
+    boxes[i] = to_corners(letterbox(in_h, in_w, img_h, img_w), make_float4(c.x, c.y, s.x, s.y));
 }
 
 // tf.image.non_max_suppression(boxes, scores, max_output_size, iou_threshold) (score_threshold = -inf): one warp sorts
@@ -1013,7 +976,7 @@ __global__ void __launch_bounds__(32) nms_boxes_kernel(const float4 *__restrict_
         float area;
         const float4 c = norm_box(boxes[idx], area);
         bool hit = false;
-        for (int j = lane; j < nsel; j += 32) hit = hit || iou_norm_gt(c, area, kept[j], kept_area[j], thr);
+        for (int j = lane; j < nsel; j += 32) hit = hit || iou_norm_gt_eo(c, area, kept[j], kept_area[j], thr);
         if (!__any_sync(FULL, hit)) {
             if (lane == 0) {
                 kept[nsel] = c;
@@ -1155,13 +1118,13 @@ extern "C" int k2y_detect_keras_strided(const k2y_detect_cfg *cfg, const float *
     p.alive_stride = (int)L.alive_stride;
     const size_t scan_smem = (size_t)SCAN_BOXES * (5 + p.C + 2) * sizeof(float);
     p.c_magic = (unsigned)((0x100000000ull + (unsigned long long)p.C - 1ull) / (unsigned long long)p.C);
-    const size_t nms_smem = std::max((size_t)p.cap * 24, CHUNK_SMEM);  // keys + decoded boxes | the chunked path's tables
+    const size_t nms_smem = std::max((size_t)p.cap * 24, CHUNK_SMEM_BYTES);  // keys + decoded boxes | the chunked tier's tables
     int dev = 0;
     K2Y_CUDA_CHECK(cudaGetDevice(&dev));
     static bool attr_set[64] = {false};  // per device: opt-in shared memory is a per-device function attribute
     if (dev >= 0 && dev < 64 && !attr_set[dev]) {
-        K2Y_CUDA_CHECK(cudaFuncSetAttribute(detect_nms_kernel<512, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, NMS_SMEM_CAP * 24));
-        K2Y_CUDA_CHECK(cudaFuncSetAttribute(detect_nms_kernel<512, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, NMS_SMEM_CAP * 24));
+        K2Y_CUDA_CHECK(cudaFuncSetAttribute(detect_nms_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, NMS_SMEM_CAP * 24));
+        K2Y_CUDA_CHECK(cudaFuncSetAttribute(detect_nms_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, NMS_SMEM_CAP * 24));
         K2Y_CUDA_CHECK(cudaFuncSetAttribute(detect_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
         attr_set[dev] = true;
     }
@@ -1174,8 +1137,8 @@ extern "C" int k2y_detect_keras_strided(const k2y_detect_cfg *cfg, const float *
     dim3 sgrid((p.nbox + SCAN_BOXES - 1) / SCAN_BOXES, batch);
     detect_scan_kernel<<<sgrid, SCAN_THREADS, scan_smem, st>>>(p);  // follows a memset: plain stream order
     K2Y_CUDA_CHECK(cudaGetLastError());
-    if (p.cap <= 2048) launch_k(detect_nms_kernel<512, 4>, dim3(p.C, batch), dim3(512), nms_smem, st, p);
-    else launch_k(detect_nms_kernel<512, 8>, dim3(p.C, batch), dim3(512), nms_smem, st, p);
+    if (p.cap <= 2048) launch_k(detect_nms_kernel<4>, dim3(p.C, batch), dim3(NMS_THREADS), nms_smem, st, p);
+    else launch_k(detect_nms_kernel<8>, dim3(p.C, batch), dim3(NMS_THREADS), nms_smem, st, p);
     K2Y_CUDA_CHECK(cudaGetLastError());
     return K2Y_OK;
 }

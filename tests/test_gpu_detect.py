@@ -7,7 +7,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-from k210_yolo_framework_b200 import KerasDetector, RegionDetector, _lib
+from k210_yolo_framework_b200 import Helper, KerasDetector, RegionDetector, _lib, ops
 from oracle import decode_ref, region_c
 
 
@@ -45,7 +45,7 @@ def test_dog_golden_heads(dog_heads, voc_anchors, dog_u8, dog_golden):
 
 @pytest.mark.parametrize("seed,batch,classes,out_hw,in_hw,obj,iou,sigma,shift", [
     (0, 4, 20, [7, 10, 14, 20], [224, 320], 0.7, 0.5, 2.0, 0.0),
-    (1, 3, 20, [7, 10, 14, 20], [224, 320], 0.5, 0.3, 2.0, 1.0),      # many candidates per class (> 32 -> memory sort)
+    (1, 3, 20, [7, 10, 14, 20], [224, 320], 0.5, 0.3, 2.0, 1.0),      # many candidates per class, > 60 detections in an image
     (2, 2, 20, [13, 13, 26, 26], [416, 416], 0.6, 0.45, 2.5, 0.5),    # tiny_yolo geometry
     (3, 2, 80, [3, 3, 6, 6, 12, 12], [96, 96], 0.4, 0.5, 2.0, 1.5),   # 3 layers / 80 classes, NMS stress: cap of 30 binds
     (4, 2, 5, [2, 3, 4, 6], [64, 96], 0.999, 0.5, 1.0, 0.0),          # nothing passes
@@ -77,7 +77,8 @@ def test_seeded_heads_bit_identical_sets(seed, batch, classes, out_hw, in_hw, ob
 
 
 def test_more_candidates_than_shared_memory_holds(voc_anchors):
-    """One class with > 4096 candidates: the NMS kernel sorts the keys in global memory and keeps the liveness bits there."""
+    """One class with > 4096 candidates: the NMS kernel runs its global-memory rounds, reading keys and boxes from global
+    memory and keeping the liveness bits there."""
     rng = np.random.default_rng(11)
     out_hw = np.array([[40, 40], [80, 80]])
     classes, batch = 2, 2
@@ -97,6 +98,76 @@ def test_more_candidates_than_shared_memory_holds(voc_anchors):
                                         [1280, 1280], img_hw[0])[1] >= 0.5).sum(0).max()]
     assert n_cand[0] > 4096
     _compare(got, ref)
+
+
+def _nms_tier(n, maxk, nbox):
+    """The NMS tier detect_nms_kernel runs for a class with n candidates; cap = candidates its shared memory holds."""
+    cap = min(-(-nbox // 256) * 256, 4096)
+    if n <= 256 and maxk <= 64:
+        return "chunked"
+    if n <= cap:
+        return "rounds4" if cap <= 2048 else "rounds8"
+    return "global"
+
+
+@pytest.mark.parametrize("tier,out_hw,n,maxk", [
+    ("chunked", [[8, 8], [16, 16]], 256, 64),      # nbox 960, cap 1024
+    ("rounds4", [[8, 8], [16, 16]], 256, 65),      # max_per_class > 64 sends a chunk-sized class to the rounds
+    ("rounds4", [[8, 8], [16, 16]], 257, 30),
+    ("rounds4", [[8, 8], [16, 16]], 257, 300),     # max_per_class does not bind
+    ("rounds8", [[16, 16], [32, 32]], 2049, 30),   # nbox 3840 = cap
+    ("rounds8", [[16, 16], [32, 32]], 3840, 30),
+    ("global", [[20, 20], [40, 40]], 4097, 30),    # nbox 6000, cap 4096
+])
+def test_every_nms_tier(tier, out_hw, n, maxk, voc_anchors):
+    """Exactly n candidates in one class put that class in the intended tier; its survivors equal the oracle's."""
+    rng = np.random.default_rng(n * 1000 + maxk)
+    classes, cls, in_hw = 3, 1, [256, 256]
+    out_hw = np.array(out_hw)
+    nbox = int(sum(h * w * 3 for h, w in out_hw))
+    assert _nms_tier(n, maxk, nbox) == tier
+    logits = np.full((nbox, classes), -8.0, np.float32)
+    logits[rng.choice(nbox, n, replace=False), cls] = 4.0 + rng.uniform(0.0, 0.5, n)   # score ~0.98, distinct
+    heads, off = [], 0
+    for h, w in out_hw:
+        t = np.empty((1, h, w, 3, 5 + classes), np.float32)
+        t[..., 0:2] = rng.normal(0, 1.0, (1, h, w, 3, 2))
+        t[..., 2:4] = rng.normal(0, 0.5, (1, h, w, 3, 2))
+        t[..., 4] = 8.0
+        t[..., 5:] = logits[off:off + h * w * 3].reshape(1, h, w, 3, classes)
+        off += h * w * 3
+        heads.append(t.reshape(1, h, w, -1))
+    img_hw = np.array([[480, 640]], np.float32)
+    hr = decode_ref.HelperRef(voc_anchors, in_hw, out_hw, classes)
+    scores = decode_ref.decode_layers([hd[0].reshape(hd.shape[1], hd.shape[2], 3, 5 + classes) for hd in heads], hr, in_hw,
+                                      img_hw[0])[1]
+    assert list((scores >= 0.5).sum(0)) == [0, n, 0]
+    det = KerasDetector(voc_anchors, in_hw, out_hw, classes, 0.5, 0.45, max_per_class=maxk, max_batch=1)
+    got = KerasDetector.to_host(*det.run([torch.from_numpy(t).cuda() for t in heads], img_hw))
+    ref = _oracle_keras(heads, voc_anchors, in_hw, out_hw, classes, img_hw, 0.5, 0.45, maxk)
+    _compare(got, ref)
+    assert 0 < len(ref[0]) < n    # boxes were suppressed
+
+
+def test_operators_give_the_fused_kernel_bits(voc_anchors):
+    """ops.tf_xywh_to_all + ops.correct_box give every box the fused kernel records, bit for bit."""
+    rng = np.random.default_rng(7)
+    in_hw, out_hw, classes = [224, 320], [[7, 10], [14, 20]], 20
+    heads = [rng.normal(0.5, 2.0, (2, h, w, 3, 5 + classes)).astype(np.float32) for h, w in out_hw]
+    img_hw = np.array([[374, 499], [480, 640]], np.float32)
+    det = KerasDetector(voc_anchors, in_hw, out_hw, classes, 0.6, 0.5, max_batch=2)
+    got = KerasDetector.to_host(*det.run([torch.from_numpy(t).cuda() for t in heads], img_hw))
+    helper = Helper(None, classes, voc_anchors, [in_hw] * 2, out_hw)
+    for b in range(2):
+        boxes = []
+        for layer, t in enumerate(heads):
+            y = torch.from_numpy(t[b]).cuda()
+            xy, wh = ops.tf_xywh_to_all(y[..., 0:2], y[..., 2:4], layer, helper)
+            boxes.append(ops.correct_box(xy, wh, in_hw, img_hw[b]).reshape(-1, 4))
+        boxes = torch.cat(boxes).cpu().numpy()     # box-index order: layer 0 first, then [row][col][anchor]
+        assert len(got[b]) > 20
+        for rec in got[b]:
+            assert (np.array(rec[3:], np.float32).view(np.uint32) == boxes[rec[1]].view(np.uint32)).all(), rec
 
 
 def test_strided_outputs_match_dense(voc_anchors):
