@@ -92,6 +92,92 @@ def test_random_weights_all_models(model_def, alpha, classes, hw, batch, math):
         assert float(box_err.max()) < 1e-3, f"{model_def} {_lib.MATH_NAMES[math]}: normalised box error {float(box_err.max()):.2e}"
 
 
+def _record_key(model_def, name, bn, acts):
+    """The oracle record (keras_ref.forward(..., record=True)) of the tensor the engine stores as layer `name`'s output —
+    post-BN/activation, plus the block input where the layer adds one — or None when the family has no such layer."""
+    if model_def == "yolo_mobilev1" and (name.startswith(("conv_dw_", "conv_pw_")) or name == "conv1"):
+        return name + "_relu"
+    if model_def == "yolo_mobilev2":
+        if name == "Conv1":
+            return "Conv1_relu"
+        if name == "Conv_1":
+            return "out_relu"
+        if name.endswith(("_expand", "_depthwise")):
+            return name + "_relu"
+        if name.endswith("_project"):   # linear bottleneck: BN, no activation; the residual blocks record the add
+            add = name[:-len("project")] + "add"
+            return add if add in acts else bn
+    if bn.startswith("batch_normalization"):
+        return bn + "/leaky"
+    if name.startswith("conv2d") and not bn:   # a head's output conv (with bias)
+        return name
+    return None
+
+
+def _darknet_residual_layers():
+    """Creation-order indices of Darknet-53's residual 3x3 convs (the engine adds the block input in their epilogue; the
+    oracle records only the conv branch)."""
+    i, out = 1, []
+    for blocks in (1, 2, 8, 8, 4):
+        i += 1                   # the stride-2 downsample conv
+        for _ in range(blocks):
+            out.append(i + 1)    # the block's 1x1, then its 3x3
+            i += 2
+    return out
+
+
+LAYERWISE = [("yolo_mobilev2", 1.0, 20, (224, 320), 2), ("yolo_mobilev2", 0.5, 20, (96, 96), 2),
+             ("tiny_yolo", 1.0, 20, (160, 160), 2), ("yolo", 1.0, 80, (96, 96), 2)]
+_LAYERWISE_ORACLE = {}   # (case) -> (weights, input, oracle records) of the case last run; the math mode varies fastest
+
+
+@pytest.mark.parametrize("math", MODES)
+@pytest.mark.parametrize("model_def,alpha,classes,hw,batch", LAYERWISE)
+def test_random_weights_layerwise(model_def, alpha, classes, hw, batch, math):
+    """Every layer of the other families against the fp64 oracle, so that an error in a depthwise (stride 1 and 2, odd
+    maps), max-pool (stride 1 and 2), pixel-pair 1x1, residual or concat/upsample layer shows at that layer."""
+    m, _ = getattr(yolonet, model_def)([hw[0], hw[1], 3], 3, classes, alpha=alpha, max_batch=batch)
+    m.engine.set_keep_all(True)
+    m.engine.set_use_graph(False)
+    key = (model_def, alpha, classes, hw, batch)
+    if key not in _LAYERWISE_ORACLE:      # the fp64 oracle of a network runs once for its three math modes
+        _LAYERWISE_ORACLE.clear()
+        weights = random_weights(m.engine.expected_variables(), seed=7, detection_rich=True)
+        x = np.random.default_rng(11).random((batch, hw[0], hw[1], 3), dtype=np.float32)
+        _, acts = keras_ref.forward(model_def, weights, x.astype(np.float64), alpha=alpha, dtype=torch.float64, record=True)
+        _LAYERWISE_ORACLE[key] = weights, x, acts
+    weights, x, acts = _LAYERWISE_ORACLE[key]
+    m.set_weights_dict(weights)
+    m.engine.set_math(math)
+    m.predict(x)
+    layers = m.engine.layers()
+    residual = set(_darknet_residual_layers()) if model_def == "yolo" else set()
+    refs = []
+    for i, L in enumerate(layers):
+        name, bn = L.name.decode(), L.bn_name.decode()
+        key = _record_key(model_def, name, bn, acts)
+        assert key in acts, f"{model_def}: no oracle record for layer {name} (bn '{bn}')"
+        ref = acts[key].permute(0, 2, 3, 1).numpy()
+        if i in residual:
+            assert L.kh == 3 and layers[i - 1].kh == 1 and L.cout == layers[i - 1].cin, name
+            ref = ref + refs[i - 2]      # the input of the block's 1x1
+        refs.append(ref)
+        got = m.engine.read_layer(name, batch)
+        assert got.shape == ref.shape, name
+        err = _maxerr(got, ref) / max(1.0, float(np.abs(ref).max()))
+        assert err < LAYER_TOL[math], f"{model_def} {name}: rel-to-max error {err:.3e} ({_lib.MATH_NAMES[math]})"
+    if model_def == "tiny_yolo":
+        # the max-pools (not in layers()): 2x2 'SAME' over the first six convs' outputs, the last with stride 1
+        tape = keras_ref._Tape(weights, torch.float64)
+        for k, stride in enumerate((2, 2, 2, 2, 2, 1)):
+            sfx = f"_{k}" if k else ""
+            ref = tape.maxpool_same(acts[f"batch_normalization{sfx}/leaky"], stride).permute(0, 2, 3, 1).numpy()
+            got = m.engine.read_layer(f"max_pooling2d{sfx}", batch)
+            assert got.shape == ref.shape, f"max_pooling2d{sfx}"
+            err = _maxerr(got, ref) / max(1.0, float(np.abs(ref).max()))
+            assert err < LAYER_TOL[math], f"max_pooling2d{sfx}: rel-to-max error {err:.3e} ({_lib.MATH_NAMES[math]})"
+
+
 def test_device_api_graph_replay_and_batching():
     m, _ = yolonet.yolo_mobilev1([224, 320, 3], 3, 20, alpha=0.75, max_batch=4)
     weights = random_weights(m.engine.expected_variables(), seed=5, detection_rich=True)
