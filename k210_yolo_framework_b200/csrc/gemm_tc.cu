@@ -14,7 +14,11 @@
 //                            recovers fp32-class accuracy from the tensor cores; B comes from shared memory.  A k-block's
 //                            MMAs are one committed wgmma group; while it runs, the next k-block's A is read and split
 //                            into a second fragment buffer, and a stage is released once its group has completed.  After
-//                            the last k-block of a tile they apply folded BN, activation and residual and store to HBM.
+//                            the last k-block of a tile they apply folded BN, activation and residual and store to HBM:
+//                            in the plain 1x1 kernels through two 8 KB shared-memory chunk buffers per warpgroup and TMA
+//                            stores, which drain while the warpgroup moves on to the next tile's MMAs (the register
+//                            epilogue remains where the output is no legal tensor map: N % 4 != 0 or an unaligned dst);
+//                            in the gather kernels with direct global stores from the accumulator registers.
 // mbarrier ring per stage: full_b (TMA tx) / full_a (cp.async arrivals) -> [consumers] -> empty.
 //
 // Replaces the TF Conv2D + FusedBatchNorm + LeakyRelu/Relu6 (+ ResizeNearestNeighbor/ConcatV2/Add) ops that
@@ -55,6 +59,7 @@ struct TcParams {
     int BN, n_tiles, m_tiles, nkb, stages;
     int k_splits, kb_per_split;     // split-K: work item = (m-tile, n-tile, k-slice); partials go to a scratch buffer
     int partial;                    // 1: raw accumulators to dst (split-K scratch, row pitch N, rows of slice ks at ks * m_tiles * 128)
+    int tma_store;                  // plain 1x1: results leave through shared-memory chunks and TMA stores (map_c / map_c16)
     int half_taps;                  // gather: Cin is half a k-block (16 with tf32, 32 with bf16 k-blocks), a k-block holds TWO consecutive taps
     float act_slope, act_clamp;     // branch-free activation parameters
 };
@@ -64,6 +69,10 @@ struct __align__(8) Barriers {
 };
 // dynamic smem besides the stage ring: alignment slack + barriers
 constexpr size_t FIXED_SMEM = 1024 + 1024;
+// TMA-A (plain 1x1) kernels also hold the output staging: per consumer warpgroup two buffers of one 64-row x 32-column fp32
+// chunk (8 KB each), written by the warpgroup while TMA stores the other one
+constexpr int CHUNK_BYTES = 64 * 32 * 4;
+constexpr size_t STAGING_SMEM = 2 * 2 * CHUNK_BYTES;
 
 // one fp32 element of the 128B-swizzled A sub-tile: row r, column k (0..31)
 __device__ __forceinline__ uint32_t a_addr(uint32_t box, int r, int k) {
@@ -130,11 +139,14 @@ __device__ __forceinline__ void mma_ksteps(float (&acc)[BNT / 2], const uint32_t
 
 // BNT = the tile width p.BN and MODE = the math mode (K2Y_MATH_TC_*), compile-time constants so that every accumulator
 // register and every wgmma of the consumers is fixed at compile time and a k-block's MMAs are one branch-free batch (a
-// runtime-sliced accumulator made ptxas serialise the wgmma pipeline; a runtime mode test split the batch into groups)
-template <bool GATHER, int BNT, int MODE>
+// runtime-sliced accumulator made ptxas serialise the wgmma pipeline; a runtime mode test split the batch into groups).
+// STAGED (plain 1x1 only) selects the shared-memory + TMA-store epilogue; a runtime choice between the two epilogues made
+// several consumer instantiations spill.
+template <bool GATHER, int BNT, int MODE, bool STAGED>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_bhi,
-               const __grid_constant__ CUtensorMap map_blo, const TcParams p) {
+               const __grid_constant__ CUtensorMap map_blo, const __grid_constant__ CUtensorMap map_c,
+               const __grid_constant__ CUtensorMap map_c16, const TcParams p) {
     constexpr bool BF16 = MODE == K2Y_MATH_TC_BF16X3;       // operands are bf16 (hi, mid) planes, 64 k per k-block
     constexpr bool THREE_X = MODE != K2Y_MATH_TC_TF32;      // split scheme: 3 MMAs per k-step; else one tf32 pass, 32 k per k-block
     constexpr int A_BOXES = BF16 ? 2 : 1;                   // 16 KB sub-tiles of raw fp32 A per stage
@@ -142,13 +154,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     constexpr int KSTEP = BF16 ? 16 : 8;                    // k values per wgmma
     static_assert(KBK / KSTEP == 4, "a k-block is four k-steps");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [stages] x { A (raw fp32) A_BOXES x 16K | B_hi BN*128 | B_lo BN*128 (3x) }, then barriers
+    // carve: [stages] x { A (raw fp32) A_BOXES x 16K | B_hi BN*128 | B_lo BN*128 (3x) }, output staging (TMA A only), barriers
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     const uint32_t b_bytes = (uint32_t)p.BN * 128u;
     const uint32_t a_bytes = (uint32_t)A_TILE_BYTES * (uint32_t)A_BOXES;
     const uint32_t stage_bytes = a_bytes + b_bytes * (THREE_X ? 2u : 1u);
+    const uint32_t stage_c = smem_base + (uint32_t)p.stages * stage_bytes;  // 1024-aligned: stage_bytes is a multiple of 2 KB
     uint8_t *smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-    Barriers *bars = reinterpret_cast<Barriers *>(smem_gen + (size_t)p.stages * stage_bytes);
+    Barriers *bars = reinterpret_cast<Barriers *>(smem_gen + (size_t)p.stages * stage_bytes + (GATHER ? 0 : STAGING_SMEM));
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     pdl_trigger();
 
@@ -160,6 +173,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         }
         fence_barrier_init();
         if (!GATHER) prefetch_tmap(&map_a);
+        if (STAGED) prefetch_tmap(&map_c);
         prefetch_tmap(&map_bhi);
         if (THREE_X) prefetch_tmap(&map_blo);
     }
@@ -342,6 +356,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         __syncwarp();
         if (lane == 0) mbar_arrive(smem_u32(&bars->empty[stage]));
     };
+    // staged epilogue: one thread of the warpgroup issues (and waits for) its TMA stores
+    const bool lead = (threadIdx.x & 127) == 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         const int ks = t % p.k_splits, tt = t / p.k_splits;
         const int mt = tt / p.n_tiles, nt = tt - mt * p.n_tiles;
@@ -382,6 +398,59 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         }
 #pragma unroll
         for (int i = 0; i < BNT / 2; ++i) reg_fence(acc[i]);
+        if constexpr (STAGED) {
+            // ---- staged epilogue: folded BN + activation (+ residual), or the raw split-K partial, one 64-row x 32-column
+            // chunk of the warpgroup's rows at a time into a staging buffer, then one TMA store per chunk.  TMA clips rows >= M
+            // and columns >= N.  The stores run on while the warpgroup fills the other buffer and then starts the next tile's
+            // MMAs; before a buffer is rewritten, the store that read it has finished (wait_group.read before the barrier of
+            // the chunk in between).  A tile width that is an odd multiple of 16 ends with a 16-column chunk (map_c16).
+            const int row0 = (p.partial ? ks * p.m_tiles * BM : 0) + mt * BM + cg * 64;
+            constexpr int CHUNKS = (BNT + 31) / 32;
+            // chunks this warpgroup stored before this tile: the staging buffers alternate over them (derived from t rather
+            // than counted, which kept one more register live through the mainloop)
+            const uint32_t chunk0 = (uint32_t)(t - (int)blockIdx.x) / gridDim.x * (uint32_t)CHUNKS;
+#pragma unroll
+            for (int j = 0; j < CHUNKS; ++j) {
+                const bool full = 32 * j + 32 <= BNT;
+                const uint32_t buf = stage_c + (uint32_t)(cg * 2 + ((chunk0 + j) & 1u)) * CHUNK_BYTES;
+                // (a half-warp's 8-byte stores hit each bank twice; trading column groups between threads to avoid that
+                // made the bn-96 bf16x3 consumers spill)
+#pragma unroll
+                for (int q = 0; q < (full ? 4 : 2); ++q) {
+                    const int c = 4 * j + q;  // accumulator column group
+                    const int n = nt * BNT + 8 * c + 2 * tq;
+                    float sc0 = 0.f, sh0 = 0.f, sc1 = 0.f, sh1 = 0.f;
+                    if (!p.partial && n < p.N) {  // N % 4 == 0: n + 1 < N too
+                        sc0 = __ldg(p.scale + n), sh0 = __ldg(p.shift + n);
+                        sc1 = __ldg(p.scale + n + 1), sh1 = __ldg(p.shift + n + 1);
+                    }
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        float o0 = acc[4 * c + 2 * h], o1 = acc[4 * c + 2 * h + 1];
+                        const int row = wq * 16 + g + 8 * h;  // inside the warpgroup's 64 rows
+                        if (!p.partial) {
+                            o0 = act_bf(fmaf(o0, sc0, sh0), p.act_slope, p.act_clamp);
+                            o1 = act_bf(fmaf(o1, sc1, sh1), p.act_slope, p.act_clamp);
+                            const int mloc = mt * BM + cg * 64 + row;
+                            if (p.residual && mloc < p.M && n < p.N) {
+                                const float2 rr = __ldg(reinterpret_cast<const float2 *>(p.residual + (size_t)mloc * p.N + n));
+                                o0 += rr.x, o1 += rr.y;
+                            }
+                        }
+                        const int col = 8 * q + 2 * tq;
+                        st_shared_v2(full ? a_addr(buf, row, col) : buf + (uint32_t)(row * 64 + col * 4), o0, o1);
+                    }
+                }
+                fence_proxy_async_smem();
+                if (lead) bulk_wait_group_0<true>();
+                named_bar_sync(1 + cg, 128);
+                if (lead) {
+                    tma_store_2d(full ? &map_c : &map_c16, buf, nt * BNT + 32 * j, row0);
+                    bulk_commit_group();
+                }
+            }
+            continue;
+        }
         // ---- epilogue: folded BN + activation (+ residual) straight from the accumulator registers ----
         const int n_base = nt * BNT + 2 * tq;
         if (p.partial) {
@@ -433,6 +502,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             }
         }
     }
+    // the outputs are complete before the CTA exits (and before a PDL successor reads them)
+    if (STAGED && lead) bulk_wait_group_0<false>();
 }
 
 // Split-K reduction + epilogue: out[m,n] = act(scale[n] * sum_s partial[s][m][n] + shift[n]) (+ residual).
@@ -497,6 +568,21 @@ bool make_map_2d(CUtensorMap *map, const void *base, uint64_t rows, uint64_t col
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(base), dims,
                      strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    return r == CUDA_SUCCESS;
+}
+
+// fp32 output [rows][cols] of the staged epilogue (row pitch cols, a multiple of 4): box = 64 rows x box_cols, 128B
+// swizzle for the 32-column chunks (the staging layout), none for the 16-column ones
+bool make_out_map(CUtensorMap *map, void *base, uint64_t rows, uint64_t cols, uint32_t box_cols) {
+    EncodeTiledFn enc = get_encode();
+    if (!enc) return false;
+    cuuint64_t dims[2] = {cols, rows};
+    cuuint64_t strides[1] = {cols * 4};
+    cuuint32_t box[2] = {box_cols, 64};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS;
 }
@@ -567,8 +653,10 @@ int budget_sms(int sm_limit) {
 size_t stage_bytes_of(int bn, bool three_x, bool bf16) {
     return (size_t)A_TILE_BYTES * (bf16 ? 2 : 1) + (size_t)bn * 128 * (three_x ? 2 : 1);
 }
-int stages_for(int bn, bool three_x, bool bf16) {
-    int st = (int)(((g_max_smem ? g_max_smem : DEFAULT_SMEM) - FIXED_SMEM) / stage_bytes_of(bn, three_x, bf16));
+// shared memory besides the stage ring: the plain 1x1 (TMA A) kernels also hold the output staging
+size_t fixed_smem_of(bool gather) { return FIXED_SMEM + (gather ? 0 : STAGING_SMEM); }
+int stages_for(int bn, bool three_x, bool bf16, bool gather) {
+    int st = (int)(((g_max_smem ? g_max_smem : DEFAULT_SMEM) - fixed_smem_of(gather)) / stage_bytes_of(bn, three_x, bf16));
     return st > MAX_STAGES ? MAX_STAGES : st;
 }
 
@@ -582,7 +670,7 @@ void pick_tile(int M, int N, int nkb, bool three_x, bool bf16, bool gather, size
     double best_cost = 1e30;
     for (int bn = 16; bn <= MAX_BN; bn += 16) {
         if (bn > n16) break;
-        const int stages = stages_for(bn, three_x, bf16);
+        const int stages = stages_for(bn, three_x, bf16, gather);
         if (stages < 2) continue;
         const int n_tiles = (n16 + bn - 1) / bn;
         // per k-block (32 k for tf32, 64 k for bf16): tensor time (a 64 x bn x 8 tf32 or 64 x bn x 16 bf16 wgmma per warpgroup
@@ -616,30 +704,30 @@ void pick_tile(int M, int N, int nkb, bool three_x, bool bf16, bool gather, size
     *splits_out = best_s;
 }
 
-using ConvKernel = decltype(&conv_tc_kernel<false, 16, K2Y_MATH_TC_TF32>);
+using ConvKernel = decltype(&conv_tc_kernel<false, 16, K2Y_MATH_TC_TF32, false>);
 
 // the instantiation for tile width bn (a multiple of 16 up to MAX_BN)
-template <bool G, int MODE>
+template <bool G, bool S, int MODE>
 ConvKernel conv_kernel_bn(int bn) {
     switch (bn) {
-        case 16: return conv_tc_kernel<G, 16, MODE>;
-        case 32: return conv_tc_kernel<G, 32, MODE>;
-        case 48: return conv_tc_kernel<G, 48, MODE>;
-        case 64: return conv_tc_kernel<G, 64, MODE>;
-        case 80: return conv_tc_kernel<G, 80, MODE>;
-        case 96: return conv_tc_kernel<G, 96, MODE>;
-        case 112: return conv_tc_kernel<G, 112, MODE>;
-        case 128: return conv_tc_kernel<G, 128, MODE>;
+        case 16: return conv_tc_kernel<G, 16, MODE, S>;
+        case 32: return conv_tc_kernel<G, 32, MODE, S>;
+        case 48: return conv_tc_kernel<G, 48, MODE, S>;
+        case 64: return conv_tc_kernel<G, 64, MODE, S>;
+        case 80: return conv_tc_kernel<G, 80, MODE, S>;
+        case 96: return conv_tc_kernel<G, 96, MODE, S>;
+        case 112: return conv_tc_kernel<G, 112, MODE, S>;
+        case 128: return conv_tc_kernel<G, 128, MODE, S>;
         default: return nullptr;
     }
 }
 // the instantiation for a gather / TMA A operand, a tensor-core math mode (K2Y_MATH_TC_*) and tile width bn
-template <bool G>
+template <bool G, bool S>
 ConvKernel conv_kernel_for(int mode, int bn) {
     switch (mode) {
-        case K2Y_MATH_TC_TF32: return conv_kernel_bn<G, K2Y_MATH_TC_TF32>(bn);
-        case K2Y_MATH_TC_3XTF32: return conv_kernel_bn<G, K2Y_MATH_TC_3XTF32>(bn);
-        case K2Y_MATH_TC_BF16X3: return conv_kernel_bn<G, K2Y_MATH_TC_BF16X3>(bn);
+        case K2Y_MATH_TC_TF32: return conv_kernel_bn<G, S, K2Y_MATH_TC_TF32>(bn);
+        case K2Y_MATH_TC_3XTF32: return conv_kernel_bn<G, S, K2Y_MATH_TC_3XTF32>(bn);
+        case K2Y_MATH_TC_BF16X3: return conv_kernel_bn<G, S, K2Y_MATH_TC_BF16X3>(bn);
         default: return nullptr;
     }
 }
@@ -658,9 +746,11 @@ int tc_init() {
     K2Y_CUDA_CHECK(cudaGetDeviceProperties(&prop, dev));
     for (int mode : TC_MODES)
         for (int bn = 16; bn <= MAX_BN; bn += 16) {
-            K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<false>(mode, bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
+            K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<false, false>(mode, bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                 (int)prop.sharedMemPerBlockOptin));
-            K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<true>(mode, bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
+            K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<false, true>(mode, bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                (int)prop.sharedMemPerBlockOptin));
+            K2Y_CUDA_CHECK(cudaFuncSetAttribute(conv_kernel_for<true, false>(mode, bn), cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                 (int)prop.sharedMemPerBlockOptin));
         }
     if (g_num_sms == 0) {
@@ -769,7 +859,7 @@ static TcPlan plan_conv(const ConvArgs &a, int K, int math_mode) {
     pick_tile(M, a.N, pl.nkb, three_x, bf, pl.gather, a.tc_scratch ? a.tc_scratch_bytes : 0, sms, &pl.bn, &pl.k_splits);
     pl.kb_per_split = (pl.nkb + pl.k_splits - 1) / pl.k_splits;
     pl.k_splits = (pl.nkb + pl.kb_per_split - 1) / pl.kb_per_split;  // no empty slices
-    pl.stages = stages_for(pl.bn, three_x, bf);
+    pl.stages = stages_for(pl.bn, three_x, bf, pl.gather);
     pl.m_tiles = (M + BM - 1) / BM;
     pl.n_tiles = ((a.N + 15) / 16 * 16 + pl.bn - 1) / pl.bn;
     const int tiles = pl.m_tiles * pl.n_tiles * pl.k_splits;
@@ -817,10 +907,12 @@ cudaError_t launch_conv_tc(const ConvArgs &a, const TcWeights &w, int math_mode,
     p.k_splits = pl.k_splits;
     p.stages = pl.stages;
     if (p.stages < 2) return cudaErrorInvalidConfiguration;
-    const size_t smem = FIXED_SMEM + (size_t)p.stages * stage_bytes_of(p.BN, three_x, bf16);
+    const size_t smem = fixed_smem_of(pl.gather) + (size_t)p.stages * stage_bytes_of(p.BN, three_x, bf16);
 
-    CUtensorMap map_a, map_bhi, map_blo;
+    CUtensorMap map_a, map_bhi, map_blo, map_c, map_c16;
     memset(&map_a, 0, sizeof(map_a));
+    memset(&map_c, 0, sizeof(map_c));
+    memset(&map_c16, 0, sizeof(map_c16));
     const size_t mpad = (size_t)p.m_tiles * BM;
     float *scratch = a.tc_scratch;
     if (p.k_splits > 1) {
@@ -838,6 +930,14 @@ cudaError_t launch_conv_tc(const ConvArgs &a, const TcWeights &w, int math_mode,
         p.residual = nullptr;
     }
     if (!pl.gather && !make_map_2d(&map_a, a.src0, (uint64_t)p.M, (uint64_t)(a.C0 + a.C1), BM)) return cudaErrorInvalidValue;
+    // plain 1x1: TMA stores of the output (or of the split-K partials, whose scratch always qualifies) where the output is a
+    // legal tensor map — 16-byte row pitch and base; otherwise (the 75-channel head outputs) the register epilogue
+    p.tma_store = !pl.gather && (p.partial || ((a.N & 3) == 0 && ((uintptr_t)a.dst & 15) == 0)) ? 1 : 0;
+    if (p.tma_store) {
+        const uint64_t rows = p.partial ? (uint64_t)p.k_splits * mpad : (uint64_t)p.M;
+        if (!make_out_map(&map_c, p.dst, rows, (uint64_t)p.N, 32) || !make_out_map(&map_c16, p.dst, rows, (uint64_t)p.N, 16))
+            return cudaErrorInvalidValue;
+    }
     if (bf16) {
         if (!make_map_2d(&map_bhi, w.d_bh, (uint64_t)w.Npad, (uint64_t)w.Kpad64, (uint32_t)p.BN, 0, true)) return cudaErrorInvalidValue;
         if (!make_map_2d(&map_blo, w.d_bm, (uint64_t)w.Npad, (uint64_t)w.Kpad64, (uint32_t)p.BN, 0, true)) return cudaErrorInvalidValue;
@@ -847,10 +947,12 @@ cudaError_t launch_conv_tc(const ConvArgs &a, const TcWeights &w, int math_mode,
     }
 
     // null for a tile width or math mode that has no instantiation
-    const ConvKernel kern = pl.gather ? conv_kernel_for<true>(pl.mode, p.BN) : conv_kernel_for<false>(pl.mode, p.BN);
+    const ConvKernel kern = pl.gather      ? conv_kernel_for<true, false>(pl.mode, p.BN)
+                            : p.tma_store ? conv_kernel_for<false, true>(pl.mode, p.BN)
+                                          : conv_kernel_for<false, false>(pl.mode, p.BN);
     if (!kern) return cudaErrorInvalidConfiguration;
     const dim3 g((unsigned)pl.grid), b(NUM_THREADS);
-    cudaError_t le = launch_k(kern, g, b, smem, st, map_a, map_bhi, map_blo, p);
+    cudaError_t le = launch_k(kern, g, b, smem, st, map_a, map_bhi, map_blo, map_c, map_c16, p);
     if (le != cudaSuccess) return le;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;

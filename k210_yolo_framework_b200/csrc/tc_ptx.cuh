@@ -52,6 +52,27 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
         "l"(map), "r"(bar), "r"(c0), "r"(c1)
         : "memory");
 }
+// shared -> global tensor store of one box, tracked in the issuing thread's bulk async-group
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, uint32_t src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(src), "r"(c0),
+                 "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the issuing thread's bulk stores have finished reading shared memory (READ) or are complete and visible (otherwise)
+template <bool READ>
+__device__ __forceinline__ void bulk_wait_group_0() {
+    if (READ) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    else asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+}
+// orders this thread's generic-proxy shared-memory writes before later async-proxy (TMA) reads of them
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void st_shared_v2(uint32_t addr, float x, float y) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
