@@ -595,6 +595,14 @@ extern "C" int k2y_net_create(const char *model_def, int in_h, int in_w, float a
         set_error("k2y_net_create: unknown model_def '%s' (yolo_mobilev1|yolo_mobilev2|tiny_yolo|yolo)", model_def);
         return K2Y_ERR_INVALID;
     }
+    // the depthwise and max-pool kernels move 4 channels per float4 load and store; there is no scalar form of either
+    // (yolo_mobilev1 reaches such widths at alphas like 0.35 or 0.6: conv_dw_1 gets int(32 * alpha) channels)
+    for (const Layer &L : n->layers)
+        if ((L.kind == L_DW || L.kind == L_POOL) && L.cin % 4 != 0) {
+            set_error("k2y_net_create: %s at alpha %g has %d channels; depthwise and max-pool layers need a multiple of 4",
+                      L.name.c_str(), alpha, L.cin);
+            return K2Y_ERR_INVALID;
+        }
     plan_arena(n.get());
     *out = n.release();
     return K2Y_OK;

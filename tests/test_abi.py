@@ -42,4 +42,12 @@ def test_error_reporting_without_gpu():
     assert rc == -1 and "unknown model_def" in _lib.last_error()
     rc = _lib.lib.k2y_net_create(b"yolo_mobilev1", 225, 320, 1.0, 3, 20, 1, 0, ctypes.byref(h))
     assert rc == -1 and "multiple of 32" in _lib.last_error()
+    # depthwise widths the float4 kernel cannot run: conv_dw_1 of yolo_mobilev1 gets int(32 * alpha) channels
+    for alpha, channels in ((0.35, 11), (0.6, 19)):
+        rc = _lib.lib.k2y_net_create(b"yolo_mobilev1", 224, 320, alpha, 3, 20, 1, 0, ctypes.byref(h))
+        err = _lib.last_error()
+        assert rc == -1 and "conv_dw_1" in err and f"has {channels} channels" in err, err
+    rc = _lib.lib.k2y_net_create(b"yolo_mobilev1", 224, 320, 0.25, 3, 20, 1, 0, ctypes.byref(h))   # 8 channels: fine
+    assert rc == 0
+    _lib.lib.k2y_net_destroy(h)
     assert _lib.lib.k2y_version() >= 100
