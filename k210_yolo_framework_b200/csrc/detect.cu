@@ -124,8 +124,16 @@ __device__ __forceinline__ void warp_sort_desc_mem(unsigned long long *keys, int
 
 // tf.image.non_max_suppression's test `IoU(a, b) > thr` on (ymin,xmin,ymax,xmax) boxes (zero-area boxes -> IoU 0), without
 // the division in the common case: inter/uni > thr  <=>  inter > thr*uni (uni > 0).  The product form is only trusted
-// outside a 1e-6 relative margin (>> the 3 roundings involved); inside it the exact IEEE division decides, so the
-// boolean is bit-identical to the reference's `iou > iou_threshold`.  Boxes are (min,max)-normalised with their areas
+// outside a 1e-6 relative margin, and only where that margin argument holds: thr and t = fl(thr*uni) both normal floats
+// (>= 2^-126) and t < 2^126.  Then t and fl(t * 1.000001f) each carry one relative rounding <= 2^-24, so inter above it
+// puts the exact quotient above thr * (1 + 8e-7), past the next float after thr (a normal thr's ulp is <= 2^-23 * thr), and
+// fl(inter/uni) > thr; the lower side likewise.  Outside that range the exact IEEE division decides:
+//   - thr == +-0: inter > 0 does NOT imply fl(inter/uni) > 0 — a denormal-area box inside a large one has a quotient
+//     below 2^-150 that rounds to 0 (IoU 0, kept by the reference);
+//   - a subnormal thr or t: their rounding error is absolute (2^-150), not relative, and exceeds the margin;
+//   - uni infinite or NaN (boxes decoded from exp overflow): t is inf or NaN;
+//   - thr < 0: IoU >= 0 > thr is the division's own answer, and a NaN IoU (two infinite boxes) is not > thr.
+// So the boolean is bit-identical to the reference's `iou > iou_threshold` for every float input.  Boxes are (min,max)-normalised with their areas
 // cached (once per box instead of once per pair).  One body computes the intersection and union; two control-flow forms decide
 // the same boolean from them:
 //   iou_norm_gt     straight-line (selects, the exact division only under a rarely-taken branch).  The chunked tier tests up to
@@ -149,11 +157,14 @@ __device__ __forceinline__ float2 iou_terms(const float4 a, float area_a, const 
     const float inter = __fmul_rn(iy, ix);
     return make_float2(inter, __fsub_rn(__fadd_rn(area_a, area_b), inter));
 }
+__device__ __forceinline__ bool product_form_usable(float thr, float t) {
+    return thr >= 0x1p-126f && t >= 0x1p-126f && t < 0x1p126f;   // false for NaN
+}
 __device__ __forceinline__ bool iou_norm_gt(const float4 a, float area_a, const float4 b, float area_b, float thr) {
     const float2 iu = iou_terms(a, area_a, b, area_b);
     const float inter = iu.x, uni = iu.y;
     const float t = __fmul_rn(thr, uni);
-    const bool usable = thr >= 0.f && uni > 0.f;                       // the product form is only trusted then
+    const bool usable = product_form_usable(thr, t);
     const bool gt = usable && inter > __fmul_rn(t, 1.000001f);
     const bool lt = usable && inter < __fmul_rn(t, 0.999999f);
     bool res = gt;
@@ -165,8 +176,8 @@ __device__ __forceinline__ bool iou_norm_gt_eo(const float4 a, float area_a, con
     if (area_a <= 0.f || area_b <= 0.f) return 0.f > thr;
     const float2 iu = iou_terms(a, area_a, b, area_b);
     const float inter = iu.x, uni = iu.y;
-    if (thr >= 0.f && uni > 0.f) {
-        const float t = __fmul_rn(thr, uni);
+    const float t = __fmul_rn(thr, uni);
+    if (product_form_usable(thr, t)) {
         if (inter > __fmul_rn(t, 1.000001f)) return true;
         if (inter < __fmul_rn(t, 0.999999f)) return false;
     }
@@ -199,7 +210,9 @@ struct KerasParams {
     float in_h, in_w;
     float obj, iou;
     float logit_min;                  // a logit below this cannot give a sigmoid >= obj (with a wide margin); -inf = no shortcut
-    unsigned c_magic;                 // ceil(2^32 / C): it / C == __umulhi(it, c_magic) for the item counts of one slab
+    unsigned long long c_magic;       // ceil(2^32 / C) = (2^32 + e) / C, 0 <= e < C, up to 2^32 (C == 1): it / C == (it * c_magic) >> 32
+                                      // exactly while it * e < 2^32, i.e. for the it < 64 C items of a slab at every C < 8192 (the
+                                      // scan's shared memory takes C <= 377)
     int maxk;
     const float *image_hw;
     k2y_det *dets;
@@ -386,7 +399,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) detect_scan_kernel(const KerasPa
             sc4[u] = 0.f;
             cls[u] = bi[u] = 0;
             if (it < n_items) {
-                const int i = (int)__umulhi((unsigned)it, p.c_magic), c = it - i * p.C;
+                const int i = (int)(((unsigned long long)(unsigned)it * p.c_magic) >> 32), c = it - i * p.C;
                 const float t = s_rec[i * E + 5 + c];
                 if (!(t < s_thr[i])) {
                     const float sc = s_conf[i];
@@ -1117,7 +1130,7 @@ extern "C" int k2y_detect_keras_strided(const k2y_detect_cfg *cfg, const float *
     p.cap = L.cap;
     p.alive_stride = (int)L.alive_stride;
     const size_t scan_smem = (size_t)SCAN_BOXES * (5 + p.C + 2) * sizeof(float);
-    p.c_magic = (unsigned)((0x100000000ull + (unsigned long long)p.C - 1ull) / (unsigned long long)p.C);
+    p.c_magic = (0x100000000ull + (unsigned long long)p.C - 1ull) / (unsigned long long)p.C;
     const size_t nms_smem = std::max((size_t)p.cap * 24, CHUNK_SMEM_BYTES);  // keys + decoded boxes | the chunked tier's tables
     int dev = 0;
     K2Y_CUDA_CHECK(cudaGetDevice(&dev));
