@@ -243,10 +243,19 @@ int k2y_expf_eval(int mode, const float *x_dev, float *y_dev, long long n, void 
  * (tools/utils.py:372-400: AffineTransform(scale, translation) + skimage warp order 1, zero fill, .astype('uint8')).
  * inv_matrix_host: the first two rows of inv([[s,0,tx],[0,s,ty],[0,0,1]]) as 6 doubles (host memory) - what
  * `aff.inverse` hands to warp.  dst_dev: [dst_h][dst_w][3] uint8, ready for k2y_net_bind_u8.  minmax_dev: 2 ints of
- * device scratch (receives the source image's min and max, used by warp's output clipping).
+ * device scratch (receives 255 - min and the max of the source image, used by warp's output clipping).
  * ---------------------------------------------------------------------------------------- */
 int k2y_letterbox_u8(const unsigned char *src_dev, int src_h, int src_w, const double *inv_matrix_host,
                      unsigned char *dst_dev, int dst_h, int dst_w, int *minmax_dev, void *stream);
+/* The same letterbox for n images of different sizes in one call (k2y_letterbox_u8 is its n = 1 case).
+ * src_dev: the images packed back to back, image i at byte offsets_host[i] (a multiple of 16 lets pass 1 read 16 bytes at a
+ * time).  hw_host: [n][2] ints (h, w).  inv_matrices_host: [n][6] doubles, one k2y_letterbox_u8 matrix per image.
+ * dst_dev: [n][dst_h][dst_w][3] uint8.  image_hw_dev: [n][2] float32 (h, w) written for the decode's correct_box, or NULL.
+ * minmax_dev: [n][2] ints of device scratch.  Host arrays are read before the call returns; the work is asynchronous on
+ * `stream` (one memset, then two kernels per 48 images). */
+int k2y_letterbox_u8_batch(const unsigned char *src_dev, int n, const long long *offsets_host, const int *hw_host,
+                           const double *inv_matrices_host, unsigned char *dst_dev, int dst_h, int dst_w,
+                           float *image_hw_dev, int *minmax_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * Evaluation: the counters behind the reference's Yolo_Precision / Yolo_Recall metrics (tools/custom.py:13-75) on device

@@ -104,6 +104,8 @@ _SIGNATURES = {
     "k2y_expf_eval": (c_int, [c_int, c_void_p, c_void_p, ctypes.c_longlong, c_void_p]),
     "k2y_pr_counts": (c_int, [c_void_p, c_void_p, ctypes.c_longlong, c_int, c_float, c_int, c_void_p, c_void_p]),
     "k2y_letterbox_u8": (c_int, [c_void_p, c_int, c_int, POINTER(ctypes.c_double), c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "k2y_letterbox_u8_batch": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong), POINTER(c_int), POINTER(ctypes.c_double), c_void_p,
+                                       c_int, c_int, c_void_p, c_void_p, c_void_p]),
 }
 # include/region_layer.h (ABI-compatible firmware API)
 _REGION_ABI = ["region_layer_init", "region_layer_deinit", "region_layer_run", "region_layer_draw_boxes"]

@@ -10,97 +10,176 @@
 // bit-identical to the numpy oracle.
 #include "common.h"
 
+// A batch is n images of different sizes packed back to back in one device buffer.  Their descriptors travel by value in
+// the kernel parameters (__grid_constant__: indexed in place, never copied to local memory), LB_MAX_IMAGES per launch.
+// Pass 1 reduces each image's min and max into the scratch as (255 - min, max), both with atomicMax, so that one memset
+// to zero initialises it; pass 2 is the bilinear warp, one thread per output pixel, grid (pixel tile, image).
 namespace k2y {
 namespace {
 
-__global__ void __launch_bounds__(256) image_minmax_u8_kernel(const unsigned char *__restrict__ x, size_t n, int *__restrict__ minmax) {
-    int lo = 255, hi = 0;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const int v = x[i];
-        lo = min(lo, v);
-        hi = max(hi, v);
+constexpr int LB_MAX_IMAGES = 48;
+constexpr int LB_THREADS = 256;
+constexpr int LB_CHUNK = LB_THREADS * 64;   // source bytes per block of pass 1
+
+struct LbImage {
+    long long offset;   // byte offset of the image in the packed source buffer
+    int h, w;
+    double m[6];        // the first two rows of the inverse affine matrix
+};
+
+struct LbBatch {
+    const unsigned char *src;
+    unsigned char *dst;     // [n][dh][dw][3]
+    int *minmax;            // [n][2]: 255 - min, max
+    float *image_hw;        // [n][2] (h, w), or null
+    int dh, dw;
+    LbImage img[LB_MAX_IMAGES];
+};
+static_assert(sizeof(LbBatch) <= 4096, "letterbox descriptors must fit the kernel parameter space");
+
+__device__ __forceinline__ unsigned fold_min4(unsigned v) { return min(min(v & 255u, (v >> 8) & 255u), min((v >> 16) & 255u, v >> 24)); }
+__device__ __forceinline__ unsigned fold_max4(unsigned v) { return max(max(v & 255u, (v >> 8) & 255u), max((v >> 16) & 255u, v >> 24)); }
+
+__global__ void __launch_bounds__(LB_THREADS) letterbox_minmax_kernel(const __grid_constant__ LbBatch p) {
+    const LbImage &im = p.img[blockIdx.y];
+    const size_t bytes = (size_t)im.h * im.w * 3, begin = (size_t)blockIdx.x * LB_CHUNK;
+    if (begin >= bytes) return;
+    const size_t end = min(bytes, begin + (size_t)LB_CHUNK);
+    const unsigned char *s = p.src + im.offset;
+    unsigned lo4 = 0xffffffffu, hi4 = 0u;   // four byte lanes each
+    size_t tail = begin;
+    if (((uintptr_t)(s + begin) & 15) == 0) {
+        const uint4 *v = reinterpret_cast<const uint4 *>(s + begin);
+        const int nv = (int)((end - begin) / 16);
+        for (int i = threadIdx.x; i < nv; i += LB_THREADS) {
+            const uint4 q = __ldg(v + i);
+            lo4 = __vminu4(lo4, __vminu4(__vminu4(q.x, q.y), __vminu4(q.z, q.w)));
+            hi4 = __vmaxu4(hi4, __vmaxu4(__vmaxu4(q.x, q.y), __vmaxu4(q.z, q.w)));
+        }
+        tail += (size_t)nv * 16;
     }
+    for (size_t i = tail + threadIdx.x; i < end; i += LB_THREADS) {
+        const unsigned b = __ldg(s + i) * 0x01010101u;
+        lo4 = __vminu4(lo4, b);
+        hi4 = __vmaxu4(hi4, b);
+    }
+    int lo = (int)fold_min4(lo4), hi = (int)fold_max4(hi4);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         lo = min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
         hi = max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
     }
+    __shared__ int s_lo[LB_THREADS / 32], s_hi[LB_THREADS / 32];
     if ((threadIdx.x & 31) == 0) {
-        atomicMin(&minmax[0], lo);
-        atomicMax(&minmax[1], hi);
+        s_lo[threadIdx.x >> 5] = lo;
+        s_hi[threadIdx.x >> 5] = hi;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int k = 1; k < LB_THREADS / 32; ++k) {
+            lo = min(lo, s_lo[k]);
+            hi = max(hi, s_hi[k]);
+        }
+        atomicMax(&p.minmax[2 * blockIdx.y], 255 - lo);
+        atomicMax(&p.minmax[2 * blockIdx.y + 1], hi);
     }
 }
-
-struct LetterboxParams {
-    const unsigned char *src;
-    unsigned char *dst;
-    const int *minmax;
-    int sh, sw, dh, dw;
-    double m00, m01, m02, m10, m11, m12;
-};
 
 __device__ __forceinline__ double pix_or_zero(const unsigned char *src, int sh, int sw, double r, double c, int ch) {
     if (!(r >= 0.0 && r < (double)sh && c >= 0.0 && c < (double)sw)) return 0.0;
     return (double)src[((size_t)(int)r * sw + (int)c) * 3 + ch];
 }
 
-__global__ void __launch_bounds__(256) letterbox_u8_kernel(const LetterboxParams p) {
+__global__ void __launch_bounds__(LB_THREADS) letterbox_warp_kernel(const __grid_constant__ LbBatch p) {
+    const int b = blockIdx.y;
+    const LbImage &im = p.img[b];
+    if (p.image_hw && blockIdx.x == 0 && threadIdx.x == 0) {
+        p.image_hw[2 * b] = (float)im.h;
+        p.image_hw[2 * b + 1] = (float)im.w;
+    }
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= p.dh * p.dw) return;
+    const unsigned char *src = p.src + im.offset;
+    const int sh = im.h, sw = im.w;
     const double r = (double)(idx / p.dw), c = (double)(idx % p.dw);
-    const double x = __dadd_rn(__dadd_rn(__dmul_rn(p.m00, c), __dmul_rn(p.m01, r)), p.m02);
-    const double y = __dadd_rn(__dadd_rn(__dmul_rn(p.m10, c), __dmul_rn(p.m11, r)), p.m12);
+    const double x = __dadd_rn(__dadd_rn(__dmul_rn(im.m[0], c), __dmul_rn(im.m[1], r)), im.m[2]);
+    const double y = __dadd_rn(__dadd_rn(__dmul_rn(im.m[3], c), __dmul_rn(im.m[4], r)), im.m[5]);
     const double minr = floor(y), minc = floor(x), maxr = ceil(y), maxc = ceil(x);
     const double dr = __dsub_rn(y, minr), dc = __dsub_rn(x, minc);
     const double wr = __dsub_rn(1.0, dr), wc = __dsub_rn(1.0, dc);
-    const double lo = (double)p.minmax[0], hi = (double)p.minmax[1];
+    const double lo = (double)(255 - p.minmax[2 * b]), hi = (double)p.minmax[2 * b + 1];
     const bool keep_fill = lo > 0.0;  // 0 (cval) lies outside [min, max]: exact-zero pixels are preserved by the clip
+    unsigned char *dst = p.dst + ((size_t)b * p.dh * p.dw + idx) * 3;
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
-        const double p00 = pix_or_zero(p.src, p.sh, p.sw, minr, minc, ch), p01 = pix_or_zero(p.src, p.sh, p.sw, minr, maxc, ch);
-        const double p10 = pix_or_zero(p.src, p.sh, p.sw, maxr, minc, ch), p11 = pix_or_zero(p.src, p.sh, p.sw, maxr, maxc, ch);
+        const double p00 = pix_or_zero(src, sh, sw, minr, minc, ch), p01 = pix_or_zero(src, sh, sw, minr, maxc, ch);
+        const double p10 = pix_or_zero(src, sh, sw, maxr, minc, ch), p11 = pix_or_zero(src, sh, sw, maxr, maxc, ch);
         const double top = __dadd_rn(__dmul_rn(wc, p00), __dmul_rn(dc, p01));
         const double bot = __dadd_rn(__dmul_rn(wc, p10), __dmul_rn(dc, p11));
         double o = __dadd_rn(__dmul_rn(wr, top), __dmul_rn(dr, bot));
         if (!(keep_fill && o == 0.0)) o = fmin(fmax(o, lo), hi);
-        p.dst[(size_t)idx * 3 + ch] = (unsigned char)(int)o;
+        dst[ch] = (unsigned char)(int)o;
     }
 }
 
 }  // namespace
 }  // namespace k2y
 
-extern "C" int k2y_letterbox_u8(const unsigned char *src_dev, int src_h, int src_w, const double *inv_matrix_host,
-                                unsigned char *dst_dev, int dst_h, int dst_w, int *minmax_dev, void *stream) {
+extern "C" int k2y_letterbox_u8_batch(const unsigned char *src_dev, int n, const long long *offsets_host, const int *hw_host,
+                                      const double *inv_matrices_host, unsigned char *dst_dev, int dst_h, int dst_w,
+                                      float *image_hw_dev, int *minmax_dev, void *stream) {
     using namespace k2y;
-    if (!src_dev || !dst_dev || !inv_matrix_host || !minmax_dev || src_h <= 0 || src_w <= 0 || dst_h <= 0 || dst_w <= 0) {
-        set_error("k2y_letterbox_u8: bad arguments");
+    if (!src_dev || n <= 0 || !offsets_host || !hw_host || !inv_matrices_host || !dst_dev || !minmax_dev || dst_h <= 0 || dst_w <= 0 ||
+        (long long)dst_h * dst_w > (1LL << 30)) {
+        set_error("k2y_letterbox_u8_batch: bad arguments");
         return K2Y_ERR_INVALID;
     }
+    for (int i = 0; i < n; ++i) {
+        if (offsets_host[i] < 0 || hw_host[2 * i] <= 0 || hw_host[2 * i + 1] <= 0) {
+            set_error("k2y_letterbox_u8_batch: image %d has offset %lld and size %dx%d", i, offsets_host[i], hw_host[2 * i],
+                      hw_host[2 * i + 1]);
+            return K2Y_ERR_INVALID;
+        }
+    }
     cudaStream_t st = (cudaStream_t)stream;
-    static const int init[2] = {255, 0};
-    K2Y_CUDA_CHECK(cudaMemcpyAsync(minmax_dev, init, sizeof(init), cudaMemcpyHostToDevice, st));
-    const size_t n = (size_t)src_h * src_w * 3;
-    int blocks = (int)((n + 256 * 16 - 1) / (256 * 16));
-    if (blocks > 592) blocks = 592;
-    image_minmax_u8_kernel<<<blocks, 256, 0, st>>>(src_dev, n, minmax_dev);
-    LetterboxParams p;
-    p.src = src_dev;
-    p.dst = dst_dev;
-    p.minmax = minmax_dev;
-    p.sh = src_h;
-    p.sw = src_w;
-    p.dh = dst_h;
-    p.dw = dst_w;
-    p.m00 = inv_matrix_host[0];
-    p.m01 = inv_matrix_host[1];
-    p.m02 = inv_matrix_host[2];
-    p.m10 = inv_matrix_host[3];
-    p.m11 = inv_matrix_host[4];
-    p.m12 = inv_matrix_host[5];
-    letterbox_u8_kernel<<<(dst_h * dst_w + 255) / 256, 256, 0, st>>>(p);
-    K2Y_CUDA_CHECK(cudaGetLastError());
+    K2Y_CUDA_CHECK(cudaMemsetAsync(minmax_dev, 0, sizeof(int) * 2 * (size_t)n, st));
+    const size_t plane = (size_t)dst_h * dst_w * 3;
+    for (int g0 = 0; g0 < n; g0 += LB_MAX_IMAGES) {
+        const int g = n - g0 < LB_MAX_IMAGES ? n - g0 : LB_MAX_IMAGES;
+        LbBatch p;
+        memset(&p, 0, sizeof(p));
+        p.src = src_dev;
+        p.dst = dst_dev + plane * g0;
+        p.minmax = minmax_dev + 2 * g0;
+        p.image_hw = image_hw_dev ? image_hw_dev + 2 * g0 : nullptr;
+        p.dh = dst_h;
+        p.dw = dst_w;
+        size_t max_bytes = 0;
+        for (int i = 0; i < g; ++i) {
+            LbImage &im = p.img[i];
+            im.offset = offsets_host[g0 + i];
+            im.h = hw_host[2 * (g0 + i)];
+            im.w = hw_host[2 * (g0 + i) + 1];
+            for (int k = 0; k < 6; ++k) im.m[k] = inv_matrices_host[6 * (g0 + i) + k];
+            const size_t bytes = (size_t)im.h * im.w * 3;
+            if (bytes > max_bytes) max_bytes = bytes;
+        }
+        letterbox_minmax_kernel<<<dim3((unsigned)((max_bytes + LB_CHUNK - 1) / LB_CHUNK), g), LB_THREADS, 0, st>>>(p);
+        letterbox_warp_kernel<<<dim3((unsigned)((dst_h * dst_w + LB_THREADS - 1) / LB_THREADS), g), LB_THREADS, 0, st>>>(p);
+        K2Y_CUDA_CHECK(cudaGetLastError());
+    }
     return K2Y_OK;
+}
+
+extern "C" int k2y_letterbox_u8(const unsigned char *src_dev, int src_h, int src_w, const double *inv_matrix_host,
+                                unsigned char *dst_dev, int dst_h, int dst_w, int *minmax_dev, void *stream) {
+    if (!src_dev || !dst_dev || !inv_matrix_host || !minmax_dev || src_h <= 0 || src_w <= 0 || dst_h <= 0 || dst_w <= 0) {
+        k2y::set_error("k2y_letterbox_u8: bad arguments");
+        return K2Y_ERR_INVALID;
+    }
+    const long long offset = 0;
+    const int hw[2] = {src_h, src_w};
+    return k2y_letterbox_u8_batch(src_dev, 1, &offset, hw, inv_matrix_host, dst_dev, dst_h, dst_w, nullptr, minmax_dev, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -14,6 +14,11 @@ copies use a fourth stream and land directly in one of two device input buffers 
 per (input buffer, head set)), so there is no staging copy.  ``step_device(pipelined=False)`` (the default) makes the
 caller's stream wait for the decode before returning — plain stream semantics; the streaming calls (``submit``/``collect``,
 ``step_device(pipelined=True)`` + ``wait_gathered()``) keep the overlap.
+
+``submit_images`` takes raw host images of any size instead: each input slot has its own pinned staging buffer and its own
+device ``image_hw`` [batch, 2]; the packed H2D copy and the batched letterbox (which also writes ``image_hw``) run on the copy
+stream into the slot's uint8 input buffer, overlapping the previous batch's network, and the decode of that batch reads the
+slot's ``image_hw``, so two batches in flight each carry their own original sizes.
 """
 from __future__ import annotations
 
@@ -25,6 +30,7 @@ import torch
 from . import yolonet
 from .detect import DET_WORDS, KerasDetector
 from .dist import DetectionGather
+from .preprocess import BatchLayout, Staging, letterbox_packed
 
 SLOTS = 2
 
@@ -34,6 +40,7 @@ class DetectionPipeline:
                  batch: int, obj_thresh: float = 0.7, iou_thresh: float = 0.3, max_per_class: int = 30,
                  device: Optional[int] = None, world: int = 1, rank: int = 0, comm=None):
         self.batch, self.world, self.rank = int(batch), int(world), int(rank)
+        self.in_hw = (int(image_size[0]), int(image_size[1]))
         self.device_index = torch.cuda.current_device() if device is None else int(device)
         builder = getattr(yolonet, model_def)
         self.model, self.wrapper = builder([image_size[0], image_size[1], 3], len(anchors[0]), class_num, alpha=alpha,
@@ -60,6 +67,11 @@ class DetectionPipeline:
         self._gather_done = [torch.cuda.Event() for _ in range(SLOTS)]   # gather slot complete on this rank
         self._slot_free = [torch.cuda.Event() for _ in range(SLOTS)]     # last reader of gather slot is done
         self._d2h_done = [torch.cuda.Event() for _ in range(SLOTS)]
+        # submit_images: per input slot a pinned staging buffer and the (h, w) of its images, created on first use
+        self._staging: Optional[List[Staging]] = None
+        self._slot_hw: Optional[List[torch.Tensor]] = None
+        self._hw_free = [torch.cuda.Event() for _ in range(SLOTS)]       # decode finished reading the slot's image sizes
+        self._rows: List[Optional[int]] = [None] * SLOTS                 # records collect returns per gather slot (None: all)
         self._steps = 0
         self._submitted = 0
 
@@ -69,9 +81,10 @@ class DetectionPipeline:
         self._img_hw.copy_(torch.from_numpy(np.array(arr, dtype=np.float32, order="C", copy=True)))
 
     # -- device-resident step ---------------------------------------------------------------------------------------
-    def _step(self, n: int) -> int:
+    def _step(self, n: int, image_hw: Optional[torch.Tensor] = None) -> int:
         """Network on the current stream into head set s, decode/NMS on the decode stream into gather slot s, then
-        (world > 1) the all-gather on the side stream.  Returns s."""
+        (world > 1) the all-gather on the side stream.  `image_hw`: device [n, 2] original sizes (default: the shared
+        ``set_image_shapes`` tensor).  Returns s."""
         s = self._steps % SLOTS
         self._steps += 1
         compute = torch.cuda.current_stream(self.device_index)
@@ -86,7 +99,7 @@ class DetectionPipeline:
         det.wait_event(self._heads_ready[s])
         det.wait_event(self._slot_free[s])          # whoever still reads this gather slot (all-gather / D2H two steps ago)
         dets, counts = self.gather.local(s)
-        self.detector.run(heads, self._img_hw[:n], dets_out=dets, counts_out=counts, stream=det)
+        self.detector.run(heads, self._img_hw[:n] if image_hw is None else image_hw, dets_out=dets, counts_out=counts, stream=det)
         self._det_done[s].record(det)
         if self.world > 1:
             self._side.wait_event(self._det_done[s])
@@ -137,17 +150,50 @@ class DetectionPipeline:
         n = x_host.shape[0]
         slot = self._submitted % SLOTS
         self._submitted += 1
-        compute = torch.cuda.current_stream(self.device_index)
         # raw letterboxed RGB (uint8): 4x fewer PCIe bytes, the normalisation (img / max(img)) is fused into the first conv
         buf = self._input_slots(x_host.dtype == torch.uint8)[slot]
         self._copy_stream.wait_event(self._in_free[slot])
         with torch.cuda.stream(self._copy_stream):
             buf[:n].copy_(x_host, non_blocking=True)
             self._h2d_done[slot].record(self._copy_stream)
+        return self._run_slot(slot, buf, n, None, None)
+
+    def submit_images(self, images: Sequence[np.ndarray]) -> int:
+        """Streaming form for raw images: `images` is a list of n <= batch host numpy uint8 [h, w, 3] RGB arrays of any sizes.
+        They are packed into the input slot's pinned staging buffer, copied to the GPU in one H2D copy and letterboxed in one
+        launch into the slot's uint8 input buffer (``k2y_letterbox_u8_batch``, which also writes the slot's device
+        ``image_hw`` the decode reads), on the copy stream, overlapping the previous batch's network.  The network runs the n
+        images.  Returns a ticket for ``collect``, which returns the n images' records (world > 1: the gathered blocks of every
+        rank, rank r's images from row r * batch).  Same flow control as ``submit``.  Bad input raises ``ValueError`` before
+        anything is enqueued."""
+        layout = BatchLayout(images, self.in_hw)
+        n = len(layout)
+        if n > self.batch:
+            raise ValueError(f"{n} images do not fit a batch of {self.batch}")
+        slot = self._submitted % SLOTS
+        buf = self._input_slots(True)[slot]
+        dev = buf.device
+        if self._staging is None:
+            self._staging = [Staging(dev, self._copy_stream) for _ in range(SLOTS)]
+            self._slot_hw = [torch.empty((self.batch, 2), dtype=torch.float32, device=dev) for _ in range(SLOTS)]
+        self._h2d_done[slot].synchronize()     # the last copy out of this slot's pinned buffer has finished: repack / grow it
+        self._submitted += 1
+        self._copy_stream.wait_event(self._in_free[slot])
+        self._copy_stream.wait_event(self._hw_free[slot])
+        with torch.cuda.device(dev):
+            letterbox_packed(layout, images, self._staging[slot], buf, self._slot_hw[slot])
+        self._h2d_done[slot].record(self._copy_stream)
+        return self._run_slot(slot, buf, n, self._slot_hw[slot][:n], n if self.world == 1 else None)
+
+    def _run_slot(self, slot: int, buf: torch.Tensor, n: int, image_hw: Optional[torch.Tensor], rows: Optional[int]) -> int:
+        """Network + decode (+ all-gather) of input slot `slot` once its H2D is done, then the D2H of the records."""
+        compute = torch.cuda.current_stream(self.device_index)
         compute.wait_event(self._h2d_done[slot])
         self.engine.bind_input(buf)
-        s = self._step(n)
+        s = self._step(n, image_hw)
         self._in_free[slot].record(compute)
+        self._hw_free[slot].record(self._det_stream)
+        self._rows[s] = rows
         # D2H of the gathered blocks: behind the all-gather on the side stream (world > 1), else behind the decode
         st = self._side if self.world > 1 else self._det_stream
         with torch.cuda.stream(st):
@@ -160,7 +206,9 @@ class DetectionPipeline:
         """Blocks until the batch behind `ticket` is on the host; returns (dets, counts) pinned host views (valid
         until the ticket's slot is reused two submits later)."""
         self._d2h_done[ticket].synchronize()
-        return DetectionGather.split(self._host[ticket], self.gather.C, self.gather.K, DET_WORDS)
+        dets, counts = DetectionGather.split(self._host[ticket], self.gather.C, self.gather.K, DET_WORDS)
+        n = self._rows[ticket]
+        return (dets, counts) if n is None else (dets[:n], counts[:n])
 
     def launches_per_step(self) -> int:
         return self.engine.launches_per_run() + 2  # + the decode scan and the per-class NMS kernel
@@ -178,7 +226,7 @@ class LanedPipeline:
     lane sizes its persistent tensor-core grids for 1/lanes of the SMs, so the lanes' kernels share the GPU side by side.
 
     ``bind_input(x)`` / ``step_device()`` / ``wait_all()`` for device-resident inputs, ``submit`` / ``collect`` for pinned
-    host batches (tickets carry the lane)."""
+    host batches and ``submit_images`` / ``collect`` for raw host images of any size (tickets carry the lane)."""
 
     def __init__(self, lanes: int, *args, sm_split: bool = True, sm_limit: Optional[int] = None, max_queued: Optional[int] = None, **kw):
         if lanes < 1:
@@ -256,6 +304,14 @@ class LanedPipeline:
         self._next_host += 1
         with torch.cuda.stream(self._streams[k]):
             return (k, self.lanes[k].submit(x_host))
+
+    def submit_images(self, images: Sequence[np.ndarray]):
+        """``DetectionPipeline.submit_images`` on the next lane (round-robin, shared with ``submit``)."""
+        k = self._next_host % len(self.lanes)
+        with torch.cuda.stream(self._streams[k]):
+            t = self.lanes[k].submit_images(images)
+        self._next_host += 1
+        return (k, t)
 
     def collect(self, ticket):
         k, t = ticket

@@ -7,14 +7,17 @@ gathered detections, one JSON line per image.  The GPU analogue of the firmware'
                                     --anchors data/voc_anchor.npy --batch 32 --obj_thresh 0.7 --iou_thresh 0.5 --out dets.jsonl]
     python -m torch.distributed.run --nproc-per-node 8 serve.py ...        # one rank per GPU, NCCL all-gather of the records
 
-Per global batch of world*batch images: every rank decodes ITS images on the host (PIL), letterboxes each on the GPU
-(k2y_letterbox_u8) into its uint8 input buffer, runs network + decode + NMS, and ONE all-gather completes the record blocks on
-every rank; rank 0 writes the lines in file order.
+Per global batch of world*batch images: every rank decodes ITS images on the host (PIL, in a pool of --decode_threads
+threads, one batch ahead), hands them to DetectionPipeline.submit_images (one packed H2D copy, one batched letterbox launch
+into its uint8 input buffer, network + decode + NMS), and ONE all-gather completes the record blocks on every rank; two
+batches are in flight, and rank 0 writes the lines in file order.
 """
 import argparse
 import json
 import os
 import sys
+from collections import deque
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
@@ -51,30 +54,41 @@ def serve(args, out_fh=None):
                              args.iou_thresh, 30, device=local, world=world, rank=rank)
     pipe.engine.load_weights(args.ckpt)
     files = list_images(args.images)
-    buf = torch.zeros((args.batch, H, W, 3), dtype=torch.uint8, device=f"cuda:{local}")
-    shapes = np.tile(np.array([[H, W]], np.float32), (args.batch, 1))
-    G = world * args.batch
+    B, G = args.batch, world * args.batch
+    chunks = [files[g0:g0 + G] for g0 in range(0, len(files), G)]
+    # every rank runs the network on a full batch (the tensor-core plans depend on the batch size, so the records of a short
+    # final batch match a full one's bit for bit) and takes part in every all-gather: its share of a short batch is padded
+    # with a grey network-size image, whose records nobody reads
+    filler = np.full((H, W, 3), 128, np.uint8)
     n_out = 0
-    for g0 in range(0, len(files), G):
-        chunk = files[g0:g0 + G]
-        lo, hi = rank * args.batch, min((rank + 1) * args.batch, len(chunk))
-        for j in range(lo, hi):                                   # this rank's images of the global batch
-            img = h._read_img(chunk[j])
-            shapes[j - lo] = img.shape[:2]
-            buf[j - lo].copy_(h.letterbox_device(img))
-        pipe.set_image_shapes(shapes)
-        pipe.engine.bind_input(buf)
-        dets, counts = pipe.step_device(args.batch)
-        pipe.wait_gathered()
-        torch.cuda.synchronize()
-        if rank == 0:
-            recs = DetectionPipeline.records(dets[:len(chunk)].clone() if world == 1 else dets.clone(), counts.clone())
-            for j, path in enumerate(chunk):
-                line = {"image": path, "detections": [{"class": int(c), "score": round(float(s), 6), "box_tlbr": [float(t), float(l), float(b), float(r)],
-                                                       "index": int(i)} for c, i, s, t, l, b, r in recs[j]]}
-                if out_fh is not None:
-                    out_fh.write(json.dumps(line) + "\n")
-                n_out += 1
+
+    def write(chunk, ticket):
+        nonlocal n_out
+        dets, counts = pipe.collect(ticket)
+        if rank != 0:
+            return
+        recs = DetectionPipeline.records(dets, counts)
+        for j, path in enumerate(chunk):
+            line = {"image": path, "detections": [{"class": int(c), "score": round(float(s), 6), "box_tlbr": [float(t), float(l), float(b), float(r)],
+                                                   "index": int(i)} for c, i, s, t, l, b, r in recs[j]]}
+            if out_fh is not None:
+                out_fh.write(json.dumps(line) + "\n")
+            n_out += 1
+
+    with ThreadPoolExecutor(max(1, int(getattr(args, "decode_threads", 4)))) as pool:
+        def decode(chunk):      # this rank's images of a global batch, decoding in the pool
+            return [pool.submit(h._read_img, p) for p in chunk[rank * B:(rank + 1) * B]]
+
+        pending = deque()
+        nxt = decode(chunks[0]) if chunks else []
+        for g, chunk in enumerate(chunks):
+            imgs = [f.result() for f in nxt]
+            nxt = decode(chunks[g + 1]) if g + 1 < len(chunks) else []
+            pending.append((chunk, pipe.submit_images(imgs + [filler] * (B - len(imgs)))))
+            if len(pending) == 2:
+                write(*pending.popleft())
+        while pending:
+            write(*pending.popleft())
     if world > 1:
         dist.barrier()
     return n_out
@@ -92,6 +106,7 @@ def main():
     ap.add_argument("--batch", type=int, default=32, help="images per GPU per step")
     ap.add_argument("--obj_thresh", type=float, default=0.7)
     ap.add_argument("--iou_thresh", type=float, default=0.5)
+    ap.add_argument("--decode_threads", type=int, default=4, help="host threads decoding the next batch's files (PIL)")
     ap.add_argument("--out", default="-")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
