@@ -258,6 +258,49 @@ int k2y_letterbox_u8_batch(const unsigned char *src_dev, int n, const long long 
                            float *image_hw_dev, int *minmax_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Baseline JPEG decode on the device, in front of k2y_letterbox_u8_batch: replaces the file decode of
+ * Helper._read_img (tools/utils.py:339-355, skimage.io.imread -> PIL -> libjpeg-turbo) for the files it accepts.
+ * Exactness: the RGB bytes equal libjpeg-turbo's with PIL's settings, i.e. the JDCT_ISLOW integer IDCT (jidctint.c),
+ * fancy upsampling (jdsample.c, as jinit_upsampler dispatches it) and ycc_rgb_convert (jdcolor.c); grey files are
+ * written to all three channels, as _read_img stacks them.
+ * GPU-decodable: 8-bit sequential Huffman (SOF0/SOF1), one scan holding every component, 1 component or 3 that libjpeg
+ * treats as YCbCr, chroma 1x1 with luma 1x1, 2x1, 1x2, 2x2 or 4x1, any restart interval.  Every other valid file
+ * (progressive, arithmetic, 12-bit, lossless, CMYK/YCCK, RGB, multi-scan, DNL, other sampling) is reported with its
+ * reason and is left to the host.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+    int32_t height, width, components;
+    int32_t h_samp[4], v_samp[4];   /* per component, frame order (0 past `components`) */
+    int32_t restart_interval;       /* MCUs, 0 = none */
+    int32_t precision;              /* bits per sample */
+    int32_t sof_marker;             /* 0xC0 .. 0xCF */
+    int32_t gpu_decodable;          /* 1: k2y_jpeg_plan accepts the file */
+    int32_t entropy_offset;         /* first byte of the scan's entropy-coded data (GPU-decodable files) */
+    char reason[64];                /* why not, when gpu_decodable == 0 */
+} k2y_jpeg_info;
+/* Host only: walks the markers up to the first SOS.  K2Y_ERR_INVALID (message names the marker and its offset) for a
+ * malformed file; K2Y_OK with info->gpu_decodable and info->reason otherwise. */
+int k2y_jpeg_inspect(const unsigned char *data, size_t size, k2y_jpeg_info *info);
+/* Host only: the descriptor blob of a batch of n GPU-decodable files (dimensions, sampling, quantisation tables, Huffman
+ * decode tables in lookup form, restart segments and every offset).  files[i] / sizes[i]: the file bytes on the host;
+ * src_offsets[i]: where file i will lie in the device source buffer; dst_offsets[i]: where its h*w*3 RGB bytes go in the
+ * device output buffer (BatchLayout's offsets).  blob == NULL: only *blob_bytes is set (size query); otherwise blob is a
+ * 16-byte aligned host buffer of blob_capacity >= *blob_bytes.  A file that is not GPU-decodable is K2Y_ERR_INVALID. */
+int k2y_jpeg_plan(const unsigned char *const *files, const size_t *sizes, int n, const long long *src_offsets,
+                  const long long *dst_offsets, void *blob, size_t blob_capacity, size_t *blob_bytes);
+/* Device workspace k2y_jpeg_decode needs for the batch a blob describes (read from the host copy of the blob). */
+int k2y_jpeg_workspace_bytes(const void *blob_host, size_t *bytes);
+/* Decodes the batch, asynchronous on `stream`: blob_host is read before the call returns (launch sizes), blob_dev is the
+ * same bytes on the device (16-byte aligned), src_dev the files at their src_offsets, dst_dev the output.  Five kernels,
+ * one launch each whatever the image count: unstuff/split at RSTn, self-synchronising Huffman decode (one CTA per restart
+ * segment), DC prediction, dequantise + IDCT, upsample + colour convert.  status_dev: int32 [n][4] per image: error bits
+ * (1 invalid Huffman code, 2 entropy data ended early: the image's pixels are then undefined, the other images' are
+ * exact), the most synchronisation rounds one window of subsequences took, their sum and the number of windows.
+ * Corrupt data never makes a kernel read outside its image's bytes or write outside its output. */
+int k2y_jpeg_decode(const void *blob_host, const void *blob_dev, const unsigned char *src_dev, unsigned char *dst_dev,
+                    void *workspace_dev, size_t workspace_bytes, int32_t *status_dev, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Evaluation: the counters behind the reference's Yolo_Precision / Yolo_Recall metrics (tools/custom.py:13-75) on device
  * tensors.  y_true_dev / y_pred_dev: n_boxes records of entry_floats = 5 + classes floats (any [..., A, 5+C] head or label
  * tensor, flattened); element 4 is the confidence.  counts_dev[3] (uint64, caller-zeroed, accumulated into): tp, fp, fn with

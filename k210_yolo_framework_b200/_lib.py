@@ -49,6 +49,12 @@ class RegionCfg(ctypes.Structure):
                 ("anchors", c_float * 16), ("threshold", c_float), ("nms_value", c_float)]
 
 
+class JpegInfo(ctypes.Structure):
+    _fields_ = [("height", c_int32), ("width", c_int32), ("components", c_int32), ("h_samp", c_int32 * 4), ("v_samp", c_int32 * 4),
+                ("restart_interval", c_int32), ("precision", c_int32), ("sof_marker", c_int32), ("gpu_decodable", c_int32),
+                ("entropy_offset", c_int32), ("reason", ctypes.c_char * 64)]
+
+
 # Every symbol include/k210_yolo_b200.h declares (tests/test_abi.py checks the two lists agree).
 _SIGNATURES = {
     "k2y_last_error": (c_char_p, []),
@@ -106,6 +112,11 @@ _SIGNATURES = {
     "k2y_letterbox_u8": (c_int, [c_void_p, c_int, c_int, POINTER(ctypes.c_double), c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "k2y_letterbox_u8_batch": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong), POINTER(c_int), POINTER(ctypes.c_double), c_void_p,
                                        c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "k2y_jpeg_inspect": (c_int, [c_void_p, c_size_t, POINTER(JpegInfo)]),
+    "k2y_jpeg_plan": (c_int, [POINTER(c_void_p), POINTER(c_size_t), c_int, POINTER(ctypes.c_longlong), POINTER(ctypes.c_longlong),
+                              c_void_p, c_size_t, POINTER(c_size_t)]),
+    "k2y_jpeg_workspace_bytes": (c_int, [c_void_p, POINTER(c_size_t)]),
+    "k2y_jpeg_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
 }
 # include/region_layer.h (ABI-compatible firmware API)
 _REGION_ABI = ["region_layer_init", "region_layer_deinit", "region_layer_run", "region_layer_draw_boxes"]

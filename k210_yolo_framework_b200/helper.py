@@ -30,26 +30,7 @@ class Helper(object):
 
     def _read_img(self, img_path: str) -> np.ndarray:
         """tools/utils.py:339-355 (skimage.io.imread -> RGB uint8, grey -> 3 channels, alpha dropped)."""
-        from PIL import Image
-        im = Image.open(img_path)
-        # skimage.io.imread semantics by PIL mode: palette / CMYK / YCbCr images are expanded to RGB, grey (+alpha) becomes
-        # 3 equal channels, 16/32-bit grey is scaled down to 8 bits, alpha is dropped
-        if im.mode in ("P", "CMYK", "YCbCr", "PA"):
-            im = im.convert("RGB")
-        elif im.mode in ("LA", "La"):
-            im = im.convert("L")
-        elif im.mode == "1":
-            im = im.convert("L")
-        elif im.mode in ("I", "I;16", "I;16B", "I;16L", "F"):
-            arr = np.asarray(im, dtype=np.float64)
-            hi = float(arr.max()) if arr.size else 0.0
-            im = Image.fromarray(np.clip(arr * (255.0 / hi if hi > 255.0 else 1.0), 0, 255).astype(np.uint8))
-        elif im.mode not in ("RGB", "RGBA", "L"):
-            im = im.convert("RGB")
-        img = np.asarray(im, dtype=np.uint8)
-        if img.ndim != 3:
-            img = np.stack([img] * 3, axis=-1)
-        return img[..., :3]
+        return read_image(img_path)
 
     def _process_img(self, img: np.ndarray, true_box=None, is_training: bool = False, is_resize: bool = True):
         """tools/utils.py:357-406, inference branch: letterbox to in_hw[0] then ``img / np.max(img)``.
@@ -84,3 +65,27 @@ _COLORMAP_RGB = bytes.fromhex(
     "7009ff08ffd607ffe0ffb8060aff47ff290a07ffffe0ff086608ffff3d06ffc207ff7a0800ff14ff0829ff05990633ff"
     "eb0cffa0961400a3ff8c8c8cfa0a0f14ff001fff00ff1f00ffe00099ff000000ffff470000ebff00adff1f00ff0bc8c8")
 _COLORMAP = [tuple(_COLORMAP_RGB[i:i + 3]) for i in range(0, len(_COLORMAP_RGB), 3)]
+
+
+def read_image(img_path) -> np.ndarray:
+    """``Helper._read_img``: `img_path` is a path or a binary file object (e.g. ``io.BytesIO`` of a file's bytes)."""
+    from PIL import Image
+    im = Image.open(img_path)
+    # skimage.io.imread semantics by PIL mode: palette / CMYK / YCbCr images are expanded to RGB, grey (+alpha) becomes
+    # 3 equal channels, 16/32-bit grey is scaled down to 8 bits, alpha is dropped
+    if im.mode in ("P", "CMYK", "YCbCr", "PA"):
+        im = im.convert("RGB")
+    elif im.mode in ("LA", "La"):
+        im = im.convert("L")
+    elif im.mode == "1":
+        im = im.convert("L")
+    elif im.mode in ("I", "I;16", "I;16B", "I;16L", "F"):
+        arr = np.asarray(im, dtype=np.float64)
+        hi = float(arr.max()) if arr.size else 0.0
+        im = Image.fromarray(np.clip(arr * (255.0 / hi if hi > 255.0 else 1.0), 0, 255).astype(np.uint8))
+    elif im.mode not in ("RGB", "RGBA", "L"):
+        im = im.convert("RGB")
+    img = np.asarray(im, dtype=np.uint8)
+    if img.ndim != 3:
+        img = np.stack([img] * 3, axis=-1)
+    return img[..., :3]

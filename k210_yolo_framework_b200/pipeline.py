@@ -30,7 +30,7 @@ import torch
 from . import yolonet
 from .detect import DET_WORDS, KerasDetector
 from .dist import DetectionGather
-from .preprocess import BatchLayout, Staging, letterbox_packed
+from .preprocess import BatchLayout, Staging, check_jpeg_status, letterbox_packed
 
 SLOTS = 2
 
@@ -72,6 +72,9 @@ class DetectionPipeline:
         self._slot_hw: Optional[List[torch.Tensor]] = None
         self._hw_free = [torch.cuda.Event() for _ in range(SLOTS)]       # decode finished reading the slot's image sizes
         self._rows: List[Optional[int]] = [None] * SLOTS                 # records collect returns per gather slot (None: all)
+        # GPU-decoded JPEGs of the batch behind each gather slot: their batch positions and (pinned) status words
+        self._jpeg_idx: List[list] = [[] for _ in range(SLOTS)]
+        self._jpeg_status = [torch.zeros((batch, 4), dtype=torch.int32).pin_memory() for _ in range(SLOTS)]
         self._steps = 0
         self._submitted = 0
 
@@ -156,16 +159,20 @@ class DetectionPipeline:
         with torch.cuda.stream(self._copy_stream):
             buf[:n].copy_(x_host, non_blocking=True)
             self._h2d_done[slot].record(self._copy_stream)
+        self._jpeg_idx[self._steps % SLOTS] = []
         return self._run_slot(slot, buf, n, None, None)
 
     def submit_images(self, images: Sequence[np.ndarray]) -> int:
-        """Streaming form for raw images: `images` is a list of n <= batch host numpy uint8 [h, w, 3] RGB arrays of any sizes.
+        """Streaming form for raw images: `images` is a list of n <= batch host numpy uint8 [h, w, 3] RGB arrays of any sizes, or
+        image files (``bytes``, ``bytearray``, ``memoryview``): baseline JPEGs are decoded on the GPU on the copy stream in front
+        of the letterbox, other files on the host inside this call (``preprocess.BatchLayout``).
         They are packed into the input slot's pinned staging buffer, copied to the GPU in one H2D copy and letterboxed in one
         launch into the slot's uint8 input buffer (``k2y_letterbox_u8_batch``, which also writes the slot's device
         ``image_hw`` the decode reads), on the copy stream, overlapping the previous batch's network.  The network runs the n
         images.  Returns a ticket for ``collect``, which returns the n images' records (world > 1: the gathered blocks of every
-        rank, rank r's images from row r * batch).  Same flow control as ``submit``.  Bad input raises ``ValueError`` before
-        anything is enqueued."""
+        rank, rank r's images from row r * batch), or raises ``K2YError`` naming the JPEGs whose entropy-coded data was corrupt
+        (their records would come from undefined pixels).  Same flow control as ``submit``.  Bad input raises ``ValueError``
+        before anything is enqueued."""
         layout = BatchLayout(images, self.in_hw)
         n = len(layout)
         if n > self.batch:
@@ -180,8 +187,13 @@ class DetectionPipeline:
         self._submitted += 1
         self._copy_stream.wait_event(self._in_free[slot])
         self._copy_stream.wait_event(self._hw_free[slot])
+        s = self._steps % SLOTS                  # the gather slot this batch's step will use
         with torch.cuda.device(dev):
             letterbox_packed(layout, images, self._staging[slot], buf, self._slot_hw[slot])
+            self._jpeg_idx[s] = [i for i, _ in layout.jpeg]
+            if layout.jpeg:             # the status words travel to the host before the network starts on this slot
+                with torch.cuda.stream(self._copy_stream):
+                    self._jpeg_status[s][:len(layout.jpeg)].copy_(self._staging[slot].status[:len(layout.jpeg)], non_blocking=True)
         self._h2d_done[slot].record(self._copy_stream)
         return self._run_slot(slot, buf, n, self._slot_hw[slot][:n], n if self.world == 1 else None)
 
@@ -204,8 +216,12 @@ class DetectionPipeline:
 
     def collect(self, ticket: int):
         """Blocks until the batch behind `ticket` is on the host; returns (dets, counts) pinned host views (valid
-        until the ticket's slot is reused two submits later)."""
-        self._d2h_done[ticket].synchronize()
+        until the ticket's slot is reused two submits later).  Raises ``K2YError`` when a JPEG of a ``submit_images`` batch had
+        corrupt entropy-coded data."""
+        self._d2h_done[ticket].synchronize()      # behind the network, which waited for the batch's decode and status copy
+        if self._jpeg_idx[ticket]:
+            idx = self._jpeg_idx[ticket]
+            check_jpeg_status(self._jpeg_status[ticket][:len(idx)].numpy(), idx)
         dets, counts = DetectionGather.split(self._host[ticket], self.gather.C, self.gather.K, DET_WORDS)
         n = self._rows[ticket]
         return (dets, counts) if n is None else (dets[:n], counts[:n])

@@ -8,6 +8,14 @@ returns the uint8 network input; the ``img / np.max(img)`` normalisation is fuse
 ``letterbox_batch_device`` does the same for a list of host images of different sizes in one launch: ``BatchLayout`` packs
 them back to back into one pinned staging buffer (``Staging``), one H2D copy moves the whole batch and
 ``k2y_letterbox_u8_batch`` letterboxes every image into one uint8 [n, in_h, in_w, 3] tensor.
+
+A batch entry may also be a whole image file (``bytes``, ``bytearray`` or ``memoryview``).  Baseline JPEGs the GPU decoder
+takes (``inspect_jpeg``) travel compressed: their bytes and the batch's descriptor blob (``k2y_jpeg_plan``) go into the same
+pinned buffer, one H2D copy moves them, and ``k2y_jpeg_decode`` writes their RGB pixels into the packed buffer at their
+``BatchLayout`` offsets, in front of the letterbox launch, with the bytes PIL gives.  Every other file is decoded on the host
+inside the call, as ``Helper._read_img`` does (the slow path); so is a JPEG that does not end with its EOI marker, so that a
+truncated file raises as it does with PIL.  Corrupt entropy data in a complete file sets the image's status word, which
+``letterbox_batch_device`` and ``DetectionPipeline.collect`` turn into a ``K2YError``.  ``decode_jpeg_batch`` returns the decoded pixels themselves.
 """
 from __future__ import annotations
 
@@ -17,7 +25,8 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from ._lib import check, lib
+from ._lib import JpegInfo, K2YError, check, lib
+from .helper import read_image
 
 
 def letterbox_params(img_hw, in_hw):
@@ -55,39 +64,140 @@ def letterbox_device(img_u8: torch.Tensor, in_hw, out: Optional[torch.Tensor] = 
 ALIGN = 16   # byte alignment of each packed image (pass 1 of the batch kernel then reads 16 bytes at a time)
 
 
+ENCODED = (bytes, bytearray, memoryview)
+
+
+def _file_bytes(data) -> np.ndarray:
+    """A whole image file as a read-only uint8 array over the caller's buffer (no copy)."""
+    return np.frombuffer(data, dtype=np.uint8)
+
+
+def _jpeg_info(buf: np.ndarray) -> Optional[JpegInfo]:
+    """The header of a JPEG file, or None when `buf` is not one the parser accepts (other formats, malformed headers)."""
+    if buf.size < 4 or buf[0] != 0xFF or buf[1] != 0xD8:
+        return None
+    info = JpegInfo()
+    if lib.k2y_jpeg_inspect(buf.ctypes.data, buf.size, ctypes.byref(info)) != 0:
+        return None
+    return info
+
+
+def inspect_jpeg(data):
+    """Header of a JPEG file held in memory (``bytes``, ``bytearray`` or ``memoryview``), read on the host:
+    ``(h, w, gpu_decodable, reason)``; `reason` says why a valid file is not for the GPU decoder ("" when it is).
+    Raises ``K2YError`` for a file that is not a JPEG or whose headers are malformed (the message names the marker)."""
+    if not isinstance(data, ENCODED):
+        raise ValueError(f"expected the bytes of a file, got {type(data).__name__}")
+    buf = _file_bytes(data)
+    info = JpegInfo()
+    check(lib.k2y_jpeg_inspect(buf.ctypes.data, buf.size, ctypes.byref(info)))
+    return int(info.height), int(info.width), bool(info.gpu_decodable), info.reason.decode()
+
+
+def _gpu_route(buf: np.ndarray) -> Optional[JpegInfo]:
+    """The header of `buf` when the batch routes send it to the GPU decoder, else None.  A file must be GPU-decodable and end
+    with its EOI marker: a truncated file (or one with data appended after EOI) goes to the host decoder, which reports the
+    truncation as PIL does instead of decoding pixels the missing data would have set."""
+    info = _jpeg_info(buf)
+    if info is None or not info.gpu_decodable or buf[-2] != 0xFF or buf[-1] != 0xD9:
+        return None
+    return info
+
+
+def gpu_decodable(data) -> bool:
+    """True when `data` (the bytes of a file) goes to the GPU decoder in ``submit_images``: a JPEG the decoder takes, ending
+    with its EOI marker.  False for anything else, malformed or truncated files included."""
+    return _gpu_route(_file_bytes(data)) is not None
+
+
 def _check_images(images) -> None:
     if not isinstance(images, (list, tuple)) or len(images) == 0:
-        raise ValueError("expected a non-empty list of host uint8 [h, w, 3] arrays")
+        raise ValueError("expected a non-empty list of host uint8 [h, w, 3] arrays or image files")
     for i, im in enumerate(images):
+        if isinstance(im, ENCODED):
+            if not memoryview(im).c_contiguous:
+                raise ValueError(f"image {i}: the memoryview of a file must be contiguous")
+            if memoryview(im).nbytes == 0:
+                raise ValueError(f"image {i}: empty file")
+            continue
         if not isinstance(im, np.ndarray) or im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3 or im.shape[0] < 1 or im.shape[1] < 1:
             desc = f"{im.dtype} {im.shape}" if isinstance(im, np.ndarray) else type(im).__name__
-            raise ValueError(f"image {i}: expected a host numpy uint8 [h, w, 3] array, got {desc}")
+            raise ValueError(f"image {i}: expected a host numpy uint8 [h, w, 3] array or the bytes of an image file, got {desc}")
+
+
+def _host_decode(buf: np.ndarray, i: int) -> np.ndarray:
+    import io
+    try:
+        return read_image(io.BytesIO(buf.tobytes()))
+    except Exception as e:  # PIL raises several types for unreadable files
+        raise ValueError(f"image {i}: cannot decode the file: {e}") from e
 
 
 class BatchLayout:
     """Where each image of a ragged batch lies in the packed buffer, and its letterbox descriptor.
 
     ``offsets`` int64 [n] (multiples of ``ALIGN``), ``hw`` int32 [n, 2] (h, w), ``matrices`` float64 [n, 6] (the first two
-    rows of ``letterbox_params``' inverse matrix), ``nbytes`` the packed size."""
+    rows of ``letterbox_params``' inverse matrix), ``nbytes`` the packed size.
 
-    def __init__(self, images: Sequence[np.ndarray], in_hw):
+    Entries that are image files are resolved here: ``jpeg`` lists (index, file bytes) of the JPEGs the GPU decodes
+    (``gpu_decodable``), whose size comes from their header; every other file is decoded on the host now, and ``arrays[i]``
+    holds the host pixels of entry i (None for a GPU JPEG).  ``jpeg_plan`` is where the JPEGs' bytes and their descriptor blob
+    go in the staging buffer, behind the packed pixels (``_jpeg_layout``)."""
+
+    def __init__(self, images: Sequence, in_hw):
         _check_images(images)
         n = len(images)
         self.in_hw = (int(in_hw[0]), int(in_hw[1]))
-        self.hw = np.array([im.shape[:2] for im in images], dtype=np.int32).reshape(n, 2)
+        self.arrays: List[Optional[np.ndarray]] = []
+        self.jpeg = []
+        shapes = []
+        for i, im in enumerate(images):
+            if isinstance(im, ENCODED):
+                buf = _file_bytes(im)
+                info = _gpu_route(buf)
+                if info is not None:
+                    self.jpeg.append((i, buf))
+                    self.arrays.append(None)
+                    shapes.append((info.height, info.width))
+                    continue
+                im = _host_decode(buf, i)
+            self.arrays.append(im)
+            shapes.append(im.shape[:2])
+        self.hw = np.array(shapes, dtype=np.int32).reshape(n, 2)
         sizes = self.hw[:, 0].astype(np.int64) * self.hw[:, 1] * 3
         padded = (sizes + ALIGN - 1) // ALIGN * ALIGN
         self.offsets = np.concatenate([[0], np.cumsum(padded)[:-1]]).astype(np.int64)
         self.nbytes = int(padded.sum())
         self.matrices = np.array([letterbox_params((int(h[0]), int(h[1])), self.in_hw)[2][:2].reshape(-1) for h in self.hw], dtype=np.float64)
+        self.jpeg_plan = None
+        if self.jpeg:
+            self.jpeg_dst = self.offsets[[i for i, _ in self.jpeg]].astype(np.int64)
+            self.jpeg_plan = _jpeg_layout([f for _, f in self.jpeg], self.jpeg_dst, (self.nbytes + ALIGN - 1) // ALIGN * ALIGN)
 
     def __len__(self) -> int:
         return len(self.hw)
 
-    def pack(self, images: Sequence[np.ndarray], host: np.ndarray) -> None:
-        """Copies `images` into the uint8 buffer `host` (at least ``nbytes`` long) at their offsets."""
-        for im, off, (h, w) in zip(images, self.offsets, self.hw):
-            np.copyto(host[off:off + h * w * 3].reshape(h, w, 3), im)
+    def pack(self, images: Sequence, host: np.ndarray) -> None:
+        """Copies the host pixels of `images` (the entries this layout was made of) into the uint8 buffer `host` (at least
+        ``nbytes`` long) at their offsets.  The GPU JPEGs' ranges are left as they are: the decoder fills them on the device."""
+        assert len(images) == len(self.arrays)
+        for im, off, (h, w) in zip(self.arrays, self.offsets, self.hw):
+            if im is not None:
+                np.copyto(host[off:off + h * w * 3].reshape(h, w, 3), im)
+
+    def host_ranges(self):
+        """[begin, end) ranges of the packed buffer that hold the host-side images, one per run of consecutive ones (the GPU
+        JPEGs' ranges between them are filled on the device and need no copy)."""
+        out = []
+        for i, a in enumerate(self.arrays):
+            if a is None:
+                continue
+            b, e = int(self.offsets[i]), int(self.offsets[i] + self.hw[i, 0] * self.hw[i, 1] * 3)
+            if out and self.arrays[i - 1] is not None:
+                out[-1] = (out[-1][0], e)
+            else:
+                out.append((b, e))
+        return out
 
 
 class Staging:
@@ -100,6 +210,17 @@ class Staging:
         self.host: Optional[torch.Tensor] = None
         self.dev: Optional[torch.Tensor] = None
         self.minmax: Optional[torch.Tensor] = None
+        self.workspace: Optional[torch.Tensor] = None   # k2y_jpeg_decode's
+        self.status: Optional[torch.Tensor] = None      # int32 [n, 4] per decoded JPEG (k2y_jpeg_decode)
+
+    def reserve_jpeg(self, workspace_bytes: int, n: int) -> None:
+        with torch.cuda.stream(self.stream):
+            if self.workspace is None or self.workspace.numel() < workspace_bytes:
+                cap = max(workspace_bytes, 2 * self.workspace.numel() if self.workspace is not None else 0)
+                self.workspace = torch.empty((cap,), dtype=torch.uint8, device=self.device)
+            if self.status is None or self.status.shape[0] < n:
+                self.status = torch.empty((max(n, 2 * self.status.shape[0] if self.status is not None else 0), 4), dtype=torch.int32,
+                                          device=self.device)
 
     def reserve(self, nbytes: int, n: int) -> None:
         if self.host is None or self.host.numel() < nbytes:
@@ -123,18 +244,72 @@ def _check_out(t: Optional[torch.Tensor], n: int, shape, dtype, name: str, devic
         raise ValueError(f"{n} images do not fit {name}, which holds {t.shape[0]}")
 
 
-def letterbox_packed(layout: BatchLayout, images: Sequence[np.ndarray], staging: Staging, out: torch.Tensor,
+def _jpeg_plan(files: Sequence[np.ndarray], src_offsets: np.ndarray, dst_offsets: np.ndarray, blob: Optional[np.ndarray]) -> int:
+    """k2y_jpeg_plan: the blob's size (blob None), or the blob written into `blob` (16-byte aligned)."""
+    n = len(files)
+    ptrs = (ctypes.c_void_p * n)(*[f.ctypes.data for f in files])
+    sizes = (ctypes.c_size_t * n)(*[f.size for f in files])
+    nbytes = ctypes.c_size_t()
+    ll = ctypes.POINTER(ctypes.c_longlong)
+    check(lib.k2y_jpeg_plan(ptrs, sizes, n, src_offsets.ctypes.data_as(ll), dst_offsets.ctypes.data_as(ll),
+                            blob.ctypes.data if blob is not None else None, blob.size if blob is not None else 0, ctypes.byref(nbytes)))
+    return nbytes.value
+
+
+def stage_jpegs(files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: Staging, plan, dst: torch.Tensor) -> None:
+    """Puts the JPEG `files` and their descriptor blob into ``staging.host`` where `plan` (``_jpeg_layout``) places them
+    (``staging.reserve`` of the whole batch first), copies that range to ``staging.dev`` in one H2D copy and decodes the files
+    into `dst` (a device uint8 buffer) at `dst_offsets`, on ``staging.stream``.  Per-image status words land in
+    ``staging.status``."""
+    n = len(files)
+    src_offsets, blob_at, blob_bytes, end = plan
+    base = int(src_offsets[0])
+    host = staging.host.numpy()
+    for f, off in zip(files, src_offsets):
+        host[off:off + f.size] = f
+    blob = host[blob_at:blob_at + blob_bytes]
+    _jpeg_plan(files, src_offsets, dst_offsets, blob)
+    ws = ctypes.c_size_t()
+    check(lib.k2y_jpeg_workspace_bytes(blob.ctypes.data, ctypes.byref(ws)))
+    staging.reserve_jpeg(ws.value, n)
+    st = staging.stream
+    with torch.cuda.stream(st):
+        staging.dev[base:end].copy_(staging.host[base:end], non_blocking=True)
+        check(lib.k2y_jpeg_decode(blob.ctypes.data, staging.dev.data_ptr() + blob_at, staging.dev.data_ptr(), dst.data_ptr(),
+                                  staging.workspace.data_ptr(), staging.workspace.numel(), staging.status.data_ptr(),
+                                  ctypes.c_void_p(st.cuda_stream)))
+
+
+def _jpeg_layout(files: Sequence[np.ndarray], dst_offsets: np.ndarray, base: int):
+    """Offsets of the files and of the blob in the staging buffer from `base` on, the blob's size and the end of the range.
+    The blob's size query parses every header: a file the plan refuses raises ``ValueError`` here."""
+    sizes = np.array([f.size for f in files], np.int64)
+    padded = (sizes + ALIGN - 1) // ALIGN * ALIGN
+    src_offsets = (base + np.concatenate([[0], np.cumsum(padded)[:-1]])).astype(np.int64)
+    blob_at = int(base + padded.sum())
+    try:
+        blob_bytes = _jpeg_plan(files, src_offsets, dst_offsets, None)
+    except K2YError as e:
+        raise ValueError(str(e)) from e
+    return src_offsets, blob_at, blob_bytes, blob_at + blob_bytes
+
+
+def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, out: torch.Tensor,
                      image_hw_out: Optional[torch.Tensor]) -> None:
     """Packs `images` into ``staging.host``, copies them to the device and letterboxes them into ``out[:n]`` (and their sizes
-    into ``image_hw_out[:n]``), all on ``staging.stream``.  The host buffer is reused by the next call: wait for this copy
+    into ``image_hw_out[:n]``), all on ``staging.stream``.  GPU-decodable JPEGs travel compressed behind the packed pixels and
+    are decoded into their place first (``stage_jpegs``).  The host buffer is reused by the next call: wait for this copy
     before packing into it again."""
     n = len(layout)
-    staging.reserve(layout.nbytes, n)
+    staging.reserve(layout.jpeg_plan[3] if layout.jpeg else layout.nbytes, n)
     layout.pack(images, staging.host.numpy())
     in_h, in_w = layout.in_hw
     st = staging.stream
     with torch.cuda.stream(st):
-        staging.dev[:layout.nbytes].copy_(staging.host[:layout.nbytes], non_blocking=True)
+        for b, e in layout.host_ranges():
+            staging.dev[b:e].copy_(staging.host[b:e], non_blocking=True)
+        if layout.jpeg:
+            stage_jpegs([f for _, f in layout.jpeg], layout.jpeg_dst, staging, layout.jpeg_plan, staging.dev)
         offs = layout.offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong))
         hw = layout.hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int))
         mats = layout.matrices.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
@@ -143,12 +318,15 @@ def letterbox_packed(layout: BatchLayout, images: Sequence[np.ndarray], staging:
                                          ctypes.c_void_p(st.cuda_stream)))
 
 
-def letterbox_batch_device(images: List[np.ndarray], in_hw, out: Optional[torch.Tensor] = None,
+def letterbox_batch_device(images: List, in_hw, out: Optional[torch.Tensor] = None,
                            image_hw_out: Optional[torch.Tensor] = None, stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
-    """images: host numpy uint8 [h, w, 3] RGB arrays of any sizes -> CUDA uint8 [n, in_h, in_w, 3] letterboxed (zero fill), the
+    """images: host numpy uint8 [h, w, 3] RGB arrays of any sizes, or image files (``bytes``, ``bytearray``, ``memoryview``:
+    see ``BatchLayout``) -> CUDA uint8 [n, in_h, in_w, 3] letterboxed (zero fill), the
     same bytes ``letterbox_device`` gives each image.  One pinned staging buffer, one H2D copy, one batched letterbox launch on
     `stream` (default: the current stream), asynchronous.  `out` ([N >= n, in_h, in_w, 3] uint8, e.g. a network's bound input)
-    receives the images in its first n rows; `image_hw_out` ([N >= n, 2] float32), if given, receives each image's (h, w)."""
+    receives the images in its first n rows; `image_hw_out` ([N >= n, 2] float32), if given, receives each image's (h, w).
+    When the batch holds JPEGs decoded on the GPU, the call synchronises `stream` to read their status words and raises
+    ``K2YError`` if one of them was corrupt (``check_jpeg_status``)."""
     in_h, in_w = int(in_hw[0]), int(in_hw[1])
     layout = BatchLayout(images, (in_h, in_w))
     n = len(layout)
@@ -159,6 +337,57 @@ def letterbox_batch_device(images: List[np.ndarray], in_hw, out: Optional[torch.
     if out is None:
         with torch.cuda.stream(st):
             out = torch.empty((n, in_h, in_w, 3), dtype=torch.uint8, device=device)
+    staging = Staging(device, st)
     with torch.cuda.device(device):
-        letterbox_packed(layout, images, Staging(device, st), out, image_hw_out)
+        letterbox_packed(layout, images, staging, out, image_hw_out)
+        if layout.jpeg:
+            with torch.cuda.stream(st):
+                check_jpeg_status(staging.status[:len(layout.jpeg)].cpu().numpy(), [i for i, _ in layout.jpeg])
     return out
+
+
+def decode_jpeg_batch(files: Sequence, stream: Optional[torch.cuda.Stream] = None, with_status: bool = False):
+    """GPU-decodable JPEG files (``bytes``, ``bytearray``, ``memoryview``) -> list of CUDA uint8 [h, w, 3] RGB views of one
+    packed device buffer, byte for byte what ``Helper._read_img`` (PIL) gives.  One pinned staging buffer, one H2D copy and
+    one launch per decode stage on `stream` (default: the current stream), then a synchronise to read the per-image status.
+    A file the GPU decoder does not take raises ``ValueError`` before anything is enqueued; corrupt entropy data raises
+    ``K2YError`` naming the images, unless `with_status`, which returns (views, status int32 [n, 4]: error bits, max / sum of
+    synchronisation rounds per window, windows) instead."""
+    if not isinstance(files, (list, tuple)) or len(files) == 0:
+        raise ValueError("expected a non-empty list of JPEG files")
+    bufs, shapes = [], []
+    for i, f in enumerate(files):
+        if not isinstance(f, ENCODED):
+            raise ValueError(f"file {i}: expected bytes, bytearray or memoryview, got {type(f).__name__}")
+        buf = _file_bytes(f)
+        info = _jpeg_info(buf)
+        if info is None or not info.gpu_decodable:
+            why = info.reason.decode() if info is not None else "not a well-formed JPEG file"
+            raise ValueError(f"file {i}: not decodable on the GPU: {why}")
+        bufs.append(buf)
+        shapes.append((int(info.height), int(info.width)))
+    sizes = np.array([h * w * 3 for h, w in shapes], np.int64)
+    padded = (sizes + ALIGN - 1) // ALIGN * ALIGN
+    offsets = np.concatenate([[0], np.cumsum(padded)[:-1]]).astype(np.int64)
+    device = torch.device("cuda", torch.cuda.current_device())
+    st = stream if stream is not None else torch.cuda.current_stream(device)
+    staging = Staging(device, st)
+    plan = _jpeg_layout(bufs, offsets, int(padded.sum()))
+    staging.reserve(plan[3], len(bufs))
+    with torch.cuda.stream(st):
+        stage_jpegs(bufs, offsets, staging, plan, staging.dev)
+        status = staging.status[:len(bufs)].cpu().numpy()
+    out = [staging.dev[o:o + h * w * 3].view(h, w, 3) for o, (h, w) in zip(offsets, shapes)]
+    if with_status:
+        return out, status
+    check_jpeg_status(status, range(len(bufs)))
+    return out
+
+
+def check_jpeg_status(status: np.ndarray, images) -> None:
+    """Raises ``K2YError`` naming the images whose entropy-coded data was corrupt or ended early.  `status`: the decode's
+    int32 [n, 4] words of the GPU-decoded JPEGs, `images`: their positions in the caller's batch."""
+    bad = [(int(i), int(w)) for i, w in zip(images, status[:, 0]) if w]
+    if bad:
+        what = {1: "invalid Huffman code", 2: "entropy-coded data ends early", 3: "invalid Huffman code, data ends early"}
+        raise K2YError("corrupt JPEG data: " + ", ".join(f"image {i}: {what.get(w, w)}" for i, w in bad))

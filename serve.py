@@ -7,12 +7,15 @@ gathered detections, one JSON line per image.  The GPU analogue of the firmware'
                                     --anchors data/voc_anchor.npy --batch 32 --obj_thresh 0.7 --iou_thresh 0.5 --out dets.jsonl]
     python -m torch.distributed.run --nproc-per-node 8 serve.py ...        # one rank per GPU, NCCL all-gather of the records
 
-Per global batch of world*batch images: every rank decodes ITS images on the host (PIL, in a pool of --decode_threads
-threads, one batch ahead), hands them to DetectionPipeline.submit_images (one packed H2D copy, one batched letterbox launch
-into its uint8 input buffer, network + decode + NMS), and ONE all-gather completes the record blocks on every rank; two
-batches are in flight, and rank 0 writes the lines in file order.
+Per global batch of world*batch images: every rank reads ITS files in a pool of --decode_threads threads, one batch ahead.
+Baseline JPEGs the GPU decoder takes (preprocess.gpu_decodable) stay compressed; every other file is decoded there by PIL as
+Helper._read_img does.  DetectionPipeline.submit_images takes both (one packed H2D copy, the JPEG decode on the GPU, one
+batched letterbox launch into its uint8 input buffer, network + decode + NMS), and ONE all-gather completes the record blocks
+on every rank; two batches are in flight, and rank 0 writes the lines in file order.  The GPU decode gives the bytes PIL
+gives, so the lines do not depend on which route a file took.
 """
 import argparse
+import io
 import json
 import os
 import sys
@@ -24,8 +27,9 @@ import torch
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-from k210_yolo_framework_b200 import Helper  # noqa: E402
 from k210_yolo_framework_b200.dist import shard_range  # noqa: E402
+from k210_yolo_framework_b200.helper import read_image  # noqa: E402
+from k210_yolo_framework_b200.preprocess import gpu_decodable  # noqa: E402
 from k210_yolo_framework_b200.pipeline import DetectionPipeline  # noqa: E402
 
 EXTS = (".jpg", ".jpeg", ".png", ".bmp")
@@ -38,6 +42,13 @@ def list_images(path):
         return [l.strip() for l in fh if l.strip()]
 
 
+def load_image(path):
+    """The file's bytes when the GPU decodes it, else its pixels decoded on the host (Helper._read_img)."""
+    with open(path, "rb") as fh:
+        data = fh.read()
+    return data if gpu_decodable(data) else read_image(io.BytesIO(data))
+
+
 def serve(args, out_fh=None):
     import torch.distributed as dist
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -48,8 +59,6 @@ def serve(args, out_fh=None):
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     anchors = np.load(args.anchors)
     H, W = args.image_size
-    out_hw = [(H // 32 * 2 ** l, W // 32 * 2 ** l) for l in range(len(anchors))]
-    h = Helper(None, args.class_num, anchors, np.reshape(np.array(args.image_size), (-1, 2)), np.reshape(np.array(out_hw), (-1, 2)))
     pipe = DetectionPipeline(args.model_def, (H, W), anchors, args.class_num, args.depth_multiplier, args.batch, args.obj_thresh,
                              args.iou_thresh, 30, device=local, world=world, rank=rank)
     pipe.engine.load_weights(args.ckpt)
@@ -77,7 +86,7 @@ def serve(args, out_fh=None):
 
     with ThreadPoolExecutor(max(1, int(getattr(args, "decode_threads", 4)))) as pool:
         def decode(chunk):      # this rank's images of a global batch, decoding in the pool
-            return [pool.submit(h._read_img, p) for p in chunk[rank * B:(rank + 1) * B]]
+            return [pool.submit(load_image, p) for p in chunk[rank * B:(rank + 1) * B]]
 
         pending = deque()
         nxt = decode(chunks[0]) if chunks else []
@@ -106,7 +115,7 @@ def main():
     ap.add_argument("--batch", type=int, default=32, help="images per GPU per step")
     ap.add_argument("--obj_thresh", type=float, default=0.7)
     ap.add_argument("--iou_thresh", type=float, default=0.5)
-    ap.add_argument("--decode_threads", type=int, default=4, help="host threads decoding the next batch's files (PIL)")
+    ap.add_argument("--decode_threads", type=int, default=4, help="host threads reading the next batch's files and decoding those the GPU does not (PIL)")
     ap.add_argument("--out", default="-")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
