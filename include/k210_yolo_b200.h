@@ -311,6 +311,39 @@ int k2y_jpeg_decode(const void *blob_host, const void *blob_dev, const unsigned 
 int k2y_pr_counts(const float *y_true_dev, const float *y_pred_dev, long long n_boxes, int entry_floats, float threshold,
                   int apply_sigmoid, unsigned long long *counts_dev, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * Detection AP / mAP over an annotated image list (VOC matching rule, all-point and 11-point AP), on the device.  The
+ * protocol is written down in oracle/ap_ref.py: IoU without a "+1 pixel" term, no "difficult" objects, ties in score keep
+ * stream order.  An evaluator holds the per-class ground-truth counts and one slot per (image, class, k < max_per_class)
+ * of every image matched so far (score bits + one TP bit per threshold); the store grows by doubling.
+ *   k2y_ap_create     class_num 1..1024, max_per_class >= 1, 1..16 IoU thresholds in (0, 1] (compared in float32).
+ *   k2y_ap_match      one update of n_images, asynchronous on `stream` (one kernel): dets_dev / counts_dev as
+ *                     k2y_detect_keras_strided writes them (same per-image strides, device memory), gt_dev the images'
+ *                     ground truth packed as [total][5] float32 (class, ymin, xmin, ymax, xmax) in image pixels, image i's
+ *                     rows at [gt_offsets_dev[i], gt_offsets_dev[i+1]) (int64, device), max_gt_per_image >= every image's
+ *                     row count.  The inputs may be reused once the stream has passed the call.
+ *   k2y_ap_result     ranks every stored detection by (class, score descending, stream order) and reduces the curves;
+ *                     synchronous.  ap_host [T][C], ap07_host [C] (first threshold), npos_host [C]: float64 / int64; AP is NaN
+ *                     for a class without ground truth.  status_host: K2Y_AP_* bits of anything invalid seen since the last
+ *                     reset (the APs are then meaningless).
+ *   k2y_ap_reset      forgets every update (keeps the store's memory).
+ *   k2y_ap_tp_flags   n_images matched so far; with tp_host != NULL also copies the TP bits, uint16 [n_images][C][K] (bit t:
+ *                     TP at threshold t, 0 past each count), synchronous.
+ * Every call of one evaluator is ordered after the previous one, whatever streams they use.
+ * ---------------------------------------------------------------------------------------- */
+#define K2Y_AP_BAD_SCORE 1     /* a record within its count has a NaN score or one with the sign bit set */
+#define K2Y_AP_BAD_COUNT 2     /* a count outside [0, max_per_class] (clamped) */
+#define K2Y_AP_GT_OVERFLOW 4   /* an image has more ground-truth rows than max_gt_per_image (the rest were ignored) */
+typedef struct k2y_ap k2y_ap;
+int k2y_ap_create(int class_num, int max_per_class, const float *iou_thresholds, int n_thresholds, int device, k2y_ap **out);
+int k2y_ap_destroy(k2y_ap *ap);
+int k2y_ap_match(k2y_ap *ap, const int32_t *dets_dev, const int32_t *counts_dev, long long det_image_stride_words,
+                 long long count_image_stride_words, int n_images, const float *gt_dev, const long long *gt_offsets_dev,
+                 int max_gt_per_image, void *stream);
+int k2y_ap_result(k2y_ap *ap, double *ap_host, double *ap07_host, long long *npos_host, unsigned *status_host, void *stream);
+int k2y_ap_reset(k2y_ap *ap, void *stream);
+int k2y_ap_tp_flags(k2y_ap *ap, uint16_t *tp_host, long long capacity, long long *n_images, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

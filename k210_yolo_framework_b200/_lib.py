@@ -117,6 +117,13 @@ _SIGNATURES = {
                               c_void_p, c_size_t, POINTER(c_size_t)]),
     "k2y_jpeg_workspace_bytes": (c_int, [c_void_p, POINTER(c_size_t)]),
     "k2y_jpeg_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "k2y_ap_create": (c_int, [c_int, c_int, POINTER(c_float), c_int, c_int, POINTER(c_void_p)]),
+    "k2y_ap_destroy": (c_int, [c_void_p]),
+    "k2y_ap_match": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_longlong, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_int,
+                             c_void_p]),
+    "k2y_ap_result": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(ctypes.c_uint), c_void_p]),
+    "k2y_ap_reset": (c_int, [c_void_p, c_void_p]),
+    "k2y_ap_tp_flags": (c_int, [c_void_p, c_void_p, ctypes.c_longlong, POINTER(ctypes.c_longlong), c_void_p]),
 }
 # include/region_layer.h (ABI-compatible firmware API)
 _REGION_ABI = ["region_layer_init", "region_layer_deinit", "region_layer_run", "region_layer_draw_boxes"]

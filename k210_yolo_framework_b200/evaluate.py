@@ -1,13 +1,25 @@
-"""Precision / recall of the confidence channel, as the reference's Keras metrics define them
-(/root/reference/tools/custom.py:13-75 ``Yolo_Precision`` / ``Yolo_Recall``), counted on the GPU (k2y_pr_counts)."""
+"""Evaluation on the GPU.
+
+``PrecisionRecall``: precision / recall of the confidence channel, as the reference's Keras metrics define them
+(/root/reference/tools/custom.py:13-75 ``Yolo_Precision`` / ``Yolo_Recall``), counted by k2y_pr_counts.
+
+``DetectionAP``: per-class AP and mAP of the detection records against annotated boxes (VOC matching rule, all-point and
+VOC 2007 11-point AP, any set of IoU thresholds), matched, ranked and reduced by the k2y_ap_* kernels.  The protocol is
+that of oracle/ap_ref.py: IoU without a "+1 pixel" term, and every object counts (the annotation lists carry no
+"difficult" flag).  ``load_voc_annotations`` reads the lists make_voc_list.py writes.
+"""
 from __future__ import annotations
 
 import ctypes
-from typing import Sequence, Tuple
+from typing import List, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from ._lib import check, lib, require_cuda
+
+AP_STATUS = {1: "a record has a negative or NaN score", 2: "a record count is outside [0, max_per_class]",
+             4: "an image has more ground-truth boxes than the match kernel was told"}
 
 
 class PrecisionRecall:
@@ -34,3 +46,123 @@ class PrecisionRecall:
 
     def reset(self) -> None:
         self.counts.zero_()
+
+
+def load_voc_annotations(npy_path: str) -> Tuple[List[str], List[np.ndarray], List[Tuple[int, int]]]:
+    """A make_voc_list.py list (rows ``(path, labels [n, 5] = (class, x, y, w, h) relative, (h, w))``) as
+    ``(paths, labels, hw)``."""
+    rows = np.load(npy_path, allow_pickle=True)
+    paths, labels, hw = [], [], []
+    for row in rows:
+        if len(row) != 3:
+            raise ValueError(f"{npy_path}: rows must be (path, labels, (h, w)), got {len(row)} fields")
+        paths.append(str(row[0]))
+        labels.append(np.asarray(row[1], np.float64))
+        h, w = (int(v) for v in np.asarray(row[2]).reshape(2))
+        hw.append((h, w))
+    return paths, labels, hw
+
+
+def voc_gt_boxes(labels, hw, class_num: int) -> np.ndarray:
+    """One annotation row's labels ``[n, 5] (class, x, y, w, h)`` relative to an image of size ``hw = (H, W)`` as
+    ``[n, 5]`` float32 ``(class, ymin, xmin, ymax, xmax)`` in image pixels: the corner order and frame of the detection
+    records, computed in float64 and rounded once.  ``ValueError`` for a malformed array or a class outside [0, C)."""
+    lab = np.asarray(labels, dtype=np.float64)
+    if lab.size == 0:
+        if lab.shape not in ((0, 5), (0,)):
+            raise ValueError(f"an empty label array must have shape (0, 5) or (0,), not {lab.shape}")
+        return np.zeros((0, 5), np.float32)
+    if lab.ndim != 2 or lab.shape[1] != 5:
+        raise ValueError(f"labels must be [n, 5] (class, x, y, w, h), not {lab.shape}")
+    cls = lab[:, 0]
+    if not np.all((cls == np.floor(cls)) & (cls >= 0) & (cls < class_num)):
+        raise ValueError(f"class ids must be integers in [0, {class_num}); got {cls.tolist()}")
+    H, W = (float(v) for v in np.asarray(hw, np.float64).reshape(2))
+    x, y, w, h = lab[:, 1], lab[:, 2], lab[:, 3], lab[:, 4]
+    return np.stack([cls, (y - h / 2) * H, (x - w / 2) * W, (y + h / 2) * H, (x + w / 2) * W], 1).astype(np.float32)
+
+
+class DetectionAP:
+    """Accumulates detection records and ground truth over ``update`` calls; ``result`` ranks and reduces on the GPU.
+
+    ``iou_thresholds``: 1 to 16 matching thresholds in (0, 1]; the 11-point AP is reported at the first.  Every call runs on
+    the current CUDA stream."""
+
+    def __init__(self, class_num: int, max_per_class: int, iou_thresholds: Sequence[float] = (0.5,), device=None):
+        require_cuda()
+        self.C, self.K = int(class_num), int(max_per_class)
+        self.thresholds = [float(t) for t in iou_thresholds]
+        if not 1 <= len(self.thresholds) <= 16 or not all(0.0 < t <= 1.0 for t in self.thresholds):
+            raise ValueError(f"1 to 16 IoU thresholds in (0, 1] are needed, got {self.thresholds}")
+        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device or "cuda")
+        self.device = torch.device("cuda", torch.cuda.current_device() if dev.index is None else dev.index)
+        thr = (ctypes.c_float * len(self.thresholds))(*self.thresholds)
+        h = ctypes.c_void_p()
+        check(lib.k2y_ap_create(self.C, self.K, thr, len(self.thresholds), self.device.index, ctypes.byref(h)))
+        self._h = h
+
+    def _stream(self):
+        return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def update(self, dets: torch.Tensor, counts: torch.Tensor, gt: Sequence) -> None:
+        """dets int32 ``[N, C, K, 6]`` (dense per image) and counts int32 ``[N, C]`` as ``DetectionPipeline`` returns them:
+        the device views of ``step_device`` or the pinned host views of ``collect``, strided per image.  gt: one
+        ``(labels, (h, w))`` pair per image, the last two fields of an annotation row (``load_voc_annotations``).  Device
+        records are read asynchronously on the current stream; host records have been copied when this returns."""
+        n = len(gt)
+        if (dets.dtype != torch.int32 or counts.dtype != torch.int32 or dets.dim() != 4 or counts.dim() != 2
+                or tuple(dets.shape) != (n, self.C, self.K, 6) or tuple(counts.shape) != (n, self.C)
+                or tuple(dets.stride()[1:]) != (self.K * 6, 6, 1) or counts.stride(1) != 1 or dets.is_cuda != counts.is_cuda):
+            raise ValueError(f"expected int32 dets [{n}, {self.C}, {self.K}, 6] (dense per image) and counts [{n}, {self.C}] "
+                             f"on one side of the bus, one per ground-truth entry; got {tuple(dets.shape)} / {tuple(counts.shape)}")
+        if n == 0:
+            return
+        boxes = [voc_gt_boxes(labels, hw, self.C) for labels, hw in gt]
+        sizes = np.array([len(b) for b in boxes], np.int64)
+        off = np.zeros(n + 1, np.int64)
+        np.cumsum(sizes, out=off[1:])
+        with torch.cuda.device(self.device):
+            if dets.is_cuda:
+                if dets.device != self.device or counts.device != self.device:
+                    raise ValueError(f"records on {dets.device}, evaluator on {self.device}")
+            else:   # a blocking copy: the host views may be overwritten as soon as this returns
+                dets, counts = dets.to(self.device), counts.to(self.device)
+            packed = torch.from_numpy(np.concatenate(boxes + [np.zeros((1, 5), np.float32)])).to(self.device)
+            offsets = torch.from_numpy(off).to(self.device)
+            check(lib.k2y_ap_match(self._h, dets.data_ptr(), counts.data_ptr(), dets.stride(0), counts.stride(0), n,
+                                   packed.data_ptr(), offsets.data_ptr(), int(sizes.max()), self._stream()))
+
+    def result(self) -> dict:
+        """``{"ap": [T, C], "ap07": [C], "npos": [C], "map": [T], "map07": float}``: all-point AP per threshold and class, the
+        VOC 2007 11-point AP at the first threshold, ground-truth counts, and the means over the classes with ground
+        truth (AP is NaN for the others).  ``ValueError`` if an update held an invalid record."""
+        T, C = len(self.thresholds), self.C
+        ap, ap07, npos = np.zeros((T, C)), np.zeros(C), np.zeros(C, np.int64)
+        status = ctypes.c_uint()
+        with torch.cuda.device(self.device):
+            check(lib.k2y_ap_result(self._h, ap.ctypes.data, ap07.ctypes.data, npos.ctypes.data, ctypes.byref(status),
+                                    self._stream()))
+        if status.value:
+            raise ValueError("DetectionAP: " + "; ".join(m for bit, m in AP_STATUS.items() if status.value & bit))
+        valid = npos > 0
+        mean = (lambda v: float(np.mean(v[valid])) if valid.any() else float("nan"))
+        return {"ap": ap, "ap07": ap07, "npos": npos, "map": np.array([mean(ap[t]) for t in range(T)]), "map07": mean(ap07)}
+
+    def tp_flags(self) -> np.ndarray:
+        """uint16 ``[images, C, K]``: bit t of entry (image, class, k) is set when record k was a TP at threshold t."""
+        n = ctypes.c_longlong()
+        check(lib.k2y_ap_tp_flags(self._h, None, 0, ctypes.byref(n), self._stream()))
+        out = np.zeros((n.value, self.C, self.K), np.uint16)
+        with torch.cuda.device(self.device):
+            check(lib.k2y_ap_tp_flags(self._h, out.ctypes.data, out.size, ctypes.byref(n), self._stream()))
+        return out
+
+    def reset(self) -> None:
+        with torch.cuda.device(self.device):
+            check(lib.k2y_ap_reset(self._h, self._stream()))
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            lib.k2y_ap_destroy(h)
+            self._h = None

@@ -49,7 +49,9 @@ def load_image(path):
     return data if gpu_decodable(data) else read_image(io.BytesIO(data))
 
 
-def serve(args, out_fh=None):
+def open_pipeline(args, max_per_class=30):
+    """(pipe, world, rank): this rank's DetectionPipeline for the model / anchor / batch / threshold flags, after joining the
+    process group when the job spans several GPUs (torch.distributed.run's environment)."""
     import torch.distributed as dist
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -58,35 +60,27 @@ def serve(args, out_fh=None):
     if world > 1 and not dist.is_initialized():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     anchors = np.load(args.anchors)
-    H, W = args.image_size
-    pipe = DetectionPipeline(args.model_def, (H, W), anchors, args.class_num, args.depth_multiplier, args.batch, args.obj_thresh,
-                             args.iou_thresh, 30, device=local, world=world, rank=rank)
+    pipe = DetectionPipeline(args.model_def, tuple(args.image_size), anchors, args.class_num, args.depth_multiplier, args.batch,
+                             args.obj_thresh, args.iou_thresh, max_per_class, device=local, world=world, rank=rank)
     pipe.engine.load_weights(args.ckpt)
-    files = list_images(args.images)
-    B, G = args.batch, world * args.batch
+    return pipe, world, rank
+
+
+def detect_files(pipe, files, decode_threads=4, load=None):
+    """Yields ``(paths, dets, counts)`` per global batch of world * batch files, in file order: the batch's gathered record
+    blocks as ``collect`` returns them (pinned host views, valid until the generator resumes twice).  Every rank reads ITS
+    files of the next batch in a pool of `decode_threads` threads while the GPU works, and two batches are in flight.
+    Every rank runs the network on a full batch (the tensor-core plans depend on the batch size, so the records of a short
+    final batch match a full one's bit for bit) and takes part in every all-gather: its share of a short batch is padded
+    with a grey network-size image, whose records nobody reads.  `load` maps a path to what submit_images takes
+    (default: load_image)."""
+    load = load or load_image
+    B, G, rank = pipe.batch, pipe.world * pipe.batch, pipe.rank
     chunks = [files[g0:g0 + G] for g0 in range(0, len(files), G)]
-    # every rank runs the network on a full batch (the tensor-core plans depend on the batch size, so the records of a short
-    # final batch match a full one's bit for bit) and takes part in every all-gather: its share of a short batch is padded
-    # with a grey network-size image, whose records nobody reads
-    filler = np.full((H, W, 3), 128, np.uint8)
-    n_out = 0
-
-    def write(chunk, ticket):
-        nonlocal n_out
-        dets, counts = pipe.collect(ticket)
-        if rank != 0:
-            return
-        recs = DetectionPipeline.records(dets, counts)
-        for j, path in enumerate(chunk):
-            line = {"image": path, "detections": [{"class": int(c), "score": round(float(s), 6), "box_tlbr": [float(t), float(l), float(b), float(r)],
-                                                   "index": int(i)} for c, i, s, t, l, b, r in recs[j]]}
-            if out_fh is not None:
-                out_fh.write(json.dumps(line) + "\n")
-            n_out += 1
-
-    with ThreadPoolExecutor(max(1, int(getattr(args, "decode_threads", 4)))) as pool:
+    filler = np.full(pipe.in_hw + (3,), 128, np.uint8)
+    with ThreadPoolExecutor(max(1, int(decode_threads))) as pool:
         def decode(chunk):      # this rank's images of a global batch, decoding in the pool
-            return [pool.submit(load_image, p) for p in chunk[rank * B:(rank + 1) * B]]
+            return [pool.submit(load, p) for p in chunk[rank * B:(rank + 1) * B]]
 
         pending = deque()
         nxt = decode(chunks[0]) if chunks else []
@@ -95,27 +89,50 @@ def serve(args, out_fh=None):
             nxt = decode(chunks[g + 1]) if g + 1 < len(chunks) else []
             pending.append((chunk, pipe.submit_images(imgs + [filler] * (B - len(imgs)))))
             if len(pending) == 2:
-                write(*pending.popleft())
+                chunk, ticket = pending.popleft()
+                yield (chunk,) + tuple(pipe.collect(ticket))
         while pending:
-            write(*pending.popleft())
+            chunk, ticket = pending.popleft()
+            yield (chunk,) + tuple(pipe.collect(ticket))
+
+
+def serve(args, out_fh=None):
+    import torch.distributed as dist
+    pipe, world, rank = open_pipeline(args)
+    n_out = 0
+    for chunk, dets, counts in detect_files(pipe, list_images(args.images), getattr(args, "decode_threads", 4), load_image):
+        if rank != 0:
+            continue
+        recs = DetectionPipeline.records(dets, counts)
+        for j, path in enumerate(chunk):
+            line = {"image": path, "detections": [{"class": int(c), "score": round(float(s), 6), "box_tlbr": [float(t), float(l), float(b), float(r)],
+                                                   "index": int(i)} for c, i, s, t, l, b, r in recs[j]]}
+            if out_fh is not None:
+                out_fh.write(json.dumps(line) + "\n")
+            n_out += 1
     if world > 1:
         dist.barrier()
     return n_out
 
 
-def main():
-    ap = argparse.ArgumentParser()
+def add_model_args(ap):
+    """The model, anchor, batch and decode-thread flags serve.py and evaluate_map.py share."""
     ap.add_argument("ckpt")
-    ap.add_argument("images", help="directory of images, or a text file with one path per line")
     ap.add_argument("--model_def", default="yolo_mobilev1", choices=["yolo_mobilev1", "yolo_mobilev2", "tiny_yolo", "yolo"])
     ap.add_argument("--depth_multiplier", type=float, default=0.75)
     ap.add_argument("--image_size", type=int, nargs=2, default=(224, 320))
     ap.add_argument("--class_num", type=int, default=20)
     ap.add_argument("--anchors", default="data/voc_anchor.npy")
     ap.add_argument("--batch", type=int, default=32, help="images per GPU per step")
+    ap.add_argument("--decode_threads", type=int, default=4, help="host threads reading the next batch's files and decoding those the GPU does not (PIL)")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    add_model_args(ap)
+    ap.add_argument("images", help="directory of images, or a text file with one path per line")
     ap.add_argument("--obj_thresh", type=float, default=0.7)
     ap.add_argument("--iou_thresh", type=float, default=0.5)
-    ap.add_argument("--decode_threads", type=int, default=4, help="host threads reading the next batch's files and decoding those the GPU does not (PIL)")
     ap.add_argument("--out", default="-")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
