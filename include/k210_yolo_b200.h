@@ -301,6 +301,39 @@ int k2y_jpeg_decode(const void *blob_host, const void *blob_dev, const unsigned 
                     void *workspace_dev, size_t workspace_bytes, int32_t *status_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Baseline JPEG encoding, byte-identical to PIL's Image.fromarray(rgb).save(f, "JPEG", quality=q) with libjpeg-turbo 3.1:
+ * JFIF APP0, two DQT, SOF0 4:2:0, the four standard Huffman tables, one interleaved scan, EOI.
+ *   k2y_jpeg_encode_plan             host only: the descriptor blob of n images, hw_host int32 [n][2] (1..65535 each),
+ *                                    src_offsets_host: where image i's h*w*3 RGB bytes lie in the device source buffer.
+ *                                    blob == NULL: only *blob_bytes (size query); else a 16-byte aligned host buffer.
+ *                                    quality 1..100; anything else is K2Y_ERR_INVALID.
+ *   k2y_jpeg_encode_workspace_bytes  device workspace, and the output capacity (bytes the batch's files take at most).
+ *   k2y_jpeg_encode                  asynchronous on `stream`, seven launches whatever the image count: blob_host is read
+ *                                    before the call returns, blob_dev is the same bytes on the device (16-byte aligned).
+ *                                    The files are written back to back from dst_dev; lengths_dev (int64 [n]) their sizes.
+ * ---------------------------------------------------------------------------------------- */
+int k2y_jpeg_encode_plan(int n, const int *hw_host, const long long *src_offsets_host, int quality, void *blob,
+                         size_t blob_capacity, size_t *blob_bytes);
+/* Host only: the bytes a file of that size and quality starts with, SOI up to and including SOS (out == NULL: size query). */
+int k2y_jpeg_encode_header(int h, int w, int quality, unsigned char *out, size_t capacity, size_t *length);
+int k2y_jpeg_encode_workspace_bytes(const void *blob_host, size_t *workspace_bytes, size_t *output_capacity);
+int k2y_jpeg_encode(const void *blob_host, const void *blob_dev, const unsigned char *src_dev, unsigned char *dst_dev,
+                    long long *lengths_dev, void *workspace_dev, size_t workspace_bytes, void *stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Detection rendering in place, pixel for pixel draw.draw_detections (see csrc/render.cu for the one deliberate difference:
+ * a box whose outline rings cross stops at the first crossing ring instead of raising).  images_dev: packed HWC RGB, image i
+ * at offsets_host[i] with size hw_host[i] (1..65535 each).  atlas_dev[i]: the device label atlas of image i's font
+ * (render.LabelAtlas: int32 header [8] with [0] = classes, int32 entries [classes][101][8], then the glyph masks).  dets_dev /
+ * counts_dev: k2y_det records [n][class_num][max_per_class] and counts [n][class_num] with the given per-image strides.
+ * colors_dev: uint8 [class_num][3], class_num 1..80.  Asynchronous on `stream`, one launch per 128 images.
+ * ---------------------------------------------------------------------------------------- */
+int k2y_render_detections(unsigned char *images_dev, int n, const long long *offsets_host, const int *hw_host,
+                          const int32_t *const *atlas_dev, const int32_t *dets_dev, const int32_t *counts_dev,
+                          long long det_image_stride_words, long long count_image_stride_words, int class_num,
+                          int max_per_class, const unsigned char *colors_dev, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Evaluation: the counters behind the reference's Yolo_Precision / Yolo_Recall metrics (tools/custom.py:13-75) on device
  * tensors.  y_true_dev / y_pred_dev: n_boxes records of entry_floats = 5 + classes floats (any [..., A, 5+C] head or label
  * tensor, flattened); element 4 is the confidence.  counts_dev[3] (uint64, caller-zeroed, accumulated into): tp, fp, fn with

@@ -22,15 +22,26 @@ def box_geometry(image_shape: Sequence[int], box: Sequence[float], label_size: S
     return top, left, bottom, right, origin
 
 
+def label_font(image_h: int, font_path: str = "asset/FiraMono-Medium.otf"):
+    """The label font keras_inference.py picks for an image `image_h` rows high: the TrueType file at ``floor(0.03 h + 0.5)``
+    points, or PIL's default font when the file cannot be opened."""
+    from PIL import ImageFont
+    try:
+        return ImageFont.truetype(font=font_path, size=label_font_size(image_h))
+    except OSError:
+        return ImageFont.load_default()
+
+
+def label_font_size(image_h: int) -> int:
+    return int(np.floor(3e-2 * image_h + 0.5))
+
+
 def draw_detections(orig_img: np.ndarray, found: List[Tuple], colormap, font_path: str = "asset/FiraMono-Medium.otf"):
     """found: (class, flat_index, score, top, left, bottom, right) tuples.  Returns the annotated PIL image."""
-    from PIL import Image, ImageDraw, ImageFont
+    from PIL import Image, ImageDraw
     image_shape = orig_img.shape[0:2]
     pil_img = Image.fromarray(orig_img)
-    try:
-        font = ImageFont.truetype(font=font_path, size=int(np.floor(3e-2 * image_shape[0] + 0.5)))
-    except OSError:
-        font = ImageFont.load_default()
+    font = label_font(image_shape[0], font_path)
     thickness = (image_shape[0] + image_shape[1]) // 300
     for c, _idx, score, top, left, bottom, right in found:
         label = "{:2d} {:.2f}".format(int(c), score)

@@ -19,6 +19,11 @@ caller's stream wait for the decode before returning — plain stream semantics;
 device ``image_hw`` [batch, 2]; the packed H2D copy and the batched letterbox (which also writes ``image_hw``) run on the copy
 stream into the slot's uint8 input buffer, overlapping the previous batch's network, and the decode of that batch reads the
 slot's ``image_hw``, so two batches in flight each carry their own original sizes.
+
+``enable_rendering`` adds the drawn result to ``submit_images``: behind the NMS, on the decode stream, the batch's local records
+are drawn onto its original images where they lie in the slot's device staging buffer and encoded as JPEG files;
+``rendered(ticket)`` brings them back after ``collect`` with one exact-size copy.  The next ``submit_images`` into that input
+slot waits for the render before it overwrites the originals.
 """
 from __future__ import annotations
 
@@ -77,6 +82,11 @@ class DetectionPipeline:
         self._jpeg_status = [torch.zeros((batch, 4), dtype=torch.int32).pin_memory() for _ in range(SLOTS)]
         self._steps = 0
         self._submitted = 0
+        # enable_rendering: label atlas, colour table, quality, one encoder per gather slot (its files live until rendered())
+        self._render = None
+        self._render_done = [torch.cuda.Event() for _ in range(SLOTS)]   # files of gather slot ready to copy back
+        self._render_free = [torch.cuda.Event() for _ in range(SLOTS)]   # render + encode finished with input slot's originals
+        self._rendered_slot: List[bool] = [False] * SLOTS
 
     def set_image_shapes(self, image_hw) -> None:
         """Original (pre-letterbox) image sizes, [batch, 2] (h, w); defaults to the network input size."""
@@ -160,7 +170,51 @@ class DetectionPipeline:
             buf[:n].copy_(x_host, non_blocking=True)
             self._h2d_done[slot].record(self._copy_stream)
         self._jpeg_idx[self._steps % SLOTS] = []
-        return self._run_slot(slot, buf, n, None, None)
+        t = self._run_slot(slot, buf, n, None, None)
+        self._rendered_slot[t] = False
+        return t
+
+    def enable_rendering(self, quality: int = 75, font_path: str = "asset/FiraMono-Medium.otf", colormap=None) -> None:
+        """From now on every ``submit_images`` batch also has its local records drawn onto its original images (as
+        ``draw.draw_detections`` draws them, ``render.render_detections_device``) and encoded as JPEG files (as PIL saves them at
+        `quality`, ``render.JpegEncoder``), on the decode stream behind the NMS; ``rendered(ticket)`` returns them after
+        ``collect``.  `colormap`: RGB triples per class (default ``Helper.colormap``, 80 classes).  Records and ``collect``
+        are unchanged."""
+        from .helper import _COLORMAP
+        from .render import JpegEncoder, LabelAtlas, color_table
+        colormap = _COLORMAP if colormap is None else colormap
+        C = self.gather.C
+        if C > len(colormap):
+            raise ValueError(f"class_num {C} exceeds the colormap's {len(colormap)} classes")
+        if not 1 <= int(quality) <= 100:
+            raise ValueError(f"quality {quality} is outside 1..100")
+        dev = torch.device("cuda", self.device_index)
+        self._render = dict(quality=int(quality), atlas=LabelAtlas(C, font_path), colors=color_table(colormap, C, dev),
+                            encoders=[JpegEncoder(dev) for _ in range(SLOTS)])
+
+    def rendered(self, ticket: int) -> List[bytes]:
+        """The JPEG files of this rank's images of the ``submit_images`` batch behind `ticket`, with its records drawn on them;
+        valid after ``collect(ticket)`` until the ticket's slot is reused."""
+        if self._render is None or not self._rendered_slot[ticket]:
+            raise RuntimeError("no rendered files for this ticket: call enable_rendering() before submit_images()")
+        self._render_done[ticket].synchronize()
+        return self._render["encoders"][ticket].fetch()
+
+    def _render_slot(self, slot: int, s: int, layout: BatchLayout) -> None:
+        """Draws gather slot s's local records onto input slot `slot`'s originals and encodes them, on the decode stream."""
+        from .render import render_packed
+        r = self._render
+        det = self._det_stream
+        det.wait_event(self._h2d_done[slot])     # the originals are in place (already implied by the network's wait)
+        staging = self._staging[slot]
+        dets, counts = self.gather.local(s)
+        n = len(layout)
+        with torch.cuda.stream(det):
+            render_packed(staging.dev.data_ptr(), layout.offsets, layout.hw, dets[:n], counts[:n], r["atlas"], r["colors"],
+                          staging.dev.device, det)
+            r["encoders"][s].enqueue(staging.dev.data_ptr(), layout.offsets, layout.hw, r["quality"], det)
+        self._render_done[s].record(det)
+        self._render_free[slot].record(det)
 
     def submit_images(self, images: Sequence[np.ndarray]) -> int:
         """Streaming form for raw images: `images` is a list of n <= batch host numpy uint8 [h, w, 3] RGB arrays of any sizes, or
@@ -187,6 +241,7 @@ class DetectionPipeline:
         self._submitted += 1
         self._copy_stream.wait_event(self._in_free[slot])
         self._copy_stream.wait_event(self._hw_free[slot])
+        self._copy_stream.wait_event(self._render_free[slot])    # the last render read this slot's originals
         s = self._steps % SLOTS                  # the gather slot this batch's step will use
         with torch.cuda.device(dev):
             letterbox_packed(layout, images, self._staging[slot], buf, self._slot_hw[slot])
@@ -195,7 +250,12 @@ class DetectionPipeline:
                 with torch.cuda.stream(self._copy_stream):
                     self._jpeg_status[s][:len(layout.jpeg)].copy_(self._staging[slot].status[:len(layout.jpeg)], non_blocking=True)
         self._h2d_done[slot].record(self._copy_stream)
-        return self._run_slot(slot, buf, n, self._slot_hw[slot][:n], n if self.world == 1 else None)
+        t = self._run_slot(slot, buf, n, self._slot_hw[slot][:n], n if self.world == 1 else None)
+        self._rendered_slot[t] = self._render is not None
+        if self._render is not None:
+            with torch.cuda.device(dev):
+                self._render_slot(slot, t, layout)
+        return t
 
     def _run_slot(self, slot: int, buf: torch.Tensor, n: int, image_hw: Optional[torch.Tensor], rows: Optional[int]) -> int:
         """Network + decode (+ all-gather) of input slot `slot` once its H2D is done, then the D2H of the records."""
@@ -219,6 +279,8 @@ class DetectionPipeline:
         until the ticket's slot is reused two submits later).  Raises ``K2YError`` when a JPEG of a ``submit_images`` batch had
         corrupt entropy-coded data."""
         self._d2h_done[ticket].synchronize()      # behind the network, which waited for the batch's decode and status copy
+        if self._rendered_slot[ticket]:
+            self._render_done[ticket].synchronize()   # the files' lengths are on the host
         if self._jpeg_idx[ticket]:
             idx = self._jpeg_idx[ticket]
             check_jpeg_status(self._jpeg_status[ticket][:len(idx)].numpy(), idx)
@@ -332,6 +394,15 @@ class LanedPipeline:
     def collect(self, ticket):
         k, t = ticket
         return self.lanes[k].collect(t)
+
+    def enable_rendering(self, quality: int = 75, font_path: str = "asset/FiraMono-Medium.otf", colormap=None) -> None:
+        """``DetectionPipeline.enable_rendering`` on every lane."""
+        for ln in self.lanes:
+            ln.enable_rendering(quality, font_path, colormap)
+
+    def rendered(self, ticket) -> List[bytes]:
+        k, t = ticket
+        return self.lanes[k].rendered(t)
 
     def in_flight_limit(self) -> int:
         """Batches that may be submitted before the oldest must be collected."""

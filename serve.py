@@ -6,6 +6,7 @@ gathered detections, one JSON line per image.  The GPU analogue of the firmware'
     python serve.py CKPT IMAGE_DIR [--model_def yolo_mobilev1 --depth_multiplier 0.75 --image_size 224 320 --class_num 20
                                     --anchors data/voc_anchor.npy --batch 32 --obj_thresh 0.7 --iou_thresh 0.5 --out dets.jsonl]
     python -m torch.distributed.run --nproc-per-node 8 serve.py ...        # one rank per GPU, NCCL all-gather of the records
+    python serve.py CKPT IMAGE_DIR --draw OUT_DIR [--draw_quality 75]       # also OUT_DIR/<stem>.jpg with the detections drawn
 
 Per global batch of world*batch images: every rank reads ITS files in a pool of --decode_threads threads, one batch ahead.
 Baseline JPEGs the GPU decoder takes (preprocess.gpu_decodable) stay compressed; every other file is decoded there by PIL as
@@ -13,6 +14,10 @@ Helper._read_img does.  DetectionPipeline.submit_images takes both (one packed H
 batched letterbox launch into its uint8 input buffer, network + decode + NMS), and ONE all-gather completes the record blocks
 on every rank; two batches are in flight, and rank 0 writes the lines in file order.  The GPU decode gives the bytes PIL
 gives, so the lines do not depend on which route a file took.
+
+With --draw DIR every rank also writes DIR/<stem>.jpg for its own files: the records are drawn onto the original images where
+they already lie on the GPU and encoded there (DetectionPipeline.enable_rendering), with the bytes PIL's draw_detections + save
+give; only the compressed files come back.  Duplicate stems are refused before any work starts.
 """
 import argparse
 import io
@@ -66,14 +71,27 @@ def open_pipeline(args, max_per_class=30):
     return pipe, world, rank
 
 
-def detect_files(pipe, files, decode_threads=4, load=None):
+def draw_paths(files, out_dir):
+    """``out_dir/<stem>.jpg`` for every input file; raises ValueError when two files share a stem (their drawn results would
+    overwrite each other)."""
+    seen = {}
+    for p in files:
+        stem = os.path.splitext(os.path.basename(p))[0]
+        if stem in seen:
+            raise ValueError(f"--draw: {seen[stem]} and {p} would both be written to {stem}.jpg")
+        seen[stem] = p
+    return [os.path.join(out_dir, os.path.splitext(os.path.basename(p))[0] + ".jpg") for p in files]
+
+
+def detect_files(pipe, files, decode_threads=4, load=None, rendered=False):
     """Yields ``(paths, dets, counts)`` per global batch of world * batch files, in file order: the batch's gathered record
     blocks as ``collect`` returns them (pinned host views, valid until the generator resumes twice).  Every rank reads ITS
     files of the next batch in a pool of `decode_threads` threads while the GPU works, and two batches are in flight.
     Every rank runs the network on a full batch (the tensor-core plans depend on the batch size, so the records of a short
     final batch match a full one's bit for bit) and takes part in every all-gather: its share of a short batch is padded
     with a grey network-size image, whose records nobody reads.  `load` maps a path to what submit_images takes
-    (default: load_image)."""
+    (default: load_image).  With `rendered` (the pipeline's rendering enabled) each tuple also carries this rank's drawn
+    JPEG files of the batch, its padding images' files left out."""
     load = load or load_image
     B, G, rank = pipe.batch, pipe.world * pipe.batch, pipe.rank
     chunks = [files[g0:g0 + G] for g0 in range(0, len(files), G)]
@@ -82,25 +100,40 @@ def detect_files(pipe, files, decode_threads=4, load=None):
         def decode(chunk):      # this rank's images of a global batch, decoding in the pool
             return [pool.submit(load, p) for p in chunk[rank * B:(rank + 1) * B]]
 
+        def result(chunk, ticket, mine):
+            out = (chunk,) + tuple(pipe.collect(ticket))
+            return out + (pipe.rendered(ticket)[:mine],) if rendered else out
+
         pending = deque()
         nxt = decode(chunks[0]) if chunks else []
         for g, chunk in enumerate(chunks):
             imgs = [f.result() for f in nxt]
             nxt = decode(chunks[g + 1]) if g + 1 < len(chunks) else []
-            pending.append((chunk, pipe.submit_images(imgs + [filler] * (B - len(imgs)))))
+            pending.append((chunk, pipe.submit_images(imgs + [filler] * (B - len(imgs))), len(imgs)))
             if len(pending) == 2:
-                chunk, ticket = pending.popleft()
-                yield (chunk,) + tuple(pipe.collect(ticket))
+                yield result(*pending.popleft())
         while pending:
-            chunk, ticket = pending.popleft()
-            yield (chunk,) + tuple(pipe.collect(ticket))
+            yield result(*pending.popleft())
 
 
 def serve(args, out_fh=None):
     import torch.distributed as dist
+    files = list_images(args.images)
+    draw_dir = getattr(args, "draw", None)
+    targets = draw_paths(files, draw_dir) if draw_dir else None     # refuses duplicate stems before any work
     pipe, world, rank = open_pipeline(args)
+    if draw_dir:
+        os.makedirs(draw_dir, exist_ok=True)
+        pipe.enable_rendering(quality=args.draw_quality)
     n_out = 0
-    for chunk, dets, counts in detect_files(pipe, list_images(args.images), getattr(args, "decode_threads", 4), load_image):
+    B = pipe.batch
+    for g, item in enumerate(detect_files(pipe, files, getattr(args, "decode_threads", 4), load_image, rendered=bool(draw_dir))):
+        chunk, dets, counts = item[:3]
+        if draw_dir:        # this rank's files of the global batch
+            first = g * world * B + rank * B
+            for path, data in zip(targets[first:first + len(item[3])], item[3]):
+                with open(path, "wb") as fh:
+                    fh.write(data)
         if rank != 0:
             continue
         recs = DetectionPipeline.records(dets, counts)
@@ -127,14 +160,29 @@ def add_model_args(ap):
     ap.add_argument("--decode_threads", type=int, default=4, help="host threads reading the next batch's files and decoding those the GPU does not (PIL)")
 
 
-def main():
+def quality_arg(v):
+    q = int(v)
+    if not 1 <= q <= 100:
+        raise argparse.ArgumentTypeError(f"JPEG quality {v} is outside 1..100")
+    return q
+
+
+def build_parser():
     ap = argparse.ArgumentParser()
     add_model_args(ap)
     ap.add_argument("images", help="directory of images, or a text file with one path per line")
     ap.add_argument("--obj_thresh", type=float, default=0.7)
     ap.add_argument("--iou_thresh", type=float, default=0.5)
     ap.add_argument("--out", default="-")
-    args = ap.parse_args()
+    ap.add_argument("--draw", default=None, metavar="DIR",
+                    help="also write every image with its detections drawn (as keras_inference.py draws them) to DIR/<stem>.jpg, "
+                         "rendered and JPEG-encoded on the GPU")
+    ap.add_argument("--draw_quality", type=quality_arg, default=75, help="JPEG quality of the --draw files (1..100)")
+    return ap
+
+
+def main():
+    args = build_parser().parse_args()
     rank = int(os.environ.get("RANK", "0"))
     fh = (sys.stdout if args.out == "-" else open(args.out, "w")) if rank == 0 else None
     n = serve(args, fh)
