@@ -1,6 +1,6 @@
-// Baseline JPEG decoding on the GPU, bit-exact with libjpeg-turbo as PIL runs it (the reference reads every image with
-// skimage.io.imread, tools/utils.py:339-355, i.e. PIL / libjpeg-turbo underneath): JDCT_ISLOW integer IDCT, fancy
-// upsampling, ycc_rgb_convert.  The pixels land in the packed uint8 HWC buffer k2y_letterbox_u8_batch reads.
+// Baseline JPEG decoding on the GPU, bit-exact with libjpeg-turbo as PIL runs it on x86-64 (the reference reads every image
+// with skimage.io.imread, tools/utils.py:339-355, i.e. PIL / libjpeg-turbo underneath): the x86 SIMD JDCT_ISLOW integer IDCT,
+// fancy upsampling, ycc_rgb_convert.  The pixels land in the packed uint8 HWC buffer k2y_letterbox_u8_batch reads.
 //
 // Host side: a marker walker classifies each file (GPU-decodable, valid but not for the GPU, malformed) and builds one
 // descriptor blob per batch (JpegBlobHeader, JpegImg[n], JpegSeg[segments], JpegHuff[2 * components per image]).  The caller
@@ -14,7 +14,8 @@
 //                            scan of completed blocks gives each thread its first block, and a last pass writes int16
 //                            coefficients in natural order (DC as differences)
 //   3. jpeg_dc_kernel        (CTA per segment) per-component scan of the DC differences in decode order
-//   4. jpeg_idct_kernel      dequantise + jidctint.c jpeg_idct_islow -> uint8 component planes at the MCU-padded size
+//   4. jpeg_idct_kernel      dequantise + libjpeg-turbo's x86 SIMD islow (jidctint-avx2.asm / -sse2.asm, 16-bit lanes)
+//                            -> uint8 component planes at the MCU-padded size
 //   5. jpeg_color_kernel     libjpeg-turbo's upsampler dispatch (fancy on) + ycc_rgb_convert, cropped, HWC RGB out
 #include "common.h"
 
@@ -281,6 +282,11 @@ int parse_jpeg(const uint8_t *d, size_t n, Parsed &p, const char *who) {
                     if (p.id[c] == cid) f = c;
                 if (f < 0) {
                     set_error("%s: SOS marker at offset %zu names component id %d the frame does not have", who, at, cid);
+                    return K2Y_ERR_INVALID;
+                }
+                // T.81 B.2.3: a scan lists its components in frame order; libjpeg-turbo refuses the file otherwise
+                if (k > 0 && f <= p.scan_comp[k - 1]) {
+                    set_error("%s: SOS marker at offset %zu lists component id %d out of frame order", who, at, cid);
                     return K2Y_ERR_INVALID;
                 }
                 p.scan_comp[k] = f;
@@ -789,7 +795,13 @@ __global__ void __launch_bounds__(DC_THREADS) jpeg_dc_kernel(const uint8_t *__re
     }
 }
 
-// jidctint.c jpeg_idct_islow (13-bit constants, 2 pass bits) with its range-limit table indexed with & RANGE_MASK.
+// libjpeg-turbo's x86 SIMD islow (jidctint-avx2.asm, jidctint-sse2.asm), the IDCT PIL runs on x86-64.  Same 13-bit
+// constants and 2 pass bits as jidctint.c, but on 16-bit lanes: the dequantised product keeps its low 16 bits (pmullw); the
+// sums feeding a multiply (in0 +- in4, in7 + in3, in5 + in1) wrap to 16 bits (paddw); products and the other sums are 32-bit
+// (pmaddwd; they stay below 2^31 for 16-bit inputs); pass 1 saturates its results to int16 (packssdw), pass 2 to int16 and
+// then int8 before adding 128 (packssdw, packsswb).  When rows 1-7 of the whole block are zero, pass 1 is row 0 shifted left
+// by 2 in 16 bits (psllw, wrapping).  On the coefficients an 8-bit encoder writes this equals jidctint.c; outside them it
+// does not, and jidctint.c's masked range-limit table gives other pixels.
 #define FIX_0_298631336 2446
 #define FIX_0_390180644 3196
 #define FIX_0_541196100 4433
@@ -803,59 +815,34 @@ __global__ void __launch_bounds__(DC_THREADS) jpeg_dc_kernel(const uint8_t *__re
 #define FIX_2_562915447 20995
 #define FIX_3_072711026 25172
 
-__device__ __forceinline__ int idct_limit(int x) {   // range_limit[x & RANGE_MASK] of the post-IDCT table, RANGE_MASK 1023
-    int v = x & 1023;
-    if (v >= 512) v -= 1024;
-    return min(max(v + 128, 0), 255);
-}
+__device__ __forceinline__ int wrap16(int x) { return (int)(int16_t)x; }
 
+// One 1-D pass on int16 inputs: pass 1 -> int16 (saturated), pass 2 -> the sample value (saturated to [-128, 127], + 128).
 template <int PASS>
 __device__ __forceinline__ void idct_1d(int i0, int i1, int i2, int i3, int i4, int i5, int i6, int i7, int *o) {
-    int z1, z2, z3, z4, z5, tmp0, tmp1, tmp2, tmp3, tmp10, tmp11, tmp12, tmp13;
-    z2 = i2;
-    z3 = i6;
-    z1 = (z2 + z3) * FIX_0_541196100;
-    tmp2 = z1 + z3 * (-FIX_1_847759065);
-    tmp3 = z1 + z2 * FIX_0_765366865;
-    tmp0 = (i0 + i4) * (1 << 13);
-    tmp1 = (i0 - i4) * (1 << 13);
-    tmp10 = tmp0 + tmp3;
-    tmp13 = tmp0 - tmp3;
-    tmp11 = tmp1 + tmp2;
-    tmp12 = tmp1 - tmp2;
-    tmp0 = i7;
-    tmp1 = i5;
-    tmp2 = i3;
-    tmp3 = i1;
-    z1 = tmp0 + tmp3;
-    z2 = tmp1 + tmp2;
-    z3 = tmp0 + tmp2;
-    z4 = tmp1 + tmp3;
-    z5 = (z3 + z4) * FIX_1_175875602;
-    tmp0 = tmp0 * FIX_0_298631336;
-    tmp1 = tmp1 * FIX_2_053119869;
-    tmp2 = tmp2 * FIX_3_072711026;
-    tmp3 = tmp3 * FIX_1_501321110;
-    z1 = z1 * (-FIX_0_899976223);
-    z2 = z2 * (-FIX_2_562915447);
-    z3 = z3 * (-FIX_1_961570560);
-    z4 = z4 * (-FIX_0_390180644);
-    z3 += z5;
-    z4 += z5;
-    tmp0 += z1 + z3;
-    tmp1 += z2 + z4;
-    tmp2 += z2 + z3;
-    tmp3 += z1 + z4;
+    const int tmp3 = i2 * (FIX_0_541196100 + FIX_0_765366865) + i6 * FIX_0_541196100;
+    const int tmp2 = i2 * FIX_0_541196100 + i6 * (FIX_0_541196100 - FIX_1_847759065);
+    const int tmp0 = wrap16(i0 + i4) * (1 << 13);
+    const int tmp1 = wrap16(i0 - i4) * (1 << 13);
+    const int tmp10 = tmp0 + tmp3, tmp13 = tmp0 - tmp3, tmp11 = tmp1 + tmp2, tmp12 = tmp1 - tmp2;
+    const int z3 = wrap16(i7 + i3), z4 = wrap16(i5 + i1);
+    const int z3p = z3 * (FIX_1_175875602 - FIX_1_961570560) + z4 * FIX_1_175875602;
+    const int z4p = z3 * FIX_1_175875602 + z4 * (FIX_1_175875602 - FIX_0_390180644);
+    const int o0 = i7 * (FIX_0_298631336 - FIX_0_899976223) - i1 * FIX_0_899976223 + z3p;
+    const int o3 = -i7 * FIX_0_899976223 + i1 * (FIX_1_501321110 - FIX_0_899976223) + z4p;
+    const int o1 = i5 * (FIX_2_053119869 - FIX_2_562915447) - i3 * FIX_2_562915447 + z4p;
+    const int o2 = -i5 * FIX_2_562915447 + i3 * (FIX_3_072711026 - FIX_2_562915447) + z3p;
     constexpr int sh = PASS == 1 ? 13 - 2 : 13 + 2 + 3;
     constexpr int rnd = 1 << (sh - 1);
-    o[0] = (tmp10 + tmp3 + rnd) >> sh;
-    o[7] = (tmp10 - tmp3 + rnd) >> sh;
-    o[1] = (tmp11 + tmp2 + rnd) >> sh;
-    o[6] = (tmp11 - tmp2 + rnd) >> sh;
-    o[2] = (tmp12 + tmp1 + rnd) >> sh;
-    o[5] = (tmp12 - tmp1 + rnd) >> sh;
-    o[3] = (tmp13 + tmp0 + rnd) >> sh;
-    o[4] = (tmp13 - tmp0 + rnd) >> sh;
+    constexpr int lo = PASS == 1 ? -32768 : -128, hi = PASS == 1 ? 32767 : 127, add = PASS == 1 ? 0 : 128;
+    o[0] = min(max((tmp10 + o3 + rnd) >> sh, lo), hi) + add;
+    o[7] = min(max((tmp10 - o3 + rnd) >> sh, lo), hi) + add;
+    o[1] = min(max((tmp11 + o2 + rnd) >> sh, lo), hi) + add;
+    o[6] = min(max((tmp11 - o2 + rnd) >> sh, lo), hi) + add;
+    o[2] = min(max((tmp12 + o1 + rnd) >> sh, lo), hi) + add;
+    o[5] = min(max((tmp12 - o1 + rnd) >> sh, lo), hi) + add;
+    o[3] = min(max((tmp13 + o0 + rnd) >> sh, lo), hi) + add;
+    o[4] = min(max((tmp13 - o0 + rnd) >> sh, lo), hi) + add;
 }
 
 // One thread per 8x8 block; grid (block tiles, image).
@@ -872,23 +859,34 @@ __global__ void __launch_bounds__(IDCT_THREADS) jpeg_idct_kernel(const uint8_t *
     const int bx = local % im.bw[comp], by = local / im.bw[comp];
     const int4 *cp = reinterpret_cast<const int4 *>(ws + H.ws_coef + im.coef_offset) + (long long)b * 8;
     int ws_[64];
+    int ac_rows = 0;   // any coefficient of rows 1-7
 #pragma unroll
     for (int r = 0; r < 8; ++r) {
         const int4 q = cp[r];
         const int v[4] = {q.x, q.y, q.z, q.w};
+        if (r > 0) ac_rows |= q.x | q.y | q.z | q.w;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            ws_[r * 8 + 2 * j] = (int)(int16_t)(v[j] & 0xffff) * s_q[comp][r * 8 + 2 * j];
-            ws_[r * 8 + 2 * j + 1] = (int)(int16_t)((unsigned)v[j] >> 16) * s_q[comp][r * 8 + 2 * j + 1];
+        for (int j = 0; j < 4; ++j) {   // the low 16 bits of the product
+            ws_[r * 8 + 2 * j] = wrap16((int)(int16_t)(v[j] & 0xffff) * s_q[comp][r * 8 + 2 * j]);
+            ws_[r * 8 + 2 * j + 1] = wrap16((int)(int16_t)((unsigned)v[j] >> 16) * s_q[comp][r * 8 + 2 * j + 1]);
         }
     }
     // pass 1: columns
+    if (ac_rows == 0) {
 #pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        int o[8];
-        idct_1d<1>(ws_[c], ws_[8 + c], ws_[16 + c], ws_[24 + c], ws_[32 + c], ws_[40 + c], ws_[48 + c], ws_[56 + c], o);
+        for (int c = 0; c < 8; ++c) {
+            const int dc = wrap16(ws_[c] * 4);
 #pragma unroll
-        for (int r = 0; r < 8; ++r) ws_[r * 8 + c] = o[r];
+            for (int r = 0; r < 8; ++r) ws_[r * 8 + c] = dc;
+        }
+    } else {
+#pragma unroll
+        for (int c = 0; c < 8; ++c) {
+            int o[8];
+            idct_1d<1>(ws_[c], ws_[8 + c], ws_[16 + c], ws_[24 + c], ws_[32 + c], ws_[40 + c], ws_[48 + c], ws_[56 + c], o);
+#pragma unroll
+            for (int r = 0; r < 8; ++r) ws_[r * 8 + c] = o[r];
+        }
     }
     const int stride = im.bw[comp] * 8;
     uint8_t *out = ws + H.ws_plane + im.plane_offset + im.plane_byte[comp] + (long long)by * 8 * stride + bx * 8;
@@ -899,8 +897,8 @@ __global__ void __launch_bounds__(IDCT_THREADS) jpeg_idct_kernel(const uint8_t *
         idct_1d<2>(ws_[r * 8], ws_[r * 8 + 1], ws_[r * 8 + 2], ws_[r * 8 + 3], ws_[r * 8 + 4], ws_[r * 8 + 5], ws_[r * 8 + 6],
                    ws_[r * 8 + 7], o);
         uint2 pk;
-        pk.x = idct_limit(o[0]) | (idct_limit(o[1]) << 8) | (idct_limit(o[2]) << 16) | ((unsigned)idct_limit(o[3]) << 24);
-        pk.y = idct_limit(o[4]) | (idct_limit(o[5]) << 8) | (idct_limit(o[6]) << 16) | ((unsigned)idct_limit(o[7]) << 24);
+        pk.x = o[0] | (o[1] << 8) | (o[2] << 16) | ((unsigned)o[3] << 24);
+        pk.y = o[4] | (o[5] << 8) | (o[6] << 16) | ((unsigned)o[7] << 24);
         *reinterpret_cast<uint2 *>(out + (long long)r * stride) = pk;
     }
 }
