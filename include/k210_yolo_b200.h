@@ -377,6 +377,43 @@ int k2y_ap_result(k2y_ap *ap, double *ap_host, double *ap07_host, long long *npo
 int k2y_ap_reset(k2y_ap *ap, void *stream);
 int k2y_ap_tp_flags(k2y_ap *ap, uint16_t *tp_host, long long capacity, long long *n_images, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * COCO detection evaluation on the device: what pycocotools' COCOeval(gt, dt, "bbox") computes with its default parameters
+ * (IoU thresholds 0.50:0.05:0.95, 101 recall points, maxDets 1 / 10 / 100, area ranges all / small / medium / large with
+ * bounds 0, 32^2, 96^2, 1e10).  The protocol is written down in oracle/coco_ref.py.  The ground truth is uploaded once;
+ * the evaluator holds one slot per (image, class, k < min(max_per_class, 100)) with the record's score bits and, per
+ * (area range, threshold), a TP bit and a not-ignored bit.
+ *   k2y_coco_create   gt_host [n_gt][7] float64 (class index, x, y, w, h, area, iscrowd): image i's annotations, in file
+ *                     order, at rows [gt_offsets_host[i], gt_offsets_host[i+1]), images in sorted image-id order and class
+ *                     index c the c-th smallest category id.  n_images counts every image, with annotations or not.
+ *                     class_num 1..1024, max_per_class >= 1.  iou_thresholds [10] / recall_thresholds [101]: COCOeval's
+ *                     np.linspace values, increasing.
+ *   k2y_coco_match    one update of n_images, asynchronous on `stream` (one kernel): dets_dev / counts_dev as k2y_ap_match
+ *                     reads them, image_positions_dev (int64, device) each image's position in the sorted image-id list.
+ *                     Records of an (image, class) are in score-descending order (the order the detection kernels emit);
+ *                     the first min(count, 100) are evaluated.  Updates may arrive in any image order.
+ *   k2y_coco_result   ranks every stored record by (class, score descending, image position, record order) and reduces the
+ *                     curves; synchronous.  precision_host [10][101][C][4][3], recall_host [10][C][4][3] float64, COCOeval's
+ *                     eval["precision"] / eval["recall"] (-1 where a class has no non-ignored ground truth in an area range;
+ *                     images never matched count as images without detections).  status_host: K2Y_COCO_* bits of anything
+ *                     invalid seen since the last reset (the results are then meaningless).
+ *   k2y_coco_reset    forgets every update.
+ * Every call of one evaluator is ordered after the previous one, whatever streams they use.
+ * ---------------------------------------------------------------------------------------- */
+#define K2Y_COCO_BAD_SCORE 1        /* a record within its count has a NaN score or one with the sign bit set */
+#define K2Y_COCO_BAD_COUNT 2        /* a count outside [0, max_per_class] (clamped) */
+#define K2Y_COCO_BAD_POSITION 4     /* an image position outside [0, n_images) (the image was skipped) */
+#define K2Y_COCO_REPEATED_IMAGE 8   /* an image position given twice since the last reset */
+typedef struct k2y_coco k2y_coco;
+int k2y_coco_create(const double *gt_host, const long long *gt_offsets_host, long long n_images, int class_num,
+                    int max_per_class, const double *iou_thresholds, const double *recall_thresholds, int device,
+                    k2y_coco **out);
+int k2y_coco_destroy(k2y_coco *coco);
+int k2y_coco_match(k2y_coco *coco, const int32_t *dets_dev, const int32_t *counts_dev, long long det_image_stride_words,
+                   long long count_image_stride_words, int n_images, const long long *image_positions_dev, void *stream);
+int k2y_coco_result(k2y_coco *coco, double *precision_host, double *recall_host, unsigned *status_host, void *stream);
+int k2y_coco_reset(k2y_coco *coco, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,11 +7,17 @@
 VOC 2007 11-point AP, any set of IoU thresholds), matched, ranked and reduced by the k2y_ap_* kernels.  The protocol is
 that of oracle/ap_ref.py: IoU without a "+1 pixel" term, and every object counts (the annotation lists carry no
 "difficult" flag).  ``load_voc_annotations`` reads the lists make_voc_list.py writes.
+
+``CocoEval``: what pycocotools' ``COCOeval(gt, dt, "bbox")`` computes with its default parameters (precision / recall
+arrays and the 12 summary stats), matched, ranked and reduced by the k2y_coco_* kernels; the protocol is that of
+oracle/coco_ref.py.  ``load_coco_annotations`` reads a COCO instances JSON file, ``coco_results`` writes the records as
+a COCO results list and ``coco_summary`` prints the stats as COCOeval does.
 """
 from __future__ import annotations
 
 import ctypes
-from typing import List, Sequence, Tuple
+import json
+from typing import List, NamedTuple, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -165,4 +171,185 @@ class DetectionAP:
         h = getattr(self, "_h", None)
         if h:
             lib.k2y_ap_destroy(h)
+            self._h = None
+
+
+COCO_STATUS = {1: "a record has a negative or NaN score", 2: "a record count is outside [0, max_per_class]",
+               4: "an image position is outside [0, images)", 8: "an image was given twice since the last reset"}
+# COCOeval's default parameters, exactly its np.linspace values
+COCO_IOU_THRS = np.linspace(.5, 0.95, int(np.round((0.95 - .5) / .05)) + 1, endpoint=True)
+COCO_REC_THRS = np.linspace(.0, 1.00, int(np.round((1.00 - .0) / .01)) + 1, endpoint=True)
+COCO_MAX_DETS = (1, 10, 100)
+COCO_AREA_LBL = ("all", "small", "medium", "large")
+
+
+class CocoGroundTruth(NamedTuple):
+    """The annotations of a COCO instances file, packed for ``CocoEval``: rows float64 [n, 7] (class index, x, y, w, h,
+    area, iscrowd), image i's (in sorted image-id order, file order within) at rows [offsets[i], offsets[i + 1])."""
+    rows: np.ndarray
+    offsets: np.ndarray
+    category_ids: Tuple[int, ...]
+
+
+def load_coco_annotations(json_path: str):
+    """``(images, category_ids, gt)`` of a COCO instances JSON file: images as ``(id, file_name, (h, w))`` sorted by id
+    (all of them, with annotations or not), the sorted category ids (class index c is ``category_ids[c]``) and the
+    ``CocoGroundTruth``.  ``ValueError`` on a malformed file: a duplicate image id, an annotation of an unknown category or
+    an unlisted image, an annotation id of 0 (COCOeval reads id 0 as "unmatched") or repeated, a bbox that is not 4
+    numbers, or an iscrowd other than 0 / 1."""
+    with open(json_path) as fh:
+        data = json.load(fh)
+    try:
+        images = sorted((int(im["id"]), str(im.get("file_name", "")), (int(im["height"]), int(im["width"])))
+                        for im in data["images"])
+        cats = sorted(int(c["id"]) for c in data["categories"])
+        anns = data["annotations"]
+    except (KeyError, TypeError, ValueError) as e:
+        raise ValueError(f"{json_path}: not a COCO instances file ({e!r})") from None
+    if len({im[0] for im in images}) != len(images) or len(set(cats)) != len(cats):
+        raise ValueError(f"{json_path}: image or category ids repeat")
+    pos = {im[0]: i for i, im in enumerate(images)}
+    cls = {c: i for i, c in enumerate(cats)}
+    per_image: List[list] = [[] for _ in images]
+    seen = set()
+    for a in anns:
+        aid, img, cat = a.get("id"), a.get("image_id"), a.get("category_id")
+        if not isinstance(aid, int) or aid == 0 or aid in seen:
+            raise ValueError(f"{json_path}: annotation id {aid!r} is 0, repeated or not an integer")
+        seen.add(aid)
+        if img not in pos:
+            raise ValueError(f"{json_path}: annotation {aid} is on image {img!r}, which is not listed")
+        if cat not in cls:
+            raise ValueError(f"{json_path}: annotation {aid} has unknown category {cat!r}")
+        bbox, crowd = a.get("bbox"), a.get("iscrowd")
+        if not (isinstance(bbox, list) and len(bbox) == 4) or crowd not in (0, 1) or "area" not in a:
+            raise ValueError(f"{json_path}: annotation {aid} needs bbox [x, y, w, h], area and iscrowd 0 / 1")
+        per_image[pos[img]].append([cls[cat]] + [float(v) for v in bbox] + [float(a["area"]), float(crowd)])
+    offsets = np.zeros(len(images) + 1, np.int64)
+    np.cumsum([len(r) for r in per_image], out=offsets[1:])
+    rows = np.array([r for rs in per_image for r in rs], np.float64).reshape(-1, 7)
+    return images, cats, CocoGroundTruth(rows, offsets, tuple(cats))
+
+
+def coco_results(dets, counts, image_ids: Sequence[int], category_ids: Sequence[int]) -> List[dict]:
+    """The COCO results list of record blocks (dets int32 [N, C, K, 6], counts [N, C], host or device; image_ids [N]):
+    one entry per record within its count, per image, class and record.  A record (ymin, xmin, ymax, xmax) becomes
+    ``bbox = [xmin, ymin, xmax - xmin, ymax - ymin]``, computed in float64 from the float32 values, and its float32 score
+    as float64: what ``CocoEval`` evaluates."""
+    d = dets.cpu().numpy() if hasattr(dets, "cpu") else np.asarray(dets)
+    n = counts.cpu().numpy() if hasattr(counts, "cpu") else np.asarray(counts)
+    rec = np.ascontiguousarray(d, np.int32).view(np.float32)
+    out = []
+    for b, img in enumerate(image_ids):
+        for c, cat in enumerate(category_ids):
+            for y0, x0, y1, x1, score in rec[b, c, :int(n[b, c]), :5].astype(np.float64).tolist():
+                out.append({"image_id": int(img), "category_id": int(cat), "bbox": [x0, y0, x1 - x0, y1 - y0], "score": score})
+    return out
+
+
+def coco_stats(precision: np.ndarray, recall: np.ndarray) -> np.ndarray:
+    """COCOeval.summarize's 12 stats of precision [10, 101, C, 4, 3] and recall [10, C, 4, 3]: each the mean of the
+    selected entries > -1 (-1 without any)."""
+    def mean(ap, iou_thr=None, area="all", max_dets=100):
+        s = precision if ap else recall
+        if iou_thr is not None:
+            s = s[np.where(iou_thr == COCO_IOU_THRS)[0]]
+        a, m = COCO_AREA_LBL.index(area), COCO_MAX_DETS.index(max_dets)
+        s = s[:, :, :, [a], [m]] if ap else s[:, :, [a], [m]]
+        return -1 if len(s[s > -1]) == 0 else np.mean(s[s > -1])
+    return np.array([mean(1), mean(1, iou_thr=.5), mean(1, iou_thr=.75), mean(1, area="small"), mean(1, area="medium"),
+                     mean(1, area="large"), mean(0, max_dets=1), mean(0, max_dets=10), mean(0), mean(0, area="small"),
+                     mean(0, area="medium"), mean(0, area="large")], np.float64)
+
+
+def coco_summary(stats: Sequence[float]) -> List[str]:
+    """The 12 lines COCOeval.summarize prints for ``stats``."""
+    spec = [(1, None, "all", 100), (1, .5, "all", 100), (1, .75, "all", 100), (1, None, "small", 100),
+            (1, None, "medium", 100), (1, None, "large", 100), (0, None, "all", 1), (0, None, "all", 10),
+            (0, None, "all", 100), (0, None, "small", 100), (0, None, "medium", 100), (0, None, "large", 100)]
+    lines = []
+    for (ap, thr, area, md), v in zip(spec, stats):
+        iou = "{:0.2f}:{:0.2f}".format(COCO_IOU_THRS[0], COCO_IOU_THRS[-1]) if thr is None else "{:0.2f}".format(thr)
+        lines.append(" {:<18} {} @[ IoU={:<9} | area={:>6s} | maxDets={:>3d} ] = {:0.3f}".format(
+            "Average Precision" if ap else "Average Recall", "(AP)" if ap else "(AR)", iou, area, md, v))
+    return lines
+
+
+class CocoEval:
+    """COCOeval (bbox, default parameters) on the GPU.  The ground truth (``load_coco_annotations``) is uploaded once;
+    ``update`` matches a batch of record blocks, ``result`` ranks and reduces.  Every call runs on the current CUDA
+    stream."""
+
+    def __init__(self, gt: CocoGroundTruth, class_num: int, max_per_class: int, device=None):
+        require_cuda()
+        self.C, self.K = int(class_num), int(max_per_class)
+        if len(gt.category_ids) != self.C:
+            raise ValueError(f"the annotations have {len(gt.category_ids)} categories, the network {self.C} classes")
+        rows = np.ascontiguousarray(gt.rows, np.float64).reshape(-1, 7)
+        offsets = np.ascontiguousarray(gt.offsets, np.int64)
+        if len(offsets) < 1 or offsets[-1] != len(rows):
+            raise ValueError("ground-truth offsets do not cover the rows")
+        self.n_images = len(offsets) - 1
+        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device or "cuda")
+        self.device = torch.device("cuda", torch.cuda.current_device() if dev.index is None else dev.index)
+        h = ctypes.c_void_p()
+        check(lib.k2y_coco_create(rows.ctypes.data, offsets.ctypes.data, self.n_images, self.C, self.K,
+                                  COCO_IOU_THRS.ctypes.data, COCO_REC_THRS.ctypes.data, self.device.index,
+                                  ctypes.byref(h)))
+        self._h = h
+
+    def _stream(self):
+        return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def update(self, dets: torch.Tensor, counts: torch.Tensor, image_positions) -> None:
+        """dets int32 ``[N, C, K, 6]`` (dense per image) and counts int32 ``[N, C]`` as ``DetectionPipeline`` returns
+        them (device views of ``step_device`` or pinned host views of ``collect``, strided per image); image_positions:
+        each image's index in the sorted image list of ``load_coco_annotations``.  Device records are read
+        asynchronously on the current stream; host records have been copied when this returns."""
+        pos = np.asarray(image_positions.cpu() if hasattr(image_positions, "cpu") else image_positions, np.int64).reshape(-1)
+        n = len(pos)
+        if (dets.dtype != torch.int32 or counts.dtype != torch.int32 or dets.dim() != 4 or counts.dim() != 2
+                or tuple(dets.shape) != (n, self.C, self.K, 6) or tuple(counts.shape) != (n, self.C)
+                or tuple(dets.stride()[1:]) != (self.K * 6, 6, 1) or counts.stride(1) != 1 or dets.is_cuda != counts.is_cuda):
+            raise ValueError(f"expected int32 dets [{n}, {self.C}, {self.K}, 6] (dense per image) and counts [{n}, {self.C}] "
+                             f"on one side of the bus, one per image position; got {tuple(dets.shape)} / {tuple(counts.shape)}")
+        if n == 0:
+            return
+        with torch.cuda.device(self.device):
+            if dets.is_cuda:
+                if dets.device != self.device or counts.device != self.device:
+                    raise ValueError(f"records on {dets.device}, evaluator on {self.device}")
+            else:   # a blocking copy: the host views may be overwritten as soon as this returns
+                dets, counts = dets.to(self.device), counts.to(self.device)
+            positions = torch.from_numpy(pos).to(self.device)
+            check(lib.k2y_coco_match(self._h, dets.data_ptr(), counts.data_ptr(), dets.stride(0), counts.stride(0), n,
+                                     positions.data_ptr(), self._stream()))
+
+    def result(self) -> dict:
+        """``{"precision": [10, 101, C, 4, 3], "recall": [10, C, 4, 3], "stats": [12], "ap_per_class": [C]}``: COCOeval's
+        eval arrays and summary stats, and per class the mean of precision[:, :, c, all, 100] over its entries > -1 (NaN
+        for a class without ground truth).  ``ValueError`` if an update held an invalid record or image position."""
+        precision = np.zeros((len(COCO_IOU_THRS), len(COCO_REC_THRS), self.C, 4, 3))
+        recall = np.zeros((len(COCO_IOU_THRS), self.C, 4, 3))
+        status = ctypes.c_uint()
+        with torch.cuda.device(self.device):
+            check(lib.k2y_coco_result(self._h, precision.ctypes.data, recall.ctypes.data, ctypes.byref(status),
+                                      self._stream()))
+        if status.value:
+            raise ValueError("CocoEval: " + "; ".join(m for bit, m in COCO_STATUS.items() if status.value & bit))
+        per_class = np.full(self.C, np.nan)
+        for c in range(self.C):
+            s = precision[:, :, c, 0, 2]
+            if np.any(s > -1):
+                per_class[c] = np.mean(s[s > -1])
+        return {"precision": precision, "recall": recall, "stats": coco_stats(precision, recall), "ap_per_class": per_class}
+
+    def reset(self) -> None:
+        with torch.cuda.device(self.device):
+            check(lib.k2y_coco_reset(self._h, self._stream()))
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            lib.k2y_coco_destroy(h)
             self._h = None
