@@ -303,7 +303,8 @@ int k2y_jpeg_decode(const void *blob_host, const void *blob_dev, const unsigned 
 /* ------------------------------------------------------------------------------------------
  * Baseline JPEG encoding, byte-identical to PIL's Image.fromarray(rgb).save(f, "JPEG", quality=q) with libjpeg-turbo 3.1:
  * JFIF APP0, two DQT, SOF0 4:2:0, the four standard Huffman tables, one interleaved scan, EOI.
- *   k2y_jpeg_encode_plan             host only: the descriptor blob of n images, hw_host int32 [n][2] (1..65535 each),
+ *   k2y_jpeg_encode_plan             host only: the descriptor blob of n images, hw_host int32 [n][2] (1..65500 each:
+ *                                    libjpeg-turbo's JPEG_MAX_DIMENSION; PIL writes and reads no larger file),
  *                                    src_offsets_host: where image i's h*w*3 RGB bytes lie in the device source buffer.
  *                                    blob == NULL: only *blob_bytes (size query); else a 16-byte aligned host buffer.
  *                                    quality 1..100; anything else is K2Y_ERR_INVALID.
@@ -314,7 +315,8 @@ int k2y_jpeg_decode(const void *blob_host, const void *blob_dev, const unsigned 
  * ---------------------------------------------------------------------------------------- */
 int k2y_jpeg_encode_plan(int n, const int *hw_host, const long long *src_offsets_host, int quality, void *blob,
                          size_t blob_capacity, size_t *blob_bytes);
-/* Host only: the bytes a file of that size and quality starts with, SOI up to and including SOS (out == NULL: size query). */
+/* Host only: the bytes a file of that size (1..65500 each) and quality starts with, SOI up to and including SOS (out == NULL:
+ * size query). */
 int k2y_jpeg_encode_header(int h, int w, int quality, unsigned char *out, size_t capacity, size_t *length);
 int k2y_jpeg_encode_workspace_bytes(const void *blob_host, size_t *workspace_bytes, size_t *output_capacity);
 int k2y_jpeg_encode(const void *blob_host, const void *blob_dev, const unsigned char *src_dev, unsigned char *dst_dev,
@@ -323,8 +325,9 @@ int k2y_jpeg_encode(const void *blob_host, const void *blob_dev, const unsigned 
 /* ------------------------------------------------------------------------------------------
  * Detection rendering in place, pixel for pixel draw.draw_detections (see csrc/render.cu for the one deliberate difference:
  * a box whose outline rings cross stops at the first crossing ring instead of raising).  images_dev: packed HWC RGB, image i
- * at offsets_host[i] with size hw_host[i] (1..65535 each).  atlas_dev[i]: the device label atlas of image i's font
- * (render.LabelAtlas: int32 header [8] with [0] = classes, int32 entries [classes][101][8], then the glyph masks).  dets_dev /
+ * at offsets_host[i] with size hw_host[i] (1..65535 each: drawing is not bound by the encoder's 65500).  atlas_dev[i]: the
+ * device label atlas of image i's font (render.LabelAtlas: int32 header [8] with [0] = classes, int32 entries
+ * [classes][101][8], then the glyph masks).  dets_dev /
  * counts_dev: k2y_det records [n][class_num][max_per_class] and counts [n][class_num] with the given per-image strides.
  * colors_dev: uint8 [class_num][3], class_num 1..80.  Asynchronous on `stream`, one launch per 128 images.
  * ---------------------------------------------------------------------------------------- */

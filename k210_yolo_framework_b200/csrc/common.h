@@ -12,6 +12,9 @@ namespace k2y {
 
 void set_error(const char *fmt, ...);
 
+// libjpeg-turbo's JPEG_MAX_DIMENSION: it (and so PIL) refuses to write or read a frame with more rows or columns.
+constexpr int JPEG_MAX_DIMENSION = 65500;
+
 #define K2Y_CUDA_CHECK(expr)                                                                     \
     do {                                                                                         \
         cudaError_t _e = (expr);                                                                 \

@@ -318,6 +318,9 @@ int parse_jpeg(const uint8_t *d, size_t n, Parsed &p, const char *who) {
         i = next;
     }
     // classification of an 8-bit sequential Huffman file
+    // jdinput.c initial_setup: libjpeg-turbo refuses a larger frame at the first SOS, so PIL cannot read the file
+    if (p.h > JPEG_MAX_DIMENSION || p.w > JPEG_MAX_DIMENSION)
+        return set_reason(p, "%dx%d exceeds libjpeg's %d-pixel limit", p.w, p.h, JPEG_MAX_DIMENSION), K2Y_OK;
     if (p.ncomp == 2) return set_reason(p, "2 components"), K2Y_OK;
     if (p.ncomp == 4) return set_reason(p, "4 components (CMYK/YCCK)"), K2Y_OK;
     if (p.ncomp == 3 && !p.jfif) {   // libjpeg's default_decompress_parms

@@ -668,8 +668,8 @@ extern "C" int k2y_jpeg_encode_plan(int n, const int *hw_host, const long long *
     }
     for (int i = 0; i < n; ++i) {
         const int h = hw_host[2 * i], w = hw_host[2 * i + 1];
-        if (h < 1 || h > 65535 || w < 1 || w > 65535) {
-            set_error("k2y_jpeg_encode_plan: image %d is %dx%d; baseline JPEG takes 1..65535 rows and columns", i, h, w);
+        if (h < 1 || h > JPEG_MAX_DIMENSION || w < 1 || w > JPEG_MAX_DIMENSION) {
+            set_error("k2y_jpeg_encode_plan: image %d is %dx%d; JPEG files have 1..%d rows and columns (libjpeg's limit)", i, h, w, JPEG_MAX_DIMENSION);
             return K2Y_ERR_INVALID;
         }
         if (src_offsets_host[i] < 0) {
@@ -758,8 +758,9 @@ extern "C" int k2y_jpeg_encode_plan(int n, const int *hw_host, const long long *
 }
 
 extern "C" int k2y_jpeg_encode_header(int h, int w, int quality, unsigned char *out, size_t capacity, size_t *length) {
-    if (h < 1 || h > 65535 || w < 1 || w > 65535 || quality < 1 || quality > 100 || !length) {
-        set_error("k2y_jpeg_encode_header: %dx%d at quality %d (1..65535 rows and columns, quality 1..100)", h, w, quality);
+    if (h < 1 || h > JPEG_MAX_DIMENSION || w < 1 || w > JPEG_MAX_DIMENSION || quality < 1 || quality > 100 || !length) {
+        set_error("k2y_jpeg_encode_header: %dx%d at quality %d (1..%d rows and columns, quality 1..100)", h, w, quality,
+                  JPEG_MAX_DIMENSION);
         return K2Y_ERR_INVALID;
     }
     uint16_t qt[2][64];

@@ -179,7 +179,8 @@ class DetectionPipeline:
         ``draw.draw_detections`` draws them, ``render.render_detections_device``) and encoded as JPEG files (as PIL saves them at
         `quality`, ``render.JpegEncoder``), on the decode stream behind the NMS; ``rendered(ticket)`` returns them after
         ``collect``.  `colormap`: RGB triples per class (default ``Helper.colormap``, 80 classes).  Records and ``collect``
-        are unchanged."""
+        are unchanged.  ``submit_images`` then refuses an image with more than ``render.JPEG_MAX_DIMENSION`` (65500) rows or
+        columns, which no JPEG file can hold."""
         from .helper import _COLORMAP
         from .render import JpegEncoder, LabelAtlas, color_table
         colormap = _COLORMAP if colormap is None else colormap
@@ -231,6 +232,11 @@ class DetectionPipeline:
         n = len(layout)
         if n > self.batch:
             raise ValueError(f"{n} images do not fit a batch of {self.batch}")
+        if self._render is not None:
+            from .render import JPEG_MAX_DIMENSION
+            for i, (h, w) in enumerate(layout.hw.tolist()):
+                if h > JPEG_MAX_DIMENSION or w > JPEG_MAX_DIMENSION:
+                    raise ValueError(f"image {i} is {h}x{w}: a rendered JPEG file has at most {JPEG_MAX_DIMENSION} rows and columns")
         slot = self._submitted % SLOTS
         buf = self._input_slots(True)[slot]
         dev = buf.device

@@ -20,13 +20,14 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 import torch
 
-from ._lib import check, lib
+from ._lib import K2YError, check, lib
 from .draw import label_font_size
 
 LABELS_PER_CLASS = 101      # hundredths 0..100
 HEADER_WORDS = 8            # atlas header: [0] classes
 ENTRY_WORDS = 8             # mask byte offset, mask w, mask h, mask x, mask y, label w, label h, 0
 MAX_CLASSES = 80            # the colour table's classes (Helper.colormap)
+JPEG_MAX_DIMENSION = 65500  # libjpeg-turbo's limit: PIL neither writes nor reads a JPEG with more rows or columns
 _LL = ctypes.POINTER(ctypes.c_longlong)
 _INT = ctypes.POINTER(ctypes.c_int)
 
@@ -201,8 +202,9 @@ class JpegEncoder:
         n = len(offsets)
         offsets = np.ascontiguousarray(offsets, np.int64)
         hw = np.ascontiguousarray(hw, np.int32)
-        if n == 0 or (hw < 1).any() or (hw > 65535).any():
-            raise ValueError("every image must have 1..65535 rows and columns")
+        if n == 0 or (hw < 1).any() or (hw > JPEG_MAX_DIMENSION).any():
+            bad = [f"{h}x{w}" for h, w in hw.tolist() if not (1 <= h <= JPEG_MAX_DIMENSION and 1 <= w <= JPEG_MAX_DIMENSION)]
+            raise ValueError(f"every image must have 1..{JPEG_MAX_DIMENSION} rows and columns (libjpeg's limit), got {', '.join(bad)}")
         nbytes = ctypes.c_size_t()
         check(lib.k2y_jpeg_encode_plan(n, hw.ctypes.data_as(_INT), offsets.ctypes.data_as(_LL), q, None, 0, ctypes.byref(nbytes)))
         self.ready.synchronize()        # the previous blob copy out of the pinned buffer has finished
@@ -240,9 +242,18 @@ class JpegEncoder:
         return [data[e - l:e] for l, e in zip(lengths.tolist(), ends.tolist())]
 
 
+class JpegArgumentError(K2YError, ValueError):
+    """A size or quality no JPEG file can have: a ``ValueError``, and the ``K2YError`` the library's refusal raises."""
+
+
 def jpeg_header(h: int, w: int, quality: int = 75) -> bytes:
     """The marker segments (SOI .. SOS) ``encode_jpeg_batch`` writes in front of an h x w image's entropy-coded data; built on
-    the host."""
+    the host.  Raises ``JpegArgumentError`` for a size PIL cannot write (outside 1..``JPEG_MAX_DIMENSION`` rows or columns) or
+    a quality outside 1..100."""
+    if not (1 <= int(h) <= JPEG_MAX_DIMENSION and 1 <= int(w) <= JPEG_MAX_DIMENSION):
+        raise JpegArgumentError(f"{h}x{w}: JPEG files have 1..{JPEG_MAX_DIMENSION} rows and columns (libjpeg's limit)")
+    if not 1 <= int(quality) <= 100:
+        raise JpegArgumentError(f"quality {quality} is outside 1..100")
     n = ctypes.c_size_t()
     check(lib.k2y_jpeg_encode_header(int(h), int(w), int(quality), None, 0, ctypes.byref(n)))
     buf = (ctypes.c_ubyte * n.value)()
