@@ -85,53 +85,50 @@ __device__ __forceinline__ uint32_t a_addr(uint32_t box, int r, int k) {
 constexpr int PRODUCER_REGS = 152;
 constexpr int CONSUMER_REGS = 176;
 
+// Attribution builds (scripts/bench_conv_tc.py), never the shipped library: K2Y_TC_ABLATE = 1 drops the epilogue's stores to
+// global memory, 2 skips the MMAs (loads, splits and barriers stay), 3 skips the A split (the raw bits are the hi plane, lo
+// is zero).  Results are wrong in every variant; only the time means something.
+#ifndef K2Y_TC_ABLATE
+#define K2Y_TC_ABLATE 0
+#endif
+constexpr int ABLATE = K2Y_TC_ABLATE;
+
 template <int I>
 struct Buf {
     static constexpr int value = I;
 };
 
 // The MMAs of one k-block for one consumer warpgroup, NKS k-steps of it (the rest of the k-block is K padding), as one batch:
-// a fence, the wgmmas, one commit.  Per k-step and tile column the split schemes issue lo*hi, hi*lo, hi*hi.
+// a fence, the wgmmas, one commit.  Per k-step the split schemes issue lo*hi, hi*lo, hi*hi, each one MMA over the whole tile
+// width (N columns are independent, so every accumulator sees the same sequence of MMAs as with narrower instructions; 16-
+// column MMAs for the tail of a tile that was no multiple of 64 wide left the tensor pipe mostly idle).
 template <int MODE, int BNT, int NKS>
 __device__ __forceinline__ void mma_ksteps(float (&acc)[BNT / 2], const uint32_t (&ahi)[4][4], const uint32_t (&alo)[4][4],
                                            uint64_t dhi, uint64_t dlo, uint32_t accumulate) {
-    constexpr int nb64 = BNT / 64;  // 64-column MMAs first, then 16-column ones for the rest
+    using W = Wgmma<BNT>;  // the whole tile width in one MMA
     wgmma_fence();
+    if constexpr (ABLATE == 2) {
+#pragma unroll
+        for (int kk = 0; kk < NKS; ++kk)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) asm volatile("" ::"r"(ahi[kk][j]), "r"(alo[kk][j]));  // keep the split alive
+        wgmma_commit();
+        return;
+    }
 #pragma unroll
     for (int kk = 0; kk < NKS; ++kk) {
-        const uint64_t adv = (uint64_t)((kk * 32) >> 4);  // 32 bytes of B per k-step inside the 128 B swizzle row
+        const uint64_t o = (uint64_t)((kk * 32) >> 4);  // 32 bytes of B per k-step inside the 128 B swizzle row
         const uint32_t first = kk == 0 ? accumulate : 1u;
-#pragma unroll
-        for (int j = 0; j < nb64; ++j) {
-            const uint64_t o = adv + (uint64_t)((j * 64 * 128) >> 4);
-            float *d = acc + j * 32;
-            if constexpr (MODE == K2Y_MATH_TC_BF16X3) {
-                wgmma_bf16_n64(d, alo[kk], dhi + o, first);
-                wgmma_bf16_n64(d, ahi[kk], dlo + o, 1u);
-                wgmma_bf16_n64(d, ahi[kk], dhi + o, 1u);
-            } else if constexpr (MODE == K2Y_MATH_TC_3XTF32) {
-                wgmma_tf32_n64(d, alo[kk], dhi + o, first);
-                wgmma_tf32_n64(d, ahi[kk], dlo + o, 1u);
-                wgmma_tf32_n64(d, ahi[kk], dhi + o, 1u);
-            } else {
-                wgmma_tf32_n64(d, ahi[kk], dhi + o, first);
-            }
-        }
-#pragma unroll
-        for (int j = nb64 * 4; j < BNT / 16; ++j) {
-            const uint64_t o = adv + (uint64_t)((j * 16 * 128) >> 4);
-            float *d = acc + j * 8;
-            if constexpr (MODE == K2Y_MATH_TC_BF16X3) {
-                wgmma_bf16_n16(d, alo[kk], dhi + o, first);
-                wgmma_bf16_n16(d, ahi[kk], dlo + o, 1u);
-                wgmma_bf16_n16(d, ahi[kk], dhi + o, 1u);
-            } else if constexpr (MODE == K2Y_MATH_TC_3XTF32) {
-                wgmma_tf32_n16(d, alo[kk], dhi + o, first);
-                wgmma_tf32_n16(d, ahi[kk], dlo + o, 1u);
-                wgmma_tf32_n16(d, ahi[kk], dhi + o, 1u);
-            } else {
-                wgmma_tf32_n16(d, ahi[kk], dhi + o, first);
-            }
+        if constexpr (MODE == K2Y_MATH_TC_BF16X3) {
+            W::bf16(acc, alo[kk], dhi + o, first);
+            W::bf16(acc, ahi[kk], dlo + o, 1u);
+            W::bf16(acc, ahi[kk], dhi + o, 1u);
+        } else if constexpr (MODE == K2Y_MATH_TC_3XTF32) {
+            W::tf32(acc, alo[kk], dhi + o, first);
+            W::tf32(acc, ahi[kk], dlo + o, 1u);
+            W::tf32(acc, ahi[kk], dhi + o, 1u);
+        } else {
+            W::tf32(acc, ahi[kk], dhi + o, first);
         }
     }
     wgmma_commit();
@@ -336,6 +333,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 }
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
+                    if constexpr (ABLATE == 3) {
+                        hi[kk][j] = __byte_perm(__float_as_uint(v[j][0]), __float_as_uint(v[j][1]), 0x7632);
+                        lo[kk][j] = 0u;
+                        continue;
+                    }
                     const uint32_t h = pack_bf16x2(v[j][0], v[j][1]);
                     hi[kk][j] = h;
                     lo[kk][j] = pack_bf16x2(v[j][0] - __uint_as_float(h << 16), v[j][1] - __uint_as_float(h & 0xffff0000u));
@@ -345,6 +347,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const float x = ld_shared_f32(a_addr(sa, r0 + 8 * (j & 1), kk * 8 + tq + 4 * (j >> 1)));
+                    if constexpr (ABLATE == 3) {
+                        hi[kk][j] = __float_as_uint(x);
+                        lo[kk][j] = 0u;
+                        continue;
+                    }
                     const float h = to_tf32_rna(x);
                     hi[kk][j] = __float_as_uint(THREE_X ? h : x);
                     if (THREE_X) lo[kk][j] = __float_as_uint(to_tf32_rna(x - h));
@@ -444,7 +451,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 fence_proxy_async_smem();
                 if (lead) bulk_wait_group_0<true>();
                 named_bar_sync(1 + cg, 128);
-                if (lead) {
+                if (lead && ABLATE != 1) {
                     tma_store_2d(full ? &map_c : &map_c16, buf, nt * BNT + 32 * j, row0);
                     bulk_commit_group();
                 }
@@ -452,6 +459,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             continue;
         }
         // ---- epilogue: folded BN + activation (+ residual) straight from the accumulator registers ----
+        if constexpr (ABLATE == 1) continue;
         const int n_base = nt * BNT + 2 * tq;
         if (p.partial) {
             // split-K partial of slice ks: raw sums, rows [ks * m_tiles * 128, ...) of the scratch tensor (N % 4 == 0)
