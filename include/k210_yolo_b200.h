@@ -171,6 +171,25 @@ int k2y_detect_keras_strided(const k2y_detect_cfg *cfg, const float *const *head
                              long long det_image_stride_words, long long count_image_stride_words, void *workspace,
                              size_t workspace_bytes, void *stream);
 
+/* Merge of views (tiled detection): an image was detected as `views` views - view 0 the whole image, the others windows of
+ * it, each letterboxed and decoded as an image of its own (k2y_letterbox_u8_views) - and this call turns their record lists
+ * into one list per (image, class) in image coordinates.
+ *   view_dets_dev / view_counts_dev: [n_images * views][C][max_per_class] records and [n_images * views][C] counts, dense,
+ *   image-major, as k2y_detect_keras writes them for n_images * views inputs.  view_yx_dev: [n_images * views][2] float32
+ *   (y0, x0), each view's origin in its image (k2y_letterbox_u8_views writes it).
+ * Per image and class: every record of every view v gets (y0, x0, y0, x0) added to (ymin, xmin, ymax, xmax) (one float32
+ * round-to-nearest add each, no clipping) and index = v * n_boxes + index (n_boxes: the boxes of one network input, so
+ * index / n_boxes tells the view and view 0 keeps its indices); the union is ordered by score descending, then view, then
+ * index ascending, and goes through the greedy NMS of k2y_detect_keras (suppressed iff IoU > iou_thresh, a zero-area box
+ * has IoU 0) until max_per_class are kept.  Outputs as k2y_detect_keras_strided's, for `rows` >= n_images images: rows past
+ * n_images get count 0.  One launch, asynchronous on `stream`, no scratch memory.
+ * K2Y_ERR_INVALID (nothing launched) when views * max_per_class exceeds k2y_merge_views_max_records() (1024: VOC's 30 per
+ * class takes 34 views, COCO's 100 takes 10) or views * n_boxes exceeds INT32_MAX. */
+int k2y_merge_views_max_records(void);
+int k2y_merge_views(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev, int n_images, int rows,
+                    int views, int n_boxes, int class_num, int max_per_class, float iou_thresh, k2y_det *dets_dev,
+                    int32_t *counts_dev, long long det_image_stride_words, long long count_image_stride_words, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Multi-GPU collation: images shard across ranks (one process per GPU), and the one exchange on the path
  * is ONE ncclAllGather of the fixed-size record blocks.  The reference is single-process (keras_inference.py:12-17), so
@@ -256,6 +275,17 @@ int k2y_letterbox_u8(const unsigned char *src_dev, int src_h, int src_w, const d
 int k2y_letterbox_u8_batch(const unsigned char *src_dev, int n, const long long *offsets_host, const int *hw_host,
                            const double *inv_matrices_host, unsigned char *dst_dev, int dst_h, int dst_w,
                            float *image_hw_dev, int *minmax_dev, void *stream);
+/* The same letterbox for n_views VIEWS: view i is the window windows_host[i] = (y0, x0, th, tw), in pixels, of the image at
+ * offsets_host[i] whose full size is hw_host[i]; several views may name the same image.  A view is letterboxed as the crop
+ * img[y0:y0+th, x0:x0+tw] submitted as an image of its own would be: inv_matrices_host[i] is the matrix of a th x tw image,
+ * pixels outside the window read as zero fill (not as the neighbouring pixels) and the output is clipped to the window's own
+ * min and max.  image_hw_dev receives (th, tw) per view, view_yx_dev ([n_views][2] float32, or NULL) receives (y0, x0), which
+ * k2y_merge_views adds to the view's boxes.  A window that is not inside its image is K2Y_ERR_INVALID before anything is
+ * enqueued.  k2y_letterbox_u8_batch is the case of one whole-image window per image; the work is the same one memset and two
+ * kernels per 48 views. */
+int k2y_letterbox_u8_views(const unsigned char *src_dev, int n_views, const long long *offsets_host, const int *hw_host,
+                           const int *windows_host, const double *inv_matrices_host, unsigned char *dst_dev, int dst_h, int dst_w,
+                           float *image_hw_dev, float *view_yx_dev, int *minmax_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * Baseline JPEG decode on the device, in front of k2y_letterbox_u8_batch: replaces the file decode of

@@ -93,6 +93,9 @@ _SIGNATURES = {
                                  c_size_t, c_void_p]),
     "k2y_detect_keras_strided": (c_int, [POINTER(DetectCfg), POINTER(c_void_p), c_int, c_void_p, c_void_p, c_void_p,
                                          ctypes.c_longlong, ctypes.c_longlong, c_void_p, c_size_t, c_void_p]),
+    "k2y_merge_views_max_records": (c_int, []),
+    "k2y_merge_views": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
+                                ctypes.c_longlong, ctypes.c_longlong, c_void_p]),
     "k2y_comm_unique_id": (c_int, [c_void_p]),
     "k2y_comm_create": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_void_p)]),
     "k2y_comm_destroy": (c_int, [c_void_p]),
@@ -112,6 +115,8 @@ _SIGNATURES = {
     "k2y_letterbox_u8": (c_int, [c_void_p, c_int, c_int, POINTER(ctypes.c_double), c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "k2y_letterbox_u8_batch": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong), POINTER(c_int), POINTER(ctypes.c_double), c_void_p,
                                        c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "k2y_letterbox_u8_views": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong), POINTER(c_int), POINTER(c_int), POINTER(ctypes.c_double),
+                                       c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "k2y_jpeg_inspect": (c_int, [c_void_p, c_size_t, POINTER(JpegInfo)]),
     "k2y_jpeg_plan": (c_int, [POINTER(c_void_p), POINTER(c_size_t), c_int, POINTER(ctypes.c_longlong), POINTER(ctypes.c_longlong),
                               c_void_p, c_size_t, POINTER(c_size_t)]),

@@ -1003,6 +1003,126 @@ __global__ void __launch_bounds__(32) nms_boxes_kernel(const float4 *__restrict_
     if (lane == 0) *out_count = nsel;
 }
 
+// ---- merge of views.  grid = (C, rows), one CTA of MERGE_THREADS per (image, class) ---------------------------------------
+// An image detected as V views (view 0 the whole image, the others windows of it, k2y_letterbox_u8_views) has V record lists
+// per class, each in the window's own coordinates.  The merge moves them into image coordinates (one float32 add of the
+// window's origin per coordinate), renumbers them (index = view * nbox + index) and runs the detector's greedy NMS once more
+// over their union in (score descending, view ascending, index ascending) order.  The union is at most MERGE_MAX records, all
+// in shared memory: keys (pack_key of the score and the new index) sorted by warp 0, every record's box scattered to its key's
+// rank (binary search; the keys are unique), then rounds of "first candidate still alive -> keep -> every thread tests its own
+// two candidates against it", one barrier per round, liveness exchanged as one ballot word per 32 candidates.
+constexpr int MERGE_THREADS = 512;
+constexpr int MERGE_MAX = 2 * MERGE_THREADS;   // records of one (image, class) over all views
+static_assert(MERGE_MAX == 1024, "one liveness word per lane: 32 words of 32 candidates");
+
+struct MergeParams {
+    const k2y_det *vdets;   // [n * V][C][K]
+    const int *vcounts;     // [n * V][C]
+    const float *view_yx;   // [n * V][2] (y0, x0)
+    int n, V, C, K, nbox;
+    float iou;
+    k2y_det *dets;
+    int *counts;
+    long long det_stride, cnt_stride;
+};
+
+__global__ void __launch_bounds__(MERGE_THREADS) merge_views_kernel(const MergeParams p) {
+    __shared__ unsigned long long s_keys[MERGE_MAX];   // arrival order (view, then position in the view's list), then sorted
+    __shared__ float4 s_box[MERGE_MAX];                // shifted boxes in sorted order
+    __shared__ int s_off[MERGE_MAX + 1];               // first arrival position of view v (V <= MERGE_MAX)
+    __shared__ unsigned s_alive[2][32];
+    const int c = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    k2y_det *out = reinterpret_cast<k2y_det *>(reinterpret_cast<int *>(p.dets) + (size_t)b * p.det_stride) + (size_t)c * p.K;
+    int *count_out = p.counts + (size_t)b * p.cnt_stride + c;
+    if (b >= p.n) {
+        if (tid == 0) *count_out = 0;
+        return;
+    }
+    const size_t view0 = (size_t)b * p.V;
+    for (int v = tid; v < p.V; v += MERGE_THREADS) s_off[v + 1] = min(max(p.vcounts[(view0 + v) * p.C + c], 0), p.K);
+    __syncthreads();
+    if (tid == 0) {
+        s_off[0] = 0;
+        for (int v = 0; v < p.V; ++v) s_off[v + 1] += s_off[v];
+    }
+    __syncthreads();
+    const int n = s_off[p.V];
+    if (n == 0) {
+        if (tid == 0) *count_out = 0;
+        return;
+    }
+    // slot i = v * K + k of the per-view lists: at most two per thread (V * K <= MERGE_MAX), kept in registers until the sort is done
+    unsigned long long mykey[2] = {0ull, 0ull};
+    float4 mybox[2];
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+        const int i = tid + s * MERGE_THREADS, v = i / p.K, k = i - v * p.K;
+        if (v >= p.V || k >= s_off[v + 1] - s_off[v]) continue;
+        const k2y_det d = p.vdets[((view0 + v) * p.C + c) * p.K + k];
+        const float y0 = p.view_yx[2 * (view0 + v)], x0 = p.view_yx[2 * (view0 + v) + 1];
+        mybox[s] = make_float4(__fadd_rn(d.ymin, y0), __fadd_rn(d.xmin, x0), __fadd_rn(d.ymax, y0), __fadd_rn(d.xmax, x0));
+        s_keys[s_off[v] + k] = mykey[s] = pack_key(d.score, v * p.nbox + d.index);
+    }
+    int P = 32;
+    while (P < n) P <<= 1;
+    for (int i = n + tid; i < P; i += MERGE_THREADS) s_keys[i] = 0ull;
+    __syncthreads();
+    if (warp == 0) {
+        if (n <= 32) s_keys[lane] = warp_sort_desc(s_keys[lane], lane);
+        else warp_sort_desc_mem(s_keys, P, lane);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+        if (mykey[s] == 0ull) continue;   // a real key is never 0: its index field is inverted
+        int lo = 0, hi = n - 1;           // descending, unique: the rank of a key is the number of keys above it
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (s_keys[mid] > mykey[s]) lo = mid + 1;
+            else hi = mid;
+        }
+        s_box[lo] = mybox[s];
+    }
+    __syncthreads();
+    // candidate tid + s * MERGE_THREADS is this thread's slot s; liveness word w covers candidates 32 w .. 32 w + 31
+    float4 nb[2];
+    float ar[2];
+    bool alive[2];
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+        const int pos = tid + s * MERGE_THREADS;
+        alive[s] = pos < n;
+        nb[s] = norm_box(alive[s] ? s_box[pos] : make_float4(0.f, 0.f, 0.f, 0.f), ar[s]);
+    }
+    int nsel = 0, par = 0;
+    while (nsel < p.K) {
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+            const unsigned m = __ballot_sync(FULL, alive[s]);
+            if (lane == 0) s_alive[par][warp + s * (MERGE_THREADS / 32)] = m;
+        }
+        __syncthreads();
+        const unsigned word = s_alive[par][lane];
+        par ^= 1;
+        const unsigned any = __ballot_sync(FULL, word != 0u);
+        if (any == 0u) break;
+        const int w = __ffs(any) - 1;
+        const int best = 32 * w + __ffs(__shfl_sync(FULL, word, w)) - 1;   // first in the order still alive: kept
+        const float4 ob = s_box[best];
+        float ka;
+        const float4 kb = norm_box(ob, ka);
+        if (tid == 0) {
+            const unsigned long long k = s_keys[best];
+            write_det(out, nsel, ob, key_score(k), key_index(k));
+        }
+#pragma unroll
+        for (int s = 0; s < 2; ++s)
+            if (alive[s] && (tid + s * MERGE_THREADS == best || iou_norm_gt_eo(kb, ka, nb[s], ar[s], p.iou))) alive[s] = false;
+        ++nsel;
+    }
+    if (tid == 0) *count_out = nsel;
+}
+
 inline int next_pow2(int v) {
     int p = 64;
     while (p < v) p <<= 1;
@@ -1152,6 +1272,49 @@ extern "C" int k2y_detect_keras_strided(const k2y_detect_cfg *cfg, const float *
     K2Y_CUDA_CHECK(cudaGetLastError());
     if (p.cap <= 2048) launch_k(detect_nms_kernel<4>, dim3(p.C, batch), dim3(NMS_THREADS), nms_smem, st, p);
     else launch_k(detect_nms_kernel<8>, dim3(p.C, batch), dim3(NMS_THREADS), nms_smem, st, p);
+    K2Y_CUDA_CHECK(cudaGetLastError());
+    return K2Y_OK;
+}
+
+extern "C" int k2y_merge_views_max_records(void) { return MERGE_MAX; }
+
+extern "C" int k2y_merge_views(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev, int n_images,
+                               int rows, int views, int n_boxes, int class_num, int max_per_class, float iou_thresh, k2y_det *dets_dev,
+                               int32_t *counts_dev, long long det_image_stride_words, long long count_image_stride_words,
+                               void *stream) {
+    if (!view_dets_dev || !view_counts_dev || !view_yx_dev || !dets_dev || !counts_dev || n_images < 0 || rows < 1 || rows < n_images ||
+        views < 1 || n_boxes < 1 || class_num < 1 || class_num > 65535 || max_per_class < 1) {
+        set_error("k2y_merge_views: null pointer, or not 0 <= n_images <= rows, rows, views, n_boxes, max_per_class >= 1, class_num 1..65535");
+        return K2Y_ERR_INVALID;
+    }
+    if ((long long)views * max_per_class > MERGE_MAX) {
+        set_error("k2y_merge_views: %d views x %d records per class exceed the %d records one merge holds", views, max_per_class,
+                  MERGE_MAX);
+        return K2Y_ERR_INVALID;
+    }
+    if ((long long)views * n_boxes > 0x7fffffffLL) {
+        set_error("k2y_merge_views: view * n_boxes + index does not fit the record's int32 index (%d views x %d boxes)", views, n_boxes);
+        return K2Y_ERR_INVALID;
+    }
+    if (det_image_stride_words < (long long)class_num * max_per_class * 6 || count_image_stride_words < class_num) {
+        set_error("k2y_merge_views: image strides smaller than one image's records / counts");
+        return K2Y_ERR_INVALID;
+    }
+    MergeParams p;
+    p.vdets = view_dets_dev;
+    p.vcounts = view_counts_dev;
+    p.view_yx = view_yx_dev;
+    p.n = n_images;
+    p.V = views;
+    p.C = class_num;
+    p.K = max_per_class;
+    p.nbox = n_boxes;
+    p.iou = iou_thresh;
+    p.dets = dets_dev;
+    p.counts = counts_dev;
+    p.det_stride = det_image_stride_words;
+    p.cnt_stride = count_image_stride_words;
+    merge_views_kernel<<<dim3(class_num, rows), MERGE_THREADS, 0, (cudaStream_t)stream>>>(p);
     K2Y_CUDA_CHECK(cudaGetLastError());
     return K2Y_OK;
 }

@@ -24,15 +24,23 @@ slot's ``image_hw``, so two batches in flight each carry their own original size
 are drawn onto its original images where they lie in the slot's device staging buffer and encoded as JPEG files;
 ``rendered(ticket)`` brings them back after ``collect`` with one exact-size copy.  The next ``submit_images`` into that input
 slot waits for the render before it overwrites the originals.
+
+``enable_tiling`` makes ``submit_images`` detect on overlapping tiles of each image as well as on the whole image: a batch of
+n <= batch // V images is letterboxed as n * V views, the network and the decode run on those, and one more per-class NMS
+(``k2y_merge_views``, on the decode stream) merges each image's views into rows [0, n) of the gather slot, in image
+coordinates and in the usual block format, so everything behind it is unchanged.
 """
 from __future__ import annotations
 
 from typing import List, Optional, Sequence
 
+import ctypes
+
 import numpy as np
 import torch
 
 from . import yolonet
+from ._lib import check, lib
 from .detect import DET_WORDS, KerasDetector
 from .dist import DetectionGather
 from .preprocess import BatchLayout, Staging, check_jpeg_status, letterbox_packed
@@ -87,6 +95,45 @@ class DetectionPipeline:
         self._render_done = [torch.cuda.Event() for _ in range(SLOTS)]   # files of gather slot ready to copy back
         self._render_free = [torch.cuda.Event() for _ in range(SLOTS)]   # render + encode finished with input slot's originals
         self._rendered_slot: List[bool] = [False] * SLOTS
+        # enable_tiling: (rows, cols, overlap), views per image, the per-view record block the decode writes and the merge reads
+        # (both on the decode stream, so one block serves every batch) and per input slot the device (y0, x0) of its views
+        self._tiling = None
+        self._views = 1
+        self._view_dets: Optional[torch.Tensor] = None
+        self._view_counts: Optional[torch.Tensor] = None
+        self._slot_yx: Optional[List[torch.Tensor]] = None
+
+    @property
+    def images_per_batch(self) -> int:
+        """Images one ``submit_images`` takes: ``batch``, or ``batch // V`` with tiling."""
+        return self.batch // self._views
+
+    def enable_tiling(self, rows: int, cols: int, overlap: float = 0.2) -> None:
+        """From now on ``submit_images`` detects every image as V = 1 + rows * cols views: the whole image and rows x cols
+        overlapping tiles of it (``tiles.tile_windows``), each letterboxed and decoded as the crop submitted as an image of
+        its own would be.  A batch holds at most ``images_per_batch`` = batch // V images; their n * V views fill the input
+        slot image-major, and ``k2y_merge_views`` merges each image's records behind the decode: boxes moved into image
+        coordinates, ``index = view * nbox + index`` (``index // nbox`` tells the view), one more greedy NMS per class over
+        the union.  ``collect`` returns the merged records in the usual format; rendering, the all-gather (rank r's images
+        from row r * batch) and the flow control are unchanged.  Raises ``ValueError`` when V exceeds the batch or
+        V * max_per_class exceeds what one merge holds (``k2y_merge_views_max_records``)."""
+        rows, cols = int(rows), int(cols)
+        if rows < 1 or cols < 1:
+            raise ValueError(f"tiling {rows}x{cols}: at least one tile per axis")
+        if not 0 <= overlap < 1:
+            raise ValueError(f"tile overlap {overlap} is outside [0, 1)")
+        V = 1 + rows * cols
+        if V > self.batch:
+            raise ValueError(f"{V} views per image do not fit a batch of {self.batch}")
+        limit = int(lib.k2y_merge_views_max_records())
+        if V * self.gather.K > limit:
+            raise ValueError(f"{V} views x {self.gather.K} records per class exceed the {limit} records one merge holds")
+        dev = torch.device("cuda", self.device_index)
+        self._tiling, self._views = (rows, cols, overlap), V
+        self._nbox = sum(h * w for h, w in self.detector.out_hw) * self.detector.A      # boxes of one network input
+        self._view_dets = torch.zeros((self.batch, self.gather.C, self.gather.K, DET_WORDS), dtype=torch.int32, device=dev)
+        self._view_counts = torch.zeros((self.batch, self.gather.C), dtype=torch.int32, device=dev)
+        self._slot_yx = [torch.zeros((self.batch, 2), dtype=torch.float32, device=dev) for _ in range(SLOTS)]
 
     def set_image_shapes(self, image_hw) -> None:
         """Original (pre-letterbox) image sizes, [batch, 2] (h, w); defaults to the network input size."""
@@ -94,10 +141,11 @@ class DetectionPipeline:
         self._img_hw.copy_(torch.from_numpy(np.array(arr, dtype=np.float32, order="C", copy=True)))
 
     # -- device-resident step ---------------------------------------------------------------------------------------
-    def _step(self, n: int, image_hw: Optional[torch.Tensor] = None) -> int:
+    def _step(self, n: int, image_hw: Optional[torch.Tensor] = None, view_yx: Optional[torch.Tensor] = None) -> int:
         """Network on the current stream into head set s, decode/NMS on the decode stream into gather slot s, then
         (world > 1) the all-gather on the side stream.  `image_hw`: device [n, 2] original sizes (default: the shared
-        ``set_image_shapes`` tensor).  Returns s."""
+        ``set_image_shapes`` tensor).  With `view_yx` (device [n, 2] origins) the n inputs are the views of n // V images: the
+        decode writes the per-view block and the merge writes the gather slot.  Returns s."""
         s = self._steps % SLOTS
         self._steps += 1
         compute = torch.cuda.current_stream(self.device_index)
@@ -112,7 +160,14 @@ class DetectionPipeline:
         det.wait_event(self._heads_ready[s])
         det.wait_event(self._slot_free[s])          # whoever still reads this gather slot (all-gather / D2H two steps ago)
         dets, counts = self.gather.local(s)
-        self.detector.run(heads, self._img_hw[:n] if image_hw is None else image_hw, dets_out=dets, counts_out=counts, stream=det)
+        if view_yx is None:
+            self.detector.run(heads, self._img_hw[:n] if image_hw is None else image_hw, dets_out=dets, counts_out=counts, stream=det)
+        else:
+            self.detector.run(heads, image_hw, dets_out=self._view_dets, counts_out=self._view_counts, stream=det)
+            check(lib.k2y_merge_views(self._view_dets.data_ptr(), self._view_counts.data_ptr(), view_yx.data_ptr(), n // self._views,
+                                      self.batch, self._views, self._nbox, self.gather.C, self.gather.K, self.detector.cfg.iou_thresh,
+                                      dets.data_ptr(), counts.data_ptr(), dets.stride(0), counts.stride(0),
+                                      ctypes.c_void_p(det.cuda_stream)))
         self._det_done[s].record(det)
         if self.world > 1:
             self._side.wait_event(self._det_done[s])
@@ -218,7 +273,7 @@ class DetectionPipeline:
         self._render_free[slot].record(det)
 
     def submit_images(self, images: Sequence[np.ndarray]) -> int:
-        """Streaming form for raw images: `images` is a list of n <= batch host numpy uint8 [h, w, 3] RGB arrays of any sizes, or
+        """Streaming form for raw images: `images` is a list of n <= ``images_per_batch`` host numpy uint8 [h, w, 3] RGB arrays of any sizes, or
         image files (``bytes``, ``bytearray``, ``memoryview``): baseline JPEGs are decoded on the GPU on the copy stream in front
         of the letterbox, other files on the host inside this call (``preprocess.BatchLayout``).
         They are packed into the input slot's pinned staging buffer, copied to the GPU in one H2D copy and letterboxed in one
@@ -228,7 +283,9 @@ class DetectionPipeline:
         rank, rank r's images from row r * batch), or raises ``K2YError`` naming the JPEGs whose entropy-coded data was corrupt
         (their records would come from undefined pixels).  Same flow control as ``submit``.  Bad input raises ``ValueError``
         before anything is enqueued."""
-        layout = BatchLayout(images, self.in_hw)
+        if self._tiling is not None and isinstance(images, (list, tuple)) and len(images) > self.images_per_batch:
+            raise ValueError(f"{len(images)} images of {self._views} views do not fit a batch of {self.batch}")
+        layout = BatchLayout(images, self.in_hw, self._tiling)
         n = len(layout)
         if n > self.batch:
             raise ValueError(f"{n} images do not fit a batch of {self.batch}")
@@ -250,25 +307,29 @@ class DetectionPipeline:
         self._copy_stream.wait_event(self._render_free[slot])    # the last render read this slot's originals
         s = self._steps % SLOTS                  # the gather slot this batch's step will use
         with torch.cuda.device(dev):
-            letterbox_packed(layout, images, self._staging[slot], buf, self._slot_hw[slot])
+            letterbox_packed(layout, images, self._staging[slot], buf, self._slot_hw[slot],
+                             self._slot_yx[slot] if self._tiling is not None else None)
             self._jpeg_idx[s] = [i for i, _ in layout.jpeg]
             if layout.jpeg:             # the status words travel to the host before the network starts on this slot
                 with torch.cuda.stream(self._copy_stream):
                     self._jpeg_status[s][:len(layout.jpeg)].copy_(self._staging[slot].status[:len(layout.jpeg)], non_blocking=True)
         self._h2d_done[slot].record(self._copy_stream)
-        t = self._run_slot(slot, buf, n, self._slot_hw[slot][:n], n if self.world == 1 else None)
+        nv = n * layout.views
+        t = self._run_slot(slot, buf, nv, self._slot_hw[slot][:nv], n if self.world == 1 else None,
+                           self._slot_yx[slot][:nv] if self._tiling is not None else None)
         self._rendered_slot[t] = self._render is not None
         if self._render is not None:
             with torch.cuda.device(dev):
                 self._render_slot(slot, t, layout)
         return t
 
-    def _run_slot(self, slot: int, buf: torch.Tensor, n: int, image_hw: Optional[torch.Tensor], rows: Optional[int]) -> int:
+    def _run_slot(self, slot: int, buf: torch.Tensor, n: int, image_hw: Optional[torch.Tensor], rows: Optional[int],
+                  view_yx: Optional[torch.Tensor] = None) -> int:
         """Network + decode (+ all-gather) of input slot `slot` once its H2D is done, then the D2H of the records."""
         compute = torch.cuda.current_stream(self.device_index)
         compute.wait_event(self._h2d_done[slot])
         self.engine.bind_input(buf)
-        s = self._step(n, image_hw)
+        s = self._step(n, image_hw, view_yx)
         self._in_free[slot].record(compute)
         self._hw_free[slot].record(self._det_stream)
         self._rows[s] = rows
@@ -405,6 +466,15 @@ class LanedPipeline:
         """``DetectionPipeline.enable_rendering`` on every lane."""
         for ln in self.lanes:
             ln.enable_rendering(quality, font_path, colormap)
+
+    def enable_tiling(self, rows: int, cols: int, overlap: float = 0.2) -> None:
+        """``DetectionPipeline.enable_tiling`` on every lane."""
+        for ln in self.lanes:
+            ln.enable_tiling(rows, cols, overlap)
+
+    @property
+    def images_per_batch(self) -> int:
+        return self.lanes[0].images_per_batch
 
     def rendered(self, ticket) -> List[bytes]:
         k, t = ticket

@@ -27,6 +27,7 @@ import torch
 
 from ._lib import JpegInfo, K2YError, check, lib
 from .helper import read_image
+from .tiles import tile_windows
 
 
 def letterbox_params(img_hw, in_hw):
@@ -142,9 +143,14 @@ class BatchLayout:
     Entries that are image files are resolved here: ``jpeg`` lists (index, file bytes) of the JPEGs the GPU decodes
     (``gpu_decodable``), whose size comes from their header; every other file is decoded on the host now, and ``arrays[i]``
     holds the host pixels of entry i (None for a GPU JPEG).  ``jpeg_plan`` is where the JPEGs' bytes and their descriptor blob
-    go in the staging buffer, behind the packed pixels (``_jpeg_layout``)."""
+    go in the staging buffer, behind the packed pixels (``_jpeg_layout``).
 
-    def __init__(self, images: Sequence, in_hw):
+    With `tiling` = (rows, cols, overlap) every image is letterboxed as V = 1 + rows * cols views (``tiles.tile_windows``:
+    the whole image, then its tiles): ``views`` = V, ``windows`` int32 [n * V, 4] (y0, x0, th, tw) and ``view_matrices``
+    float64 [n * V, 6] (each window's own ``letterbox_params`` matrix), image-major.  Everything above stays per image: staging,
+    the JPEG decode and the renderer see the originals."""
+
+    def __init__(self, images: Sequence, in_hw, tiling=None):
         _check_images(images)
         n = len(images)
         self.in_hw = (int(in_hw[0]), int(in_hw[1]))
@@ -169,6 +175,16 @@ class BatchLayout:
         self.offsets = np.concatenate([[0], np.cumsum(padded)[:-1]]).astype(np.int64)
         self.nbytes = int(padded.sum())
         self.matrices = np.array([letterbox_params((int(h[0]), int(h[1])), self.in_hw)[2][:2].reshape(-1) for h in self.hw], dtype=np.float64)
+        self.views, self.windows, self.view_matrices = 1, None, None
+        if tiling is not None:
+            rows, cols, overlap = tiling
+            try:
+                self.windows = np.concatenate([tile_windows(int(h), int(w), rows, cols, overlap) for h, w in self.hw])
+            except ValueError as e:
+                raise ValueError(f"tiling {rows}x{cols}: {e}") from e
+            self.views = len(self.windows) // n
+            self.view_matrices = np.array([letterbox_params((int(t[2]), int(t[3])), self.in_hw)[2][:2].reshape(-1) for t in self.windows],
+                                          dtype=np.float64)
         self.jpeg_plan = None
         if self.jpeg:
             self.jpeg_dst = self.offsets[[i for i, _ in self.jpeg]].astype(np.int64)
@@ -295,13 +311,15 @@ def _jpeg_layout(files: Sequence[np.ndarray], dst_offsets: np.ndarray, base: int
 
 
 def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, out: torch.Tensor,
-                     image_hw_out: Optional[torch.Tensor]) -> None:
+                     image_hw_out: Optional[torch.Tensor], view_yx_out: Optional[torch.Tensor] = None) -> None:
     """Packs `images` into ``staging.host``, copies them to the device and letterboxes them into ``out[:n]`` (and their sizes
     into ``image_hw_out[:n]``), all on ``staging.stream``.  GPU-decodable JPEGs travel compressed behind the packed pixels and
     are decoded into their place first (``stage_jpegs``).  The host buffer is reused by the next call: wait for this copy
-    before packing into it again."""
+    before packing into it again.  A layout with tiling letterboxes its n * V views instead (``k2y_letterbox_u8_views``),
+    image-major: ``out[:n * V]``, each view's (th, tw) into ``image_hw_out[:n * V]`` and its (y0, x0) into
+    ``view_yx_out[:n * V]`` (float32 [N, 2])."""
     n = len(layout)
-    staging.reserve(layout.jpeg_plan[3] if layout.jpeg else layout.nbytes, n)
+    staging.reserve(layout.jpeg_plan[3] if layout.jpeg else layout.nbytes, n * layout.views)
     layout.pack(images, staging.host.numpy())
     in_h, in_w = layout.in_hw
     st = staging.stream
@@ -311,6 +329,18 @@ def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, ou
         if layout.jpeg:
             stage_jpegs([f for _, f in layout.jpeg], layout.jpeg_dst, staging, layout.jpeg_plan, staging.dev)
         offs = layout.offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong))
+        if layout.windows is not None:
+            V = layout.views
+            offsets = np.repeat(layout.offsets, V)
+            hw = np.ascontiguousarray(np.repeat(layout.hw, V, axis=0))
+            check(lib.k2y_letterbox_u8_views(staging.dev.data_ptr(), n * V, offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
+                                             hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                                             layout.windows.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                                             layout.view_matrices.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), out.data_ptr(), in_h,
+                                             in_w, image_hw_out.data_ptr() if image_hw_out is not None else None,
+                                             view_yx_out.data_ptr() if view_yx_out is not None else None, staging.minmax.data_ptr(),
+                                             ctypes.c_void_p(st.cuda_stream)))
+            return
         hw = layout.hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int))
         mats = layout.matrices.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
         check(lib.k2y_letterbox_u8_batch(staging.dev.data_ptr(), n, offs, hw, mats, out.data_ptr(), in_h, in_w,

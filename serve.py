@@ -18,6 +18,10 @@ gives, so the lines do not depend on which route a file took.
 With --draw DIR every rank also writes DIR/<stem>.jpg for its own files: the records are drawn onto the original images where
 they already lie on the GPU and encoded there (DetectionPipeline.enable_rendering), with the bytes PIL's draw_detections + save
 give; only the compressed files come back.  Duplicate stems are refused before any work starts.
+
+With --tiles ROWS COLS every image is detected on ROWS x COLS overlapping tiles as well as whole (--tile_overlap, default 0.2;
+DetectionPipeline.enable_tiling): a batch then holds batch // (1 + ROWS * COLS) images, the views' records are merged on the GPU
+and the lines keep their shape, with "index" // (boxes per network input) telling the view a detection came from.
 """
 import argparse
 import io
@@ -68,6 +72,8 @@ def open_pipeline(args, max_per_class=30):
     pipe = DetectionPipeline(args.model_def, tuple(args.image_size), anchors, args.class_num, args.depth_multiplier, args.batch,
                              args.obj_thresh, args.iou_thresh, max_per_class, device=local, world=world, rank=rank)
     pipe.engine.load_weights(args.ckpt)
+    if getattr(args, "tiles", None):
+        pipe.enable_tiling(args.tiles[0], args.tiles[1], args.tile_overlap)
     return pipe, world, rank
 
 
@@ -84,8 +90,9 @@ def draw_paths(files, out_dir):
 
 
 def detect_files(pipe, files, decode_threads=4, load=None, rendered=False):
-    """Yields ``(paths, dets, counts)`` per global batch of world * batch files, in file order: the batch's gathered record
-    blocks as ``collect`` returns them (pinned host views, valid until the generator resumes twice).  Every rank reads ITS
+    """Yields ``(paths, dets, counts)`` per global batch of world * images_per_batch files, in file order: the batch's gathered
+    record blocks as ``collect`` returns them (pinned host views, valid until the generator resumes twice; with tiling on
+    several ranks, copies of the rows that hold images, so that row j is file j here too).  Every rank reads ITS
     files of the next batch in a pool of `decode_threads` threads while the GPU works, and two batches are in flight.
     Every rank runs the network on a full batch (the tensor-core plans depend on the batch size, so the records of a short
     final batch match a full one's bit for bit) and takes part in every all-gather: its share of a short batch is padded
@@ -93,7 +100,10 @@ def detect_files(pipe, files, decode_threads=4, load=None, rendered=False):
     (default: load_image).  With `rendered` (the pipeline's rendering enabled) each tuple also carries this rank's drawn
     JPEG files of the batch, its padding images' files left out."""
     load = load or load_image
-    B, G, rank = pipe.batch, pipe.world * pipe.batch, pipe.rank
+    B, G, rank = pipe.images_per_batch, pipe.world * pipe.images_per_batch, pipe.rank
+    rows = None
+    if pipe.world > 1 and B != pipe.batch:      # rank r's B images lie from row r * batch of the gathered block
+        rows = [r * pipe.batch + j for r in range(pipe.world) for j in range(B)]
     chunks = [files[g0:g0 + G] for g0 in range(0, len(files), G)]
     filler = np.full(pipe.in_hw + (3,), 128, np.uint8)
     with ThreadPoolExecutor(max(1, int(decode_threads))) as pool:
@@ -101,7 +111,8 @@ def detect_files(pipe, files, decode_threads=4, load=None, rendered=False):
             return [pool.submit(load, p) for p in chunk[rank * B:(rank + 1) * B]]
 
         def result(chunk, ticket, mine):
-            out = (chunk,) + tuple(pipe.collect(ticket))
+            dets, counts = pipe.collect(ticket)
+            out = (chunk, dets, counts) if rows is None else (chunk, dets[rows], counts[rows])
             return out + (pipe.rendered(ticket)[:mine],) if rendered else out
 
         pending = deque()
@@ -126,7 +137,7 @@ def serve(args, out_fh=None):
         os.makedirs(draw_dir, exist_ok=True)
         pipe.enable_rendering(quality=args.draw_quality)
     n_out = 0
-    B = pipe.batch
+    B = pipe.images_per_batch
     for g, item in enumerate(detect_files(pipe, files, getattr(args, "decode_threads", 4), load_image, rendered=bool(draw_dir))):
         chunk, dets, counts = item[:3]
         if draw_dir:        # this rank's files of the global batch
@@ -157,6 +168,10 @@ def add_model_args(ap):
     ap.add_argument("--class_num", type=int, default=20)
     ap.add_argument("--anchors", default="data/voc_anchor.npy")
     ap.add_argument("--batch", type=int, default=32, help="images per GPU per step")
+    ap.add_argument("--tiles", type=int, nargs=2, default=None, metavar=("ROWS", "COLS"),
+                    help="also detect on ROWS x COLS overlapping tiles of every image and merge the views' records on the GPU; "
+                         "a batch then holds batch // (1 + ROWS * COLS) images")
+    ap.add_argument("--tile_overlap", type=float, default=0.2, help="fraction of a tile shared with its neighbour (with --tiles)")
     ap.add_argument("--decode_threads", type=int, default=4, help="host threads reading the next batch's files and decoding those the GPU does not (PIL)")
 
 
