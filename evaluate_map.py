@@ -23,15 +23,19 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 from serve import add_model_args, detect_files, load_image, open_pipeline  # noqa: E402
 from k210_yolo_framework_b200.evaluate import DetectionAP, load_voc_annotations  # noqa: E402
-from k210_yolo_framework_b200.preprocess import inspect_jpeg  # noqa: E402
+from k210_yolo_framework_b200.preprocess import inspect_jpeg, inspect_png  # noqa: E402
 
 COCO_IOU = [round(0.5 + 0.05 * i, 2) for i in range(10)]
 
 
-def load_checked(path, hw):
-    """load_image, refusing a file whose size differs from its annotation row's (the boxes would land elsewhere)."""
-    img = load_image(path)
-    got = tuple(inspect_jpeg(img)[:2]) if isinstance(img, (bytes, bytearray, memoryview)) else tuple(img.shape[:2])
+def load_checked(path, hw, gpu_png=False):
+    """load_image, refusing a file whose size differs from its annotation row's (the boxes would land elsewhere).  The size of
+    a file kept compressed comes from its header (JPEG, or PNG with `gpu_png`)."""
+    img = load_image(path, gpu_png=True) if gpu_png else load_image(path)
+    if isinstance(img, (bytes, bytearray, memoryview)):
+        got = tuple((inspect_png if bytes(img[:4]) == b"\x89PNG" else inspect_jpeg)(img)[:2])
+    else:
+        got = tuple(img.shape[:2])
     if got != tuple(hw):
         raise ValueError(f"{path}: decoded size {got[0]}x{got[1]} differs from its annotation's {hw[0]}x{hw[1]}")
     return img
@@ -44,7 +48,7 @@ def evaluate(args):
     pipe, world, rank = open_pipeline(args, args.max_per_class)
     ev = DetectionAP(args.class_num, args.max_per_class, args.eval_iou, device=pipe.device_index) if rank == 0 else None
     idx = list(range(len(paths)))
-    for chunk, dets, counts in detect_files(pipe, idx, args.decode_threads, lambda i: load_checked(paths[i], hw[i])):
+    for chunk, dets, counts in detect_files(pipe, idx, args.decode_threads, lambda i: load_checked(paths[i], hw[i], getattr(args, "gpu_png", False))):
         if ev is not None:
             ev.update(dets[:len(chunk)], counts[:len(chunk)], [(labels[i], hw[i]) for i in chunk])
     if world > 1:

@@ -331,6 +331,47 @@ int k2y_jpeg_decode(const void *blob_host, const void *blob_dev, const unsigned 
                     void *workspace_dev, size_t workspace_bytes, int32_t *status_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * PNG decode on the device, in front of k2y_letterbox_u8_batch: the RGB pixels Helper._read_img (PIL) gives for
+ * non-interlaced PNGs of every colour type and depth except 16-bit greyscale (palette lookup with (0, 0, 0) past the PLTE
+ * entries, 1/2/4-bit grey scaled to 0..255, grey replicated, the high byte of 16-bit samples, alpha dropped).
+ * GPU-decodable: such a file of at most 65535 rows and columns and 2^31 - 1 filtered bytes whose chunks before the first IDAT have correct CRCs, with a
+ * PLTE where one is needed, no unknown critical or acTL chunk, one run of IDAT chunks, an IEND and a zlib header with CM = 8,
+ * CINFO <= 7 and no preset dictionary.  Every other file is reported with its reason and is left to the host.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+    int32_t height, width;
+    int32_t color_type, bit_depth, interlace;   /* IHDR */
+    int32_t idat_chunks;
+    int64_t stream_bytes;           /* zlib stream: the payload of every IDAT */
+    int32_t gpu_decodable;          /* 1: k2y_png_plan accepts the file */
+    char reason[64];                /* why not, when gpu_decodable == 0 */
+} k2y_png_info;
+/* Host only: walks the chunks.  K2Y_ERR_INVALID for a file without the PNG signature and a sound IHDR; K2Y_OK with
+ * info->gpu_decodable and info->reason otherwise. */
+int k2y_png_inspect(const unsigned char *data, size_t size, k2y_png_info *info);
+/* Host only: the descriptor blob of a batch of n GPU-decodable files (IDAT ranges, geometry, palette, workspace offsets), with
+ * the arguments of k2y_jpeg_plan.  A file that is not GPU-decodable is K2Y_ERR_INVALID. */
+int k2y_png_plan(const unsigned char *const *files, const size_t *sizes, int n, const long long *src_offsets,
+                 const long long *dst_offsets, void *blob, size_t blob_capacity, size_t *blob_bytes);
+/* Device workspace k2y_png_decode needs for the batch a blob describes (read from the host copy of the blob). */
+int k2y_png_workspace_bytes(const void *blob_host, size_t *bytes);
+/* Decodes the batch, asynchronous on `stream`, with the arguments of k2y_jpeg_decode.  Six kernels, one launch each whatever the
+ * image count: gather the IDAT payloads; find, in every 64 KiB chunk of compressed data after the first, the first bit where a
+ * block header parses strictly; decode every chunk from there (one warp each) into bytes and references to the 32 KiB before
+ * it, until it stands on a later chunk's candidate at a block boundary; follow the chain of those links from the stream's start
+ * and resolve the references chunk by chunk (one CTA per image), checking the Adler-32; inflate serially the images whose chain
+ * does not end exactly at the image's size with a good Adler-32 (damaged or unusual streams, with zlib's rules as PIL drives
+ * it); unfilter + colour (one CTA per image).  A stream without findable block headers (fixed Huffman only, one huge block) is
+ * decoded by its first chunk alone.  status_dev: int32 [n][4] per image: error bits (1 invalid block header, 2 invalid code, 4
+ * distance too far back, 8 image data ends early, 16 Adler-32 mismatch, 32 filter type above 4: the image's pixels are then
+ * undefined, the other images' are exact), chunks, chunks after the first whose speculative start was confirmed, and bytes the
+ * longest single decoder inflated (all of them when the image fell back to the serial decoder).  Where zlib, as PIL drives it,
+ * accepts a stream, so does the decoder, and rows a stream that ends cleanly early does not fill decode from zero bytes.
+ * Corrupt data never makes a kernel read outside its image's bytes or write outside its output. */
+int k2y_png_decode(const void *blob_host, const void *blob_dev, const unsigned char *src_dev, unsigned char *dst_dev,
+                   void *workspace_dev, size_t workspace_bytes, int32_t *status_dev, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Baseline JPEG encoding, byte-identical to PIL's Image.fromarray(rgb).save(f, "JPEG", quality=q) with libjpeg-turbo 3.1:
  * JFIF APP0, two DQT, SOF0 4:2:0, the four standard Huffman tables, one interleaved scan, EOI.
  *   k2y_jpeg_encode_plan             host only: the descriptor blob of n images, hw_host int32 [n][2] (1..65500 each:

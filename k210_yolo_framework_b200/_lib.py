@@ -55,6 +55,11 @@ class JpegInfo(ctypes.Structure):
                 ("entropy_offset", c_int32), ("reason", ctypes.c_char * 64)]
 
 
+class PngInfo(ctypes.Structure):
+    _fields_ = [("height", c_int32), ("width", c_int32), ("color_type", c_int32), ("bit_depth", c_int32), ("interlace", c_int32),
+                ("idat_chunks", c_int32), ("stream_bytes", c_int64), ("gpu_decodable", c_int32), ("reason", ctypes.c_char * 64)]
+
+
 # Every symbol include/k210_yolo_b200.h declares (tests/test_abi.py checks the two lists agree).
 _SIGNATURES = {
     "k2y_last_error": (c_char_p, []),
@@ -122,6 +127,11 @@ _SIGNATURES = {
                               c_void_p, c_size_t, POINTER(c_size_t)]),
     "k2y_jpeg_workspace_bytes": (c_int, [c_void_p, POINTER(c_size_t)]),
     "k2y_jpeg_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "k2y_png_inspect": (c_int, [c_void_p, c_size_t, POINTER(PngInfo)]),
+    "k2y_png_plan": (c_int, [POINTER(c_void_p), POINTER(c_size_t), c_int, POINTER(ctypes.c_longlong), POINTER(ctypes.c_longlong),
+                             c_void_p, c_size_t, POINTER(c_size_t)]),
+    "k2y_png_workspace_bytes": (c_int, [c_void_p, POINTER(c_size_t)]),
+    "k2y_png_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
     "k2y_jpeg_encode_plan": (c_int, [c_int, POINTER(c_int), POINTER(ctypes.c_longlong), c_int, c_void_p, c_size_t, POINTER(c_size_t)]),
     "k2y_jpeg_encode_header": (c_int, [c_int, c_int, c_int, c_void_p, c_size_t, POINTER(c_size_t)]),
     "k2y_jpeg_encode_workspace_bytes": (c_int, [c_void_p, POINTER(c_size_t), POINTER(c_size_t)]),

@@ -29,6 +29,9 @@ slot waits for the render before it overwrites the originals.
 n <= batch // V images is letterboxed as n * V views, the network and the decode run on those, and one more per-class NMS
 (``k2y_merge_views``, on the decode stream) merges each image's views into rows [0, n) of the gather slot, in image
 coordinates and in the usual block format, so everything behind it is unchanged.
+
+``enable_png_decode`` makes ``submit_images`` decode the PNG files the GPU takes there too (``preprocess.png_gpu_decodable``),
+in the same staging range and H2D copy as the batch's JPEGs; their status words travel beside the JPEGs'.
 """
 from __future__ import annotations
 
@@ -43,7 +46,7 @@ from . import yolonet
 from ._lib import check, lib
 from .detect import DET_WORDS, KerasDetector
 from .dist import DetectionGather
-from .preprocess import BatchLayout, Staging, check_jpeg_status, letterbox_packed
+from .preprocess import BatchLayout, Staging, check_jpeg_status, check_png_status, letterbox_packed
 
 SLOTS = 2
 
@@ -88,6 +91,10 @@ class DetectionPipeline:
         # GPU-decoded JPEGs of the batch behind each gather slot: their batch positions and (pinned) status words
         self._jpeg_idx: List[list] = [[] for _ in range(SLOTS)]
         self._jpeg_status = [torch.zeros((batch, 4), dtype=torch.int32).pin_memory() for _ in range(SLOTS)]
+        # enable_png_decode: the same for the batch's GPU-decoded PNGs
+        self._gpu_png = False
+        self._png_idx: List[list] = [[] for _ in range(SLOTS)]
+        self._png_status = [torch.zeros((batch, 4), dtype=torch.int32).pin_memory() for _ in range(SLOTS)]
         self._steps = 0
         self._submitted = 0
         # enable_rendering: label atlas, colour table, quality, one encoder per gather slot (its files live until rendered())
@@ -134,6 +141,12 @@ class DetectionPipeline:
         self._view_dets = torch.zeros((self.batch, self.gather.C, self.gather.K, DET_WORDS), dtype=torch.int32, device=dev)
         self._view_counts = torch.zeros((self.batch, self.gather.C), dtype=torch.int32, device=dev)
         self._slot_yx = [torch.zeros((self.batch, 2), dtype=torch.float32, device=dev) for _ in range(SLOTS)]
+
+    def enable_png_decode(self) -> None:
+        """From now on ``submit_images`` decodes the PNG files the GPU takes (``preprocess.png_gpu_decodable``: non-interlaced,
+        not 16-bit grey, sound chunks) on the GPU, with the pixels PIL gives, instead of on the host; ``collect`` raises
+        ``K2YError`` naming a PNG whose zlib stream or row filters PIL refuses.  Other PNGs keep the host route."""
+        self._gpu_png = True
 
     def set_image_shapes(self, image_hw) -> None:
         """Original (pre-letterbox) image sizes, [batch, 2] (h, w); defaults to the network input size."""
@@ -225,6 +238,7 @@ class DetectionPipeline:
             buf[:n].copy_(x_host, non_blocking=True)
             self._h2d_done[slot].record(self._copy_stream)
         self._jpeg_idx[self._steps % SLOTS] = []
+        self._png_idx[self._steps % SLOTS] = []
         t = self._run_slot(slot, buf, n, None, None)
         self._rendered_slot[t] = False
         return t
@@ -285,7 +299,7 @@ class DetectionPipeline:
         before anything is enqueued."""
         if self._tiling is not None and isinstance(images, (list, tuple)) and len(images) > self.images_per_batch:
             raise ValueError(f"{len(images)} images of {self._views} views do not fit a batch of {self.batch}")
-        layout = BatchLayout(images, self.in_hw, self._tiling)
+        layout = BatchLayout(images, self.in_hw, self._tiling, gpu_png=self._gpu_png)
         n = len(layout)
         if n > self.batch:
             raise ValueError(f"{n} images do not fit a batch of {self.batch}")
@@ -313,6 +327,10 @@ class DetectionPipeline:
             if layout.jpeg:             # the status words travel to the host before the network starts on this slot
                 with torch.cuda.stream(self._copy_stream):
                     self._jpeg_status[s][:len(layout.jpeg)].copy_(self._staging[slot].status[:len(layout.jpeg)], non_blocking=True)
+            self._png_idx[s] = [i for i, _ in layout.png]
+            if layout.png:
+                with torch.cuda.stream(self._copy_stream):
+                    self._png_status[s][:len(layout.png)].copy_(self._staging[slot].png_status[:len(layout.png)], non_blocking=True)
         self._h2d_done[slot].record(self._copy_stream)
         nv = n * layout.views
         t = self._run_slot(slot, buf, nv, self._slot_hw[slot][:nv], n if self.world == 1 else None,
@@ -351,6 +369,9 @@ class DetectionPipeline:
         if self._jpeg_idx[ticket]:
             idx = self._jpeg_idx[ticket]
             check_jpeg_status(self._jpeg_status[ticket][:len(idx)].numpy(), idx)
+        if self._png_idx[ticket]:
+            idx = self._png_idx[ticket]
+            check_png_status(self._png_status[ticket][:len(idx)].numpy(), idx)
         dets, counts = DetectionGather.split(self._host[ticket], self.gather.C, self.gather.K, DET_WORDS)
         n = self._rows[ticket]
         return (dets, counts) if n is None else (dets[:n], counts[:n])
@@ -466,6 +487,11 @@ class LanedPipeline:
         """``DetectionPipeline.enable_rendering`` on every lane."""
         for ln in self.lanes:
             ln.enable_rendering(quality, font_path, colormap)
+
+    def enable_png_decode(self) -> None:
+        """``DetectionPipeline.enable_png_decode`` on every lane."""
+        for ln in self.lanes:
+            ln.enable_png_decode()
 
     def enable_tiling(self, rows: int, cols: int, overlap: float = 0.2) -> None:
         """``DetectionPipeline.enable_tiling`` on every lane."""

@@ -16,6 +16,11 @@ pinned buffer, one H2D copy moves them, and ``k2y_jpeg_decode`` writes their RGB
 inside the call, as ``Helper._read_img`` does (the slow path); so is a JPEG that does not end with its EOI marker, so that a
 truncated file raises as it does with PIL.  Corrupt entropy data in a complete file sets the image's status word, which
 ``letterbox_batch_device`` and ``DetectionPipeline.collect`` turn into a ``K2YError``.  ``decode_jpeg_batch`` returns the decoded pixels themselves.
+
+PNG files take the same route when the caller opts in (``BatchLayout(gpu_png=True)``, ``letterbox_batch_device(gpu_png=True)``,
+``DetectionPipeline.enable_png_decode``): the PNGs ``inspect_png`` finds GPU-decodable travel compressed in the same staging
+range and H2D copy as the JPEGs, and ``k2y_png_decode`` writes the pixels PIL gives at their offsets.  A damaged zlib stream
+that PIL refuses sets the image's status word (``check_png_status``).  ``decode_png_batch`` returns the decoded pixels.
 """
 from __future__ import annotations
 
@@ -25,7 +30,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from ._lib import JpegInfo, K2YError, check, lib
+from ._lib import JpegInfo, K2YError, PngInfo, check, lib
 from .helper import read_image
 from .tiles import tile_windows
 
@@ -111,6 +116,54 @@ def gpu_decodable(data) -> bool:
     return _gpu_route(_file_bytes(data)) is not None
 
 
+def _png_info(buf: np.ndarray) -> Optional[PngInfo]:
+    """The header of a PNG file, or None when `buf` is not one the parser accepts (other formats, no sound IHDR)."""
+    if buf.size < 8 or bytes(buf[:8]) != b"\x89PNG\r\n\x1a\n":
+        return None
+    info = PngInfo()
+    if lib.k2y_png_inspect(buf.ctypes.data, buf.size, ctypes.byref(info)) != 0:
+        return None
+    return info
+
+
+def _pil_pixel_limit() -> Optional[int]:
+    from PIL import Image
+    return Image.MAX_IMAGE_PIXELS
+
+
+def inspect_png(data):
+    """Header of a PNG file held in memory (``bytes``, ``bytearray`` or ``memoryview``), read on the host:
+    ``(h, w, gpu_decodable, reason)``; `reason` says why a valid file is not for the GPU decoder ("" when it is).  A file over
+    PIL's decompression-bomb limit (``Image.MAX_IMAGE_PIXELS``) is left to PIL, which warns or raises.  Raises ``K2YError``
+    for a file that is not a PNG or has no sound IHDR chunk."""
+    if not isinstance(data, ENCODED):
+        raise ValueError(f"expected the bytes of a file, got {type(data).__name__}")
+    buf = _file_bytes(data)
+    info = PngInfo()
+    check(lib.k2y_png_inspect(buf.ctypes.data, buf.size, ctypes.byref(info)))
+    h, w, ok, why = int(info.height), int(info.width), bool(info.gpu_decodable), info.reason.decode()
+    limit = _pil_pixel_limit()
+    if ok and limit is not None and h * w > limit:
+        ok, why = False, f"over PIL's decompression-bomb limit of {limit} pixels"
+    return h, w, ok, why
+
+
+def _png_route(buf: np.ndarray) -> Optional[PngInfo]:
+    """The header of `buf` when the batch routes send it to the GPU PNG decoder (with PNG decoding enabled), else None."""
+    info = _png_info(buf)
+    if info is None or not info.gpu_decodable:
+        return None
+    limit = _pil_pixel_limit()
+    if limit is not None and int(info.height) * int(info.width) > limit:
+        return None
+    return info
+
+
+def png_gpu_decodable(data) -> bool:
+    """True when `data` (the bytes of a file) goes to the GPU PNG decoder in ``submit_images`` with PNG decoding enabled."""
+    return _png_route(_file_bytes(data)) is not None
+
+
 def _check_images(images) -> None:
     if not isinstance(images, (list, tuple)) or len(images) == 0:
         raise ValueError("expected a non-empty list of host uint8 [h, w, 3] arrays or image files")
@@ -143,26 +196,32 @@ class BatchLayout:
     Entries that are image files are resolved here: ``jpeg`` lists (index, file bytes) of the JPEGs the GPU decodes
     (``gpu_decodable``), whose size comes from their header; every other file is decoded on the host now, and ``arrays[i]``
     holds the host pixels of entry i (None for a GPU JPEG).  ``jpeg_plan`` is where the JPEGs' bytes and their descriptor blob
-    go in the staging buffer, behind the packed pixels (``_jpeg_layout``).
+    go in the staging buffer, behind the packed pixels (``_jpeg_layout``).  With `gpu_png`, ``png`` lists (index, file bytes) of
+    the PNGs the GPU decodes (``png_gpu_decodable``) in the same way, and ``png_plan`` places them and their blob behind the
+    JPEGs' range, so that one H2D copy moves both (``staged_end`` is the end of everything the staging buffer holds).
 
     With `tiling` = (rows, cols, overlap) every image is letterboxed as V = 1 + rows * cols views (``tiles.tile_windows``:
     the whole image, then its tiles): ``views`` = V, ``windows`` int32 [n * V, 4] (y0, x0, th, tw) and ``view_matrices``
     float64 [n * V, 6] (each window's own ``letterbox_params`` matrix), image-major.  Everything above stays per image: staging,
     the JPEG decode and the renderer see the originals."""
 
-    def __init__(self, images: Sequence, in_hw, tiling=None):
+    def __init__(self, images: Sequence, in_hw, tiling=None, gpu_png: bool = False):
         _check_images(images)
         n = len(images)
         self.in_hw = (int(in_hw[0]), int(in_hw[1]))
         self.arrays: List[Optional[np.ndarray]] = []
         self.jpeg = []
+        self.png = []
         shapes = []
         for i, im in enumerate(images):
             if isinstance(im, ENCODED):
                 buf = _file_bytes(im)
                 info = _gpu_route(buf)
+                to = self.jpeg
+                if info is None and gpu_png:
+                    info, to = _png_route(buf), self.png
                 if info is not None:
-                    self.jpeg.append((i, buf))
+                    to.append((i, buf))
                     self.arrays.append(None)
                     shapes.append((info.height, info.width))
                     continue
@@ -186,9 +245,17 @@ class BatchLayout:
             self.view_matrices = np.array([letterbox_params((int(t[2]), int(t[3])), self.in_hw)[2][:2].reshape(-1) for t in self.windows],
                                           dtype=np.float64)
         self.jpeg_plan = None
+        self.png_plan = None
+        self.staged_end = self.nbytes
         if self.jpeg:
             self.jpeg_dst = self.offsets[[i for i, _ in self.jpeg]].astype(np.int64)
             self.jpeg_plan = _jpeg_layout([f for _, f in self.jpeg], self.jpeg_dst, (self.nbytes + ALIGN - 1) // ALIGN * ALIGN)
+            self.staged_end = self.jpeg_plan[3]
+        if self.png:
+            self.png_dst = self.offsets[[i for i, _ in self.png]].astype(np.int64)
+            self.png_plan = _jpeg_layout([f for _, f in self.png], self.png_dst, (self.staged_end + ALIGN - 1) // ALIGN * ALIGN,
+                                         _png_plan)
+            self.staged_end = self.png_plan[3]
 
     def __len__(self) -> int:
         return len(self.hw)
@@ -228,6 +295,8 @@ class Staging:
         self.minmax: Optional[torch.Tensor] = None
         self.workspace: Optional[torch.Tensor] = None   # k2y_jpeg_decode's
         self.status: Optional[torch.Tensor] = None      # int32 [n, 4] per decoded JPEG (k2y_jpeg_decode)
+        self.png_workspace: Optional[torch.Tensor] = None   # k2y_png_decode's
+        self.png_status: Optional[torch.Tensor] = None      # int32 [n, 4] per decoded PNG (k2y_png_decode)
 
     def reserve_jpeg(self, workspace_bytes: int, n: int) -> None:
         with torch.cuda.stream(self.stream):
@@ -237,6 +306,15 @@ class Staging:
             if self.status is None or self.status.shape[0] < n:
                 self.status = torch.empty((max(n, 2 * self.status.shape[0] if self.status is not None else 0), 4), dtype=torch.int32,
                                           device=self.device)
+
+    def reserve_png(self, workspace_bytes: int, n: int) -> None:
+        with torch.cuda.stream(self.stream):
+            if self.png_workspace is None or self.png_workspace.numel() < workspace_bytes:
+                cap = max(workspace_bytes, 2 * self.png_workspace.numel() if self.png_workspace is not None else 0)
+                self.png_workspace = torch.empty((cap,), dtype=torch.uint8, device=self.device)
+            if self.png_status is None or self.png_status.shape[0] < n:
+                self.png_status = torch.empty((max(n, 2 * self.png_status.shape[0] if self.png_status is not None else 0), 4),
+                                              dtype=torch.int32, device=self.device)
 
     def reserve(self, nbytes: int, n: int) -> None:
         if self.host is None or self.host.numel() < nbytes:
@@ -272,39 +350,77 @@ def _jpeg_plan(files: Sequence[np.ndarray], src_offsets: np.ndarray, dst_offsets
     return nbytes.value
 
 
+def _png_plan(files: Sequence[np.ndarray], src_offsets: np.ndarray, dst_offsets: np.ndarray, blob: Optional[np.ndarray]) -> int:
+    """k2y_png_plan: the blob's size (blob None), or the blob written into `blob` (16-byte aligned)."""
+    n = len(files)
+    ptrs = (ctypes.c_void_p * n)(*[f.ctypes.data for f in files])
+    sizes = (ctypes.c_size_t * n)(*[f.size for f in files])
+    nbytes = ctypes.c_size_t()
+    ll = ctypes.POINTER(ctypes.c_longlong)
+    check(lib.k2y_png_plan(ptrs, sizes, n, src_offsets.ctypes.data_as(ll), dst_offsets.ctypes.data_as(ll),
+                           blob.ctypes.data if blob is not None else None, blob.size if blob is not None else 0, ctypes.byref(nbytes)))
+    return nbytes.value
+
+
+_DECODERS = {"jpeg": (_jpeg_plan, "k2y_jpeg_workspace_bytes", "k2y_jpeg_decode", "reserve_jpeg", "workspace", "status"),
+             "png": (_png_plan, "k2y_png_workspace_bytes", "k2y_png_decode", "reserve_png", "png_workspace", "png_status")}
+
+
+def _fill(kind: str, files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: Staging, plan):
+    """Writes `files` and their blob into ``staging.host`` where `plan` places them and reserves the decode's workspace and
+    status words; returns the decode call, to be enqueued once the range is on the device."""
+    planner, ws_fn, decode_fn, reserve, ws_name, status_name = _DECODERS[kind]
+    src_offsets, blob_at, blob_bytes, end = plan
+    host = staging.host.numpy()
+    for f, off in zip(files, src_offsets):
+        host[off:off + f.size] = f
+    blob = host[blob_at:blob_at + blob_bytes]
+    planner(files, src_offsets, dst_offsets, blob)
+    ws = ctypes.c_size_t()
+    check(getattr(lib, ws_fn)(blob.ctypes.data, ctypes.byref(ws)))
+    getattr(staging, reserve)(ws.value, len(files))
+    workspace, status = getattr(staging, ws_name), getattr(staging, status_name)
+
+    def decode(dst: torch.Tensor):
+        st = staging.stream
+        with torch.cuda.stream(st):
+            check(getattr(lib, decode_fn)(blob.ctypes.data, staging.dev.data_ptr() + blob_at, staging.dev.data_ptr(), dst.data_ptr(),
+                                          workspace.data_ptr(), workspace.numel(), status.data_ptr(), ctypes.c_void_p(st.cuda_stream)))
+    return decode
+
+
+def _stage(kind: str, files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: Staging, plan, dst: torch.Tensor) -> None:
+    decode = _fill(kind, files, dst_offsets, staging, plan)
+    b, e = int(plan[0][0]), plan[3]
+    with torch.cuda.stream(staging.stream):
+        staging.dev[b:e].copy_(staging.host[b:e], non_blocking=True)
+    decode(dst)
+
+
 def stage_jpegs(files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: Staging, plan, dst: torch.Tensor) -> None:
     """Puts the JPEG `files` and their descriptor blob into ``staging.host`` where `plan` (``_jpeg_layout``) places them
     (``staging.reserve`` of the whole batch first), copies that range to ``staging.dev`` in one H2D copy and decodes the files
     into `dst` (a device uint8 buffer) at `dst_offsets`, on ``staging.stream``.  Per-image status words land in
     ``staging.status``."""
-    n = len(files)
-    src_offsets, blob_at, blob_bytes, end = plan
-    base = int(src_offsets[0])
-    host = staging.host.numpy()
-    for f, off in zip(files, src_offsets):
-        host[off:off + f.size] = f
-    blob = host[blob_at:blob_at + blob_bytes]
-    _jpeg_plan(files, src_offsets, dst_offsets, blob)
-    ws = ctypes.c_size_t()
-    check(lib.k2y_jpeg_workspace_bytes(blob.ctypes.data, ctypes.byref(ws)))
-    staging.reserve_jpeg(ws.value, n)
-    st = staging.stream
-    with torch.cuda.stream(st):
-        staging.dev[base:end].copy_(staging.host[base:end], non_blocking=True)
-        check(lib.k2y_jpeg_decode(blob.ctypes.data, staging.dev.data_ptr() + blob_at, staging.dev.data_ptr(), dst.data_ptr(),
-                                  staging.workspace.data_ptr(), staging.workspace.numel(), staging.status.data_ptr(),
-                                  ctypes.c_void_p(st.cuda_stream)))
+    _stage("jpeg", files, dst_offsets, staging, plan, dst)
 
 
-def _jpeg_layout(files: Sequence[np.ndarray], dst_offsets: np.ndarray, base: int):
+def stage_pngs(files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: Staging, plan, dst: torch.Tensor) -> None:
+    """``stage_jpegs`` for GPU-decodable PNG files (`plan` from ``_jpeg_layout(..., _png_plan)``); status words land in
+    ``staging.png_status``."""
+    _stage("png", files, dst_offsets, staging, plan, dst)
+
+
+def _jpeg_layout(files: Sequence[np.ndarray], dst_offsets: np.ndarray, base: int, planner=_jpeg_plan):
     """Offsets of the files and of the blob in the staging buffer from `base` on, the blob's size and the end of the range.
-    The blob's size query parses every header: a file the plan refuses raises ``ValueError`` here."""
+    The blob's size query parses every header: a file the plan refuses raises ``ValueError`` here.  `planner`: ``_jpeg_plan``
+    or ``_png_plan``."""
     sizes = np.array([f.size for f in files], np.int64)
     padded = (sizes + ALIGN - 1) // ALIGN * ALIGN
     src_offsets = (base + np.concatenate([[0], np.cumsum(padded)[:-1]])).astype(np.int64)
     blob_at = int(base + padded.sum())
     try:
-        blob_bytes = _jpeg_plan(files, src_offsets, dst_offsets, None)
+        blob_bytes = planner(files, src_offsets, dst_offsets, None)
     except K2YError as e:
         raise ValueError(str(e)) from e
     return src_offsets, blob_at, blob_bytes, blob_at + blob_bytes
@@ -314,19 +430,28 @@ def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, ou
                      image_hw_out: Optional[torch.Tensor], view_yx_out: Optional[torch.Tensor] = None) -> None:
     """Packs `images` into ``staging.host``, copies them to the device and letterboxes them into ``out[:n]`` (and their sizes
     into ``image_hw_out[:n]``), all on ``staging.stream``.  GPU-decodable JPEGs travel compressed behind the packed pixels and
-    are decoded into their place first (``stage_jpegs``).  The host buffer is reused by the next call: wait for this copy
+    are decoded into their place first (``stage_jpegs``), and so are the layout's GPU PNGs, whose range the same H2D copy moves
+    (``stage_pngs``).  The host buffer is reused by the next call: wait for this copy
     before packing into it again.  A layout with tiling letterboxes its n * V views instead (``k2y_letterbox_u8_views``),
     image-major: ``out[:n * V]``, each view's (th, tw) into ``image_hw_out[:n * V]`` and its (y0, x0) into
     ``view_yx_out[:n * V]`` (float32 [N, 2])."""
     n = len(layout)
-    staging.reserve(layout.jpeg_plan[3] if layout.jpeg else layout.nbytes, n * layout.views)
+    staging.reserve(layout.staged_end, n * layout.views)
     layout.pack(images, staging.host.numpy())
     in_h, in_w = layout.in_hw
     st = staging.stream
     with torch.cuda.stream(st):
         for b, e in layout.host_ranges():
             staging.dev[b:e].copy_(staging.host[b:e], non_blocking=True)
-        if layout.jpeg:
+        if layout.png:      # the JPEGs' and PNGs' files and blobs in one H2D copy, then both decodes
+            decodes = [_fill(k, [f for _, f in files], dst, staging, plan) for k, files, dst, plan in
+                       (("jpeg", layout.jpeg, getattr(layout, "jpeg_dst", None), layout.jpeg_plan),
+                        ("png", layout.png, layout.png_dst, layout.png_plan)) if files]
+            b = int((layout.jpeg_plan or layout.png_plan)[0][0])
+            staging.dev[b:layout.staged_end].copy_(staging.host[b:layout.staged_end], non_blocking=True)
+            for decode in decodes:
+                decode(staging.dev)
+        elif layout.jpeg:
             stage_jpegs([f for _, f in layout.jpeg], layout.jpeg_dst, staging, layout.jpeg_plan, staging.dev)
         offs = layout.offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong))
         if layout.windows is not None:
@@ -349,16 +474,18 @@ def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, ou
 
 
 def letterbox_batch_device(images: List, in_hw, out: Optional[torch.Tensor] = None,
-                           image_hw_out: Optional[torch.Tensor] = None, stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
+                           image_hw_out: Optional[torch.Tensor] = None, stream: Optional[torch.cuda.Stream] = None,
+                           gpu_png: bool = False) -> torch.Tensor:
     """images: host numpy uint8 [h, w, 3] RGB arrays of any sizes, or image files (``bytes``, ``bytearray``, ``memoryview``:
     see ``BatchLayout``) -> CUDA uint8 [n, in_h, in_w, 3] letterboxed (zero fill), the
     same bytes ``letterbox_device`` gives each image.  One pinned staging buffer, one H2D copy, one batched letterbox launch on
     `stream` (default: the current stream), asynchronous.  `out` ([N >= n, in_h, in_w, 3] uint8, e.g. a network's bound input)
     receives the images in its first n rows; `image_hw_out` ([N >= n, 2] float32), if given, receives each image's (h, w).
     When the batch holds JPEGs decoded on the GPU, the call synchronises `stream` to read their status words and raises
-    ``K2YError`` if one of them was corrupt (``check_jpeg_status``)."""
+    ``K2YError`` if one of them was corrupt (``check_jpeg_status``).  With `gpu_png` the PNGs the GPU takes are decoded there
+    too (``BatchLayout``), and a damaged zlib stream PIL refuses raises the same way (``check_png_status``)."""
     in_h, in_w = int(in_hw[0]), int(in_hw[1])
-    layout = BatchLayout(images, (in_h, in_w))
+    layout = BatchLayout(images, (in_h, in_w), gpu_png=gpu_png)
     n = len(layout)
     device = out.device if out is not None else torch.device("cuda", torch.cuda.current_device())
     _check_out(out, n, (in_h, in_w, 3), torch.uint8, "out", None)
@@ -370,9 +497,14 @@ def letterbox_batch_device(images: List, in_hw, out: Optional[torch.Tensor] = No
     staging = Staging(device, st)
     with torch.cuda.device(device):
         letterbox_packed(layout, images, staging, out, image_hw_out)
-        if layout.jpeg:
+        if layout.jpeg or layout.png:
             with torch.cuda.stream(st):
-                check_jpeg_status(staging.status[:len(layout.jpeg)].cpu().numpy(), [i for i, _ in layout.jpeg])
+                jst = staging.status[:len(layout.jpeg)].cpu().numpy() if layout.jpeg else None
+                pst = staging.png_status[:len(layout.png)].cpu().numpy() if layout.png else None
+            if layout.jpeg:
+                check_jpeg_status(jst, [i for i, _ in layout.jpeg])
+            if layout.png:
+                check_png_status(pst, [i for i, _ in layout.png])
     return out
 
 
@@ -421,3 +553,55 @@ def check_jpeg_status(status: np.ndarray, images) -> None:
     if bad:
         what = {1: "invalid Huffman code", 2: "entropy-coded data ends early", 3: "invalid Huffman code, data ends early"}
         raise K2YError("corrupt JPEG data: " + ", ".join(f"image {i}: {what.get(w, w)}" for i, w in bad))
+
+
+def decode_png_batch(files: Sequence, stream: Optional[torch.cuda.Stream] = None, with_status: bool = False):
+    """GPU-decodable PNG files (``bytes``, ``bytearray``, ``memoryview``) -> list of CUDA uint8 [h, w, 3] RGB views of one
+    packed device buffer, byte for byte what ``Helper._read_img`` (PIL) gives.  One pinned staging buffer, one H2D copy and
+    one launch per decode stage on `stream` (default: the current stream), then a synchronise to read the per-image status.
+    A file the GPU decoder does not take raises ``ValueError`` before anything is enqueued; a zlib stream PIL refuses raises
+    ``K2YError`` naming the images, unless `with_status`, which returns (views, status int32 [n, 4]: error bits, chunks, chunks
+    whose speculative start was confirmed, bytes the longest single decoder inflated) instead."""
+    if not isinstance(files, (list, tuple)) or len(files) == 0:
+        raise ValueError("expected a non-empty list of PNG files")
+    bufs, shapes = [], []
+    for i, f in enumerate(files):
+        if not isinstance(f, ENCODED):
+            raise ValueError(f"file {i}: expected bytes, bytearray or memoryview, got {type(f).__name__}")
+        buf = _file_bytes(f)
+        if _png_route(buf) is None:
+            info = _png_info(buf)
+            why = "not a PNG file with a sound IHDR" if info is None else inspect_png(f)[3]
+            raise ValueError(f"file {i}: not decodable on the GPU: {why}")
+        info = _png_info(buf)
+        bufs.append(buf)
+        shapes.append((int(info.height), int(info.width)))
+    sizes = np.array([h * w * 3 for h, w in shapes], np.int64)
+    padded = (sizes + ALIGN - 1) // ALIGN * ALIGN
+    offsets = np.concatenate([[0], np.cumsum(padded)[:-1]]).astype(np.int64)
+    device = torch.device("cuda", torch.cuda.current_device())
+    st = stream if stream is not None else torch.cuda.current_stream(device)
+    staging = Staging(device, st)
+    plan = _jpeg_layout(bufs, offsets, int(padded.sum()), _png_plan)
+    staging.reserve(plan[3], len(bufs))
+    with torch.cuda.stream(st):
+        stage_pngs(bufs, offsets, staging, plan, staging.dev)
+        status = staging.png_status[:len(bufs)].cpu().numpy()
+    out = [staging.dev[o:o + h * w * 3].view(h, w, 3) for o, (h, w) in zip(offsets, shapes)]
+    if with_status:
+        return out, status
+    check_png_status(status, range(len(bufs)))
+    return out
+
+
+PNG_ERRORS = {1: "invalid block header", 2: "invalid code", 4: "distance too far back", 8: "image data ends early",
+              16: "Adler-32 mismatch", 32: "filter type above 4"}
+
+
+def check_png_status(status: np.ndarray, images) -> None:
+    """Raises ``K2YError`` naming the images whose zlib stream or row filters PIL refuses.  `status`: the decode's int32 [n, 4]
+    words of the GPU-decoded PNGs, `images`: their positions in the caller's batch."""
+    bad = [(int(i), int(w)) for i, w in zip(images, status[:, 0]) if w]
+    if bad:
+        raise K2YError("corrupt PNG data: " + ", ".join(
+            f"image {i}: " + ", ".join(v for k, v in PNG_ERRORS.items() if w & k) for i, w in bad))

@@ -22,6 +22,9 @@ give; only the compressed files come back.  Duplicate stems are refused before a
 With --tiles ROWS COLS every image is detected on ROWS x COLS overlapping tiles as well as whole (--tile_overlap, default 0.2;
 DetectionPipeline.enable_tiling): a batch then holds batch // (1 + ROWS * COLS) images, the views' records are merged on the GPU
 and the lines keep their shape, with "index" // (boxes per network input) telling the view a detection came from.
+
+With --gpu_png the PNG files the GPU decoder takes (preprocess.png_gpu_decodable) stay compressed too and are decoded on the GPU
+(DetectionPipeline.enable_png_decode), with the pixels PIL gives; the lines are the same as without it.
 """
 import argparse
 import io
@@ -38,7 +41,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 from k210_yolo_framework_b200.dist import shard_range  # noqa: E402
 from k210_yolo_framework_b200.helper import read_image  # noqa: E402
-from k210_yolo_framework_b200.preprocess import gpu_decodable  # noqa: E402
+from k210_yolo_framework_b200.preprocess import gpu_decodable, png_gpu_decodable  # noqa: E402
 from k210_yolo_framework_b200.pipeline import DetectionPipeline  # noqa: E402
 
 EXTS = (".jpg", ".jpeg", ".png", ".bmp")
@@ -51,11 +54,14 @@ def list_images(path):
         return [l.strip() for l in fh if l.strip()]
 
 
-def load_image(path):
-    """The file's bytes when the GPU decodes it, else its pixels decoded on the host (Helper._read_img)."""
+def load_image(path, gpu_png=False):
+    """The file's bytes when the GPU decodes it (PNGs only with `gpu_png`), else its pixels decoded on the host
+    (Helper._read_img)."""
     with open(path, "rb") as fh:
         data = fh.read()
-    return data if gpu_decodable(data) else read_image(io.BytesIO(data))
+    if gpu_decodable(data) or (gpu_png and png_gpu_decodable(data)):
+        return data
+    return read_image(io.BytesIO(data))
 
 
 def open_pipeline(args, max_per_class=30):
@@ -74,6 +80,8 @@ def open_pipeline(args, max_per_class=30):
     pipe.engine.load_weights(args.ckpt)
     if getattr(args, "tiles", None):
         pipe.enable_tiling(args.tiles[0], args.tiles[1], args.tile_overlap)
+    if getattr(args, "gpu_png", False):
+        pipe.enable_png_decode()
     return pipe, world, rank
 
 
@@ -138,7 +146,8 @@ def serve(args, out_fh=None):
         pipe.enable_rendering(quality=args.draw_quality)
     n_out = 0
     B = pipe.images_per_batch
-    for g, item in enumerate(detect_files(pipe, files, getattr(args, "decode_threads", 4), load_image, rendered=bool(draw_dir))):
+    load = (lambda p: load_image(p, gpu_png=True)) if getattr(args, "gpu_png", False) else load_image
+    for g, item in enumerate(detect_files(pipe, files, getattr(args, "decode_threads", 4), load, rendered=bool(draw_dir))):
         chunk, dets, counts = item[:3]
         if draw_dir:        # this rank's files of the global batch
             first = g * world * B + rank * B
@@ -172,6 +181,8 @@ def add_model_args(ap):
                     help="also detect on ROWS x COLS overlapping tiles of every image and merge the views' records on the GPU; "
                          "a batch then holds batch // (1 + ROWS * COLS) images")
     ap.add_argument("--tile_overlap", type=float, default=0.2, help="fraction of a tile shared with its neighbour (with --tiles)")
+    ap.add_argument("--gpu_png", action="store_true",
+                    help="decode the PNG files the GPU decoder takes on the GPU too (the same pixels as PIL), not in the host threads")
     ap.add_argument("--decode_threads", type=int, default=4, help="host threads reading the next batch's files and decoding those the GPU does not (PIL)")
 
 
