@@ -82,13 +82,15 @@ cudaError_t launch_dwconv(const DwArgs &a, cudaStream_t st);
 cudaError_t launch_maxpool(const PoolArgs &a, cudaStream_t st);
 cudaError_t launch_image_max_u8(const unsigned char *x, int batch, size_t bytes_per_image, int *max_out, cudaStream_t st);
 
-// Programmatic dependent launch: every kernel of a step is launched with programmaticStreamSerializationAllowed, calls
-// pdl_trigger() first thing (the next kernel's CTAs may be scheduled as soon as this grid's CTAs have all started and
-// SM resources free up) and pdl_wait() before it touches anything a predecessor wrote or may still read (returns once
-// the preceding grid has completed and flushed).  Hides the launch gap and the next kernel's prologue behind the tail of
-// the current one; K2Y_NO_PDL=1 falls back to plain stream order.
+// Programmatic dependent launch: every kernel of a step is launched with programmaticStreamSerializationAllowed and calls
+// pdl_wait() before it touches anything a predecessor wrote or may still read (returns once the preceding grid has
+// completed and flushed).  The next kernel is launched as each grid's CTAs exit, before the grid's completion and flush,
+// which hides the launch gap.  No kernel triggers its dependents earlier (griddepcontrol.launch_dependents): the next
+// kernel's CTAs would then be placed as soon as any SM had room and wait there, and a persistent tensor-core CTA holds a
+// whole SM's shared memory while it waits, so with several nets in flight (LanedPipeline) one lane's waiting CTAs took the
+// SMs another lane's running kernels could use (cfg 2 at two lanes ran 0.913-0.919 ms per step with the early trigger,
+// 0.784-0.787 without, on an H100 80GB HBM3 SXM at 700 W).  K2Y_NO_PDL=1 falls back to plain stream order.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 bool pdl_enabled();
 
 template <typename... KArgs, typename... Args>

@@ -34,7 +34,6 @@ __device__ __forceinline__ const float *src_ptr(const ConvArgs &a, int b, int iy
 
 template <int TM, bool VEC>
 __global__ void __launch_bounds__(256) conv_igemm_simt_kernel(const ConvArgs a) {
-    pdl_trigger();
     pdl_wait();
     constexpr int BM = 16 * TM;
     constexpr int A_PER_T = VEC ? (BM / 64) : (BM / 16);  // float4s or scalars of A per thread per k-tile
@@ -213,7 +212,6 @@ __global__ void __launch_bounds__(256) conv_igemm_simt_kernel(const ConvArgs a) 
 // ((TY-1)*S+3)*((TX-1)*S+3) / (TY*TX)  (3x for stride 1 with 2x4 outputs).  grid = (ceil(XT*C4 / 128), B*ceil(OH/TY)).
 template <int STRIDE, int TX, int TY>
 __global__ void __launch_bounds__(128) dwconv3x3_kernel(const DwArgs a) {
-    pdl_trigger();
     pdl_wait();
     constexpr int NCOL = (TX - 1) * STRIDE + 3;
     constexpr int NROW = (TY - 1) * STRIDE + 3;
@@ -303,7 +301,6 @@ struct FirstConvConsts {
 
 template <int COUT, bool U8, int ACT>  // ACT: compile-time activation (ACT_LEAKY / ACT_RELU6), -1 = read a.act at run time
 __global__ void __launch_bounds__(128) first_conv3x3_kernel(const ConvArgs a, const FirstConvConsts<COUT> cw) {
-    pdl_trigger();
     constexpr int PITCH = COUT + 4;  // floats; conflict-free float4 rows
     __shared__ __align__(16) float stage[128 * PITCH];
     __shared__ float lut[U8 ? 512 : 1];  // u8 -> u8 / max(image) (IEEE division, as the reference's float32 cast implies) for the
@@ -422,7 +419,6 @@ __global__ void __launch_bounds__(256) image_max_u8_kernel(const unsigned char *
 }
 
 __global__ void __launch_bounds__(256) maxpool2x2_kernel(const PoolArgs a) {
-    pdl_trigger();
     pdl_wait();
     const int c4n = a.C >> 2;
     const size_t total = (size_t)a.B * a.OH * a.OW * c4n;

@@ -306,7 +306,6 @@ constexpr int SCAN_BOXES = 64;
 
 __global__ void __launch_bounds__(SCAN_THREADS) detect_scan_kernel(const KerasParams p) {
     extern __shared__ __align__(16) float s_scan[];  // [SCAN_BOXES][E] records, then [SCAN_BOXES] sigmoid(conf)
-    pdl_trigger();
     const int b = blockIdx.y, box0 = blockIdx.x * SCAN_BOXES, tid = threadIdx.x;
     const int nb = min(SCAN_BOXES, p.nbox - box0);
     const int E = 5 + p.C;
@@ -795,7 +794,6 @@ __global__ void __launch_bounds__(NMS_THREADS, 2) detect_nms_kernel(const KerasP
     extern __shared__ __align__(16) unsigned char s_nms[];
     __shared__ int s_red[2][NMS_WARPS][3];
     __shared__ unsigned long long s_best[2 * NMS_WARPS];
-    pdl_trigger();
     const int c = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
     pdl_wait();
     const int n = p.ncand[b * p.C + c];

@@ -87,7 +87,8 @@ constexpr int CONSUMER_REGS = 176;
 
 // Attribution builds (scripts/bench_conv_tc.py), never the shipped library: K2Y_TC_ABLATE = 1 drops the epilogue's stores to
 // global memory, 2 skips the MMAs (loads, splits and barriers stay), 3 skips the A split (the raw bits are the hi plane, lo
-// is zero).  Results are wrong in every variant; only the time means something.
+// is zero), 4 stops loading B after a CTA's first `stages` k-blocks (the MMAs read stale weight tiles: no B traffic from L2).
+// Results are wrong in every variant; only the time means something.
 #ifndef K2Y_TC_ABLATE
 #define K2Y_TC_ABLATE 0
 #endif
@@ -160,7 +161,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     uint8_t *smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
     Barriers *bars = reinterpret_cast<Barriers *>(smem_gen + (size_t)p.stages * stage_bytes + (GATHER ? 0 : STAGING_SMEM));
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    pdl_trigger();
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < p.stages; ++s) {
@@ -190,6 +190,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         uint32_t ph = 0;
         const uint32_t tx = b_bytes * (THREE_X ? 2u : 1u) + (GATHER ? 0u : a_bytes);
         constexpr int bk_elems = BF16 ? 64 : 32;  // k-block extent in elements of the weight map (bf16 or fp32)
+        int kb_done = 0;                          // ABLATE 4: k-blocks this CTA has loaded so far
         if (!GATHER && warp != 0) return;
         const int Cin = p.C0 + p.C1;
         const int wrow0 = warp * 32;  // first tile row of this warp
@@ -210,17 +211,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             for (int kb = kb0; kb < kb1; ++kb) {
                 mbar_wait(smem_u32(&bars->empty[s]), ph ^ 1u);
                 if (warp == 0) {
+                    const bool load_b = ABLATE != 4 || kb_done < p.stages;
                     if (elect_one_sync()) {
                         const uint32_t fb = smem_u32(&bars->full_b[s]);
-                        mbar_arrive_expect_tx(fb, tx);
+                        mbar_arrive_expect_tx(fb, load_b ? tx : (GATHER ? 0u : a_bytes));
                         if (!GATHER) {
                             for (int bx = 0; bx < A_BOXES; ++bx)
                                 tma_load_2d(stage_a(s) + (uint32_t)bx * A_TILE_BYTES, &map_a, fb, kb * KBK + bx * BK, mt * BM);
                         }
-                        tma_load_2d(stage_b_hi(s), &map_bhi, fb, kb * bk_elems, nt * p.BN);
-                        if (THREE_X) tma_load_2d(stage_b_lo(s), &map_blo, fb, kb * bk_elems, nt * p.BN);
+                        if (load_b) {
+                            tma_load_2d(stage_b_hi(s), &map_bhi, fb, kb * bk_elems, nt * p.BN);
+                            if (THREE_X) tma_load_2d(stage_b_lo(s), &map_blo, fb, kb * bk_elems, nt * p.BN);
+                        }
                     }
                     __syncwarp();
+                    ++kb_done;
                 }
                 if (GATHER) {
                     // Each k-block is KBK consecutive channels of one filter tap, i.e. one contiguous run per output pixel.
@@ -519,7 +524,6 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(const float *__restr
                                                             const float *__restrict__ residual, const float *__restrict__ scale,
                                                             const float *__restrict__ shift, int M, int N, int splits,
                                                             size_t split_stride, float slope, float clamp) {
-    pdl_trigger();
     pdl_wait();
     const int n4 = N >> 2;
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

@@ -11,9 +11,10 @@ every launch, so device events around the call would time the host.  Inputs rota
 inputs and outputs do not stay in the 50 MB L2 from one launch to the next.
 
 Ablation libraries (built with -DK2Y_TC_ABLATE=N, never the shipped one) attribute the time: 1 = no epilogue stores,
-2 = no MMAs (loads, splits and barriers kept), 3 = no A split (raw bits as hi, zero lo).
+2 = no MMAs (loads, splits and barriers kept), 3 = no A split (raw bits as hi, zero lo), 4 = no B traffic (weight tiles are
+loaded for a CTA's first `stages` k-blocks only; the MMAs then read stale ones).
 
-    python scripts/bench_conv_tc.py --build-ablations DIR          # compile the three variants into DIR (no GPU needed)
+    python scripts/bench_conv_tc.py --build-ablations DIR          # compile the four variants into DIR (no GPU needed)
     python scripts/bench_conv_tc.py [--ablations DIR] [--lib NAME=PATH ...] [--rounds 3] [--launches 200] [--json OUT]
 
 With several libraries the runs alternate (lib a, lib b, ..., lib a, ...) `--rounds` times; each cell is the median.
@@ -30,7 +31,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 MATH_TC_BF16X3, MATH_TC_TF32 = 3, 2
-ABLATIONS = {1: "no_epilogue_stores", 2: "no_mma", 3: "no_a_split"}
+ABLATIONS = {1: "no_epilogue_stores", 2: "no_mma", 3: "no_a_split", 4: "no_b_traffic"}
 # tensor-pipe rate per SM and clock (dense, data-sheet): 2048 bf16 MAC, 1024 tf32 MAC
 MAC_PER_CLK = {"bf16": 2048, "tf32": 1024}
 
