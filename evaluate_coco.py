@@ -38,7 +38,8 @@ def evaluate(args):
     results = [] if rank == 0 and getattr(args, "results", None) else None
     paths = [os.path.join(args.image_dir, im[1]) for im in images]
     idx = list(range(len(images)))
-    for chunk, dets, counts in detect_files(pipe, idx, args.decode_threads, lambda i: load_checked(paths[i], images[i][2], getattr(args, "gpu_png", False))):
+    gpu_png, gpu_progressive = getattr(args, "gpu_png", False), getattr(args, "gpu_progressive", False)
+    for chunk, dets, counts in detect_files(pipe, idx, args.decode_threads, lambda i: load_checked(paths[i], images[i][2], gpu_png, gpu_progressive)):
         if ev is None:
             continue
         ev.update(dets[:len(chunk)], counts[:len(chunk)], chunk)

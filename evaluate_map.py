@@ -28,10 +28,10 @@ from k210_yolo_framework_b200.preprocess import inspect_jpeg, inspect_png  # noq
 COCO_IOU = [round(0.5 + 0.05 * i, 2) for i in range(10)]
 
 
-def load_checked(path, hw, gpu_png=False):
+def load_checked(path, hw, gpu_png=False, gpu_progressive=False):
     """load_image, refusing a file whose size differs from its annotation row's (the boxes would land elsewhere).  The size of
-    a file kept compressed comes from its header (JPEG, or PNG with `gpu_png`)."""
-    img = load_image(path, gpu_png=True) if gpu_png else load_image(path)
+    a file kept compressed comes from its header (JPEG, progressive JPEG with `gpu_progressive`, or PNG with `gpu_png`)."""
+    img = load_image(path, gpu_png, gpu_progressive) if gpu_png or gpu_progressive else load_image(path)
     if isinstance(img, (bytes, bytearray, memoryview)):
         got = tuple((inspect_png if bytes(img[:4]) == b"\x89PNG" else inspect_jpeg)(img)[:2])
     else:
@@ -48,7 +48,8 @@ def evaluate(args):
     pipe, world, rank = open_pipeline(args, args.max_per_class)
     ev = DetectionAP(args.class_num, args.max_per_class, args.eval_iou, device=pipe.device_index) if rank == 0 else None
     idx = list(range(len(paths)))
-    for chunk, dets, counts in detect_files(pipe, idx, args.decode_threads, lambda i: load_checked(paths[i], hw[i], getattr(args, "gpu_png", False))):
+    gpu_png, gpu_progressive = getattr(args, "gpu_png", False), getattr(args, "gpu_progressive", False)
+    for chunk, dets, counts in detect_files(pipe, idx, args.decode_threads, lambda i: load_checked(paths[i], hw[i], gpu_png, gpu_progressive)):
         if ev is not None:
             ev.update(dets[:len(chunk)], counts[:len(chunk)], [(labels[i], hw[i]) for i in chunk])
     if world > 1:

@@ -296,7 +296,7 @@ int k2y_letterbox_u8_views(const unsigned char *src_dev, int n_views, const long
  * GPU-decodable: 8-bit sequential Huffman (SOF0/SOF1), one scan holding every component, 1 component or 3 that libjpeg
  * treats as YCbCr, chroma 1x1 with luma 1x1, 2x1, 1x2, 2x2 or 4x1, any restart interval.  Every other valid file
  * (progressive, arithmetic, 12-bit, lossless, CMYK/YCCK, RGB, multi-scan, DNL, other sampling) is reported with its
- * reason and is left to the host.
+ * reason and is left to the host; progressive files have decode entry points of their own (k2y_jpeg_progressive_*, below).
  * ---------------------------------------------------------------------------------------- */
 typedef struct {
     int32_t height, width, components;
@@ -329,6 +329,51 @@ int k2y_jpeg_workspace_bytes(const void *blob_host, size_t *bytes);
  * Corrupt data never makes a kernel read outside its image's bytes or write outside its output. */
 int k2y_jpeg_decode(const void *blob_host, const void *blob_dev, const unsigned char *src_dev, unsigned char *dst_dev,
                     void *workspace_dev, size_t workspace_bytes, int32_t *status_dev, void *stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Progressive Huffman JPEG decode on the device (SOF2), the same pixels as libjpeg-turbo with PIL's settings: jdphuff.c's
+ * entropy decode (spectral selection, successive approximation, EOB runs, correction bits), then the baseline decoder's
+ * IDCT, upsampling and colour conversion.  The baseline entry points above do not change: they report progressive files as
+ * valid but not theirs.
+ * GPU-decodable: SOF2 with 8-bit samples, 1 component or 3 that libjpeg treats as YCbCr, the baseline decoder's sampling
+ * layouts and size limits, any restart interval (it may change between scans), at most 64 scans, ending with an EOI marker.
+ * A scan libjpeg-turbo refuses (JERR_BAD_PROGRESSION: a DC scan with Se != 0; an AC scan with Ss > Se, Se > 63 or more than
+ * one component; Ah != 0 with Al != Ah - 1; Al > 13) makes the file K2Y_ERR_INVALID naming the scan.  Valid files left to the
+ * host, with their reason: scripts libjpeg-turbo decodes only with a JWRN_BOGUS_PROGRESSION warning (an AC scan before the
+ * component's DC, a refinement whose Ah is not the coefficient's last Al) or that send a first scan of a coefficient twice;
+ * scripts after which libjpeg-turbo block-smooths the output (jdcoefct.c smoothing_ok: every component has its DC and its
+ * zig-zag quantisers 0..9 nonzero, and some component's coefficient 1..9 was never sent or only down to a bit above 0);
+ * a Huffman table not defined before a scan that needs it; more than 64 scans.  Coefficients 10..63 never sent or
+ * partly refined decode on the device.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+    int32_t height, width, components;
+    int32_t sof_marker;             /* 0xC0 .. 0xCF */
+    int32_t scans;                  /* SOS markers before EOI (0 when the walk stopped at the frame header) */
+    int32_t levels;                 /* entropy-decode launches the scan script needs (see k2y_jpeg_progressive_decode) */
+    int32_t gpu_decodable;          /* 1: k2y_jpeg_progressive_plan accepts the file */
+    char reason[64];                /* why not, when gpu_decodable == 0 */
+} k2y_jpeg_progressive_info;
+/* Host only: walks every marker to EOI.  K2Y_ERR_INVALID (the message names the marker or the scan) for a malformed file;
+ * K2Y_OK with info->gpu_decodable and info->reason otherwise ("sequential (SOF 0xC0)" for a baseline file). */
+int k2y_jpeg_progressive_inspect(const unsigned char *data, size_t size, k2y_jpeg_progressive_info *info);
+/* Host only: the descriptor blob of a batch of n GPU-decodable progressive files (geometry, quantisation tables, one record
+ * per scan with its Huffman tables, one per (scan, restart interval) with its bytes in the file), with the arguments of
+ * k2y_jpeg_plan; src_offsets must be multiples of 16.  A file that is not GPU-decodable is K2Y_ERR_INVALID. */
+int k2y_jpeg_progressive_plan(const unsigned char *const *files, const size_t *sizes, int n, const long long *src_offsets,
+                              const long long *dst_offsets, void *blob, size_t blob_capacity, size_t *blob_bytes);
+/* Device workspace k2y_jpeg_progressive_decode needs for the batch a blob describes (read from the host copy of the blob). */
+int k2y_jpeg_progressive_workspace_bytes(const void *blob_host, size_t *bytes);
+/* Decodes the batch, asynchronous on `stream`, with the arguments of k2y_jpeg_decode; src_dev is 16-byte aligned and each
+ * file's slot is readable up to its size rounded up to 16 bytes.  The entropy decode takes one launch per level of the
+ * scripts (a scan's level is one more than the highest level of the earlier scans that touched one of its coefficients, 0
+ * if none; a default libjpeg script has three), each decoding every (scan, restart interval) segment of that level serially
+ * in one thread; then dequantise + IDCT and upsample + colour, one launch each.  status_dev: int32 [n][4] per image: error
+ * bits (1 invalid Huffman code, 2 entropy data ended early, 4 a DC value outside int: the image's pixels are then undefined,
+ * the other images' are exact), 0, 0 (the decode does not speculate, so it has no synchronisation rounds), segments decoded.
+ * Corrupt data never makes a kernel read outside its image's bytes or write outside its output. */
+int k2y_jpeg_progressive_decode(const void *blob_host, const void *blob_dev, const unsigned char *src_dev, unsigned char *dst_dev,
+                                void *workspace_dev, size_t workspace_bytes, int32_t *status_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * PNG decode on the device, in front of k2y_letterbox_u8_batch: the RGB pixels Helper._read_img (PIL) gives for

@@ -55,6 +55,11 @@ class JpegInfo(ctypes.Structure):
                 ("entropy_offset", c_int32), ("reason", ctypes.c_char * 64)]
 
 
+class JpegProgressiveInfo(ctypes.Structure):
+    _fields_ = [("height", c_int32), ("width", c_int32), ("components", c_int32), ("sof_marker", c_int32), ("scans", c_int32),
+                ("levels", c_int32), ("gpu_decodable", c_int32), ("reason", ctypes.c_char * 64)]
+
+
 class PngInfo(ctypes.Structure):
     _fields_ = [("height", c_int32), ("width", c_int32), ("color_type", c_int32), ("bit_depth", c_int32), ("interlace", c_int32),
                 ("idat_chunks", c_int32), ("stream_bytes", c_int64), ("gpu_decodable", c_int32), ("reason", ctypes.c_char * 64)]
@@ -127,6 +132,11 @@ _SIGNATURES = {
                               c_void_p, c_size_t, POINTER(c_size_t)]),
     "k2y_jpeg_workspace_bytes": (c_int, [c_void_p, POINTER(c_size_t)]),
     "k2y_jpeg_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "k2y_jpeg_progressive_inspect": (c_int, [c_void_p, c_size_t, POINTER(JpegProgressiveInfo)]),
+    "k2y_jpeg_progressive_plan": (c_int, [POINTER(c_void_p), POINTER(c_size_t), c_int, POINTER(ctypes.c_longlong),
+                                          POINTER(ctypes.c_longlong), c_void_p, c_size_t, POINTER(c_size_t)]),
+    "k2y_jpeg_progressive_workspace_bytes": (c_int, [c_void_p, POINTER(c_size_t)]),
+    "k2y_jpeg_progressive_decode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p]),
     "k2y_png_inspect": (c_int, [c_void_p, c_size_t, POINTER(PngInfo)]),
     "k2y_png_plan": (c_int, [POINTER(c_void_p), POINTER(c_size_t), c_int, POINTER(ctypes.c_longlong), POINTER(ctypes.c_longlong),
                              c_void_p, c_size_t, POINTER(c_size_t)]),

@@ -32,6 +32,7 @@ coordinates and in the usual block format, so everything behind it is unchanged.
 
 ``enable_png_decode`` makes ``submit_images`` decode the PNG files the GPU takes there too (``preprocess.png_gpu_decodable``),
 in the same staging range and H2D copy as the batch's JPEGs; their status words travel beside the JPEGs'.
+``enable_progressive_jpeg_decode`` does the same for progressive JPEGs (``preprocess.progressive_gpu_decodable``).
 """
 from __future__ import annotations
 
@@ -46,7 +47,7 @@ from . import yolonet
 from ._lib import check, lib
 from .detect import DET_WORDS, KerasDetector
 from .dist import DetectionGather
-from .preprocess import BatchLayout, Staging, check_jpeg_status, check_png_status, letterbox_packed
+from .preprocess import BatchLayout, Staging, check_jpeg_status, check_png_status, check_progressive_status, letterbox_packed
 
 SLOTS = 2
 
@@ -95,6 +96,10 @@ class DetectionPipeline:
         self._gpu_png = False
         self._png_idx: List[list] = [[] for _ in range(SLOTS)]
         self._png_status = [torch.zeros((batch, 4), dtype=torch.int32).pin_memory() for _ in range(SLOTS)]
+        # enable_progressive_jpeg_decode: the same for the batch's GPU-decoded progressive JPEGs
+        self._gpu_progressive = False
+        self._prog_idx: List[list] = [[] for _ in range(SLOTS)]
+        self._prog_status = [torch.zeros((batch, 4), dtype=torch.int32).pin_memory() for _ in range(SLOTS)]
         self._steps = 0
         self._submitted = 0
         # enable_rendering: label atlas, colour table, quality, one encoder per gather slot (its files live until rendered())
@@ -147,6 +152,12 @@ class DetectionPipeline:
         not 16-bit grey, sound chunks) on the GPU, with the pixels PIL gives, instead of on the host; ``collect`` raises
         ``K2YError`` naming a PNG whose zlib stream or row filters PIL refuses.  Other PNGs keep the host route."""
         self._gpu_png = True
+
+    def enable_progressive_jpeg_decode(self) -> None:
+        """From now on ``submit_images`` decodes the progressive JPEG files the GPU takes
+        (``preprocess.progressive_gpu_decodable``) on the GPU, with the pixels PIL gives, instead of on the host; ``collect``
+        raises ``K2YError`` naming one whose entropy-coded data was corrupt.  Other progressive files keep the host route."""
+        self._gpu_progressive = True
 
     def set_image_shapes(self, image_hw) -> None:
         """Original (pre-letterbox) image sizes, [batch, 2] (h, w); defaults to the network input size."""
@@ -239,6 +250,7 @@ class DetectionPipeline:
             self._h2d_done[slot].record(self._copy_stream)
         self._jpeg_idx[self._steps % SLOTS] = []
         self._png_idx[self._steps % SLOTS] = []
+        self._prog_idx[self._steps % SLOTS] = []
         t = self._run_slot(slot, buf, n, None, None)
         self._rendered_slot[t] = False
         return t
@@ -299,7 +311,7 @@ class DetectionPipeline:
         before anything is enqueued."""
         if self._tiling is not None and isinstance(images, (list, tuple)) and len(images) > self.images_per_batch:
             raise ValueError(f"{len(images)} images of {self._views} views do not fit a batch of {self.batch}")
-        layout = BatchLayout(images, self.in_hw, self._tiling, gpu_png=self._gpu_png)
+        layout = BatchLayout(images, self.in_hw, self._tiling, gpu_png=self._gpu_png, gpu_progressive=self._gpu_progressive)
         n = len(layout)
         if n > self.batch:
             raise ValueError(f"{n} images do not fit a batch of {self.batch}")
@@ -331,6 +343,11 @@ class DetectionPipeline:
             if layout.png:
                 with torch.cuda.stream(self._copy_stream):
                     self._png_status[s][:len(layout.png)].copy_(self._staging[slot].png_status[:len(layout.png)], non_blocking=True)
+            self._prog_idx[s] = [i for i, _ in layout.progressive]
+            if layout.progressive:
+                np_ = len(layout.progressive)
+                with torch.cuda.stream(self._copy_stream):
+                    self._prog_status[s][:np_].copy_(self._staging[slot].progressive_status[:np_], non_blocking=True)
         self._h2d_done[slot].record(self._copy_stream)
         nv = n * layout.views
         t = self._run_slot(slot, buf, nv, self._slot_hw[slot][:nv], n if self.world == 1 else None,
@@ -372,6 +389,9 @@ class DetectionPipeline:
         if self._png_idx[ticket]:
             idx = self._png_idx[ticket]
             check_png_status(self._png_status[ticket][:len(idx)].numpy(), idx)
+        if self._prog_idx[ticket]:
+            idx = self._prog_idx[ticket]
+            check_progressive_status(self._prog_status[ticket][:len(idx)].numpy(), idx)
         dets, counts = DetectionGather.split(self._host[ticket], self.gather.C, self.gather.K, DET_WORDS)
         n = self._rows[ticket]
         return (dets, counts) if n is None else (dets[:n], counts[:n])
@@ -492,6 +512,11 @@ class LanedPipeline:
         """``DetectionPipeline.enable_png_decode`` on every lane."""
         for ln in self.lanes:
             ln.enable_png_decode()
+
+    def enable_progressive_jpeg_decode(self) -> None:
+        """``DetectionPipeline.enable_progressive_jpeg_decode`` on every lane."""
+        for ln in self.lanes:
+            ln.enable_progressive_jpeg_decode()
 
     def enable_tiling(self, rows: int, cols: int, overlap: float = 0.2) -> None:
         """``DetectionPipeline.enable_tiling`` on every lane."""

@@ -21,6 +21,12 @@ PNG files take the same route when the caller opts in (``BatchLayout(gpu_png=Tru
 ``DetectionPipeline.enable_png_decode``): the PNGs ``inspect_png`` finds GPU-decodable travel compressed in the same staging
 range and H2D copy as the JPEGs, and ``k2y_png_decode`` writes the pixels PIL gives at their offsets.  A damaged zlib stream
 that PIL refuses sets the image's status word (``check_png_status``).  ``decode_png_batch`` returns the decoded pixels.
+
+Progressive JPEGs take the same route when the caller opts in (``BatchLayout(gpu_progressive=True)``,
+``letterbox_batch_device(gpu_progressive=True)``, ``DetectionPipeline.enable_progressive_jpeg_decode``): the files
+``progressive_gpu_decodable`` accepts travel compressed behind the JPEGs' and PNGs' ranges in the same H2D copy, and
+``k2y_jpeg_progressive_decode`` writes the pixels PIL gives at their offsets (``check_progressive_status`` for corrupt data).
+``decode_progressive_jpeg_batch`` returns the decoded pixels.
 """
 from __future__ import annotations
 
@@ -30,7 +36,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from ._lib import JpegInfo, K2YError, PngInfo, check, lib
+from ._lib import JpegInfo, JpegProgressiveInfo, K2YError, PngInfo, check, lib
 from .helper import read_image
 from .tiles import tile_windows
 
@@ -116,6 +122,45 @@ def gpu_decodable(data) -> bool:
     return _gpu_route(_file_bytes(data)) is not None
 
 
+def _progressive_info(buf: np.ndarray) -> Optional[JpegProgressiveInfo]:
+    """What the progressive walk says of a JPEG file, or None when `buf` is not one it accepts (other formats, malformed
+    headers or scans)."""
+    if buf.size < 4 or buf[0] != 0xFF or buf[1] != 0xD8:
+        return None
+    info = JpegProgressiveInfo()
+    if lib.k2y_jpeg_progressive_inspect(buf.ctypes.data, buf.size, ctypes.byref(info)) != 0:
+        return None
+    return info
+
+
+def inspect_jpeg_progressive(data):
+    """``inspect_jpeg`` for the progressive decoder: ``(h, w, gpu_decodable, reason)``, where `reason` says why a valid file is
+    not for the GPU progressive decoder ("sequential (SOF 0xC0)" for a baseline file, a script libjpeg-turbo warns about or
+    would block-smooth, ...).  Walks every marker to EOI.  Raises ``K2YError`` for a file that is not a JPEG or whose headers
+    or scan parameters are malformed (the message names the marker or the scan)."""
+    if not isinstance(data, ENCODED):
+        raise ValueError(f"expected the bytes of a file, got {type(data).__name__}")
+    buf = _file_bytes(data)
+    info = JpegProgressiveInfo()
+    check(lib.k2y_jpeg_progressive_inspect(buf.ctypes.data, buf.size, ctypes.byref(info)))
+    return int(info.height), int(info.width), bool(info.gpu_decodable), info.reason.decode()
+
+
+def _progressive_route(buf: np.ndarray) -> Optional[JpegProgressiveInfo]:
+    """The header of `buf` when the batch routes send it to the GPU progressive decoder (with progressive decoding enabled):
+    GPU-decodable and ending with its EOI marker, as for baseline files (``_gpu_route``)."""
+    info = _progressive_info(buf)
+    if info is None or not info.gpu_decodable or buf[-2] != 0xFF or buf[-1] != 0xD9:
+        return None
+    return info
+
+
+def progressive_gpu_decodable(data) -> bool:
+    """True when `data` (the bytes of a file) goes to the GPU progressive decoder in ``submit_images`` with progressive
+    decoding enabled."""
+    return _progressive_route(_file_bytes(data)) is not None
+
+
 def _png_info(buf: np.ndarray) -> Optional[PngInfo]:
     """The header of a PNG file, or None when `buf` is not one the parser accepts (other formats, no sound IHDR)."""
     if buf.size < 8 or bytes(buf[:8]) != b"\x89PNG\r\n\x1a\n":
@@ -198,20 +243,23 @@ class BatchLayout:
     holds the host pixels of entry i (None for a GPU JPEG).  ``jpeg_plan`` is where the JPEGs' bytes and their descriptor blob
     go in the staging buffer, behind the packed pixels (``_jpeg_layout``).  With `gpu_png`, ``png`` lists (index, file bytes) of
     the PNGs the GPU decodes (``png_gpu_decodable``) in the same way, and ``png_plan`` places them and their blob behind the
-    JPEGs' range, so that one H2D copy moves both (``staged_end`` is the end of everything the staging buffer holds).
+    JPEGs' range, so that one H2D copy moves both (``staged_end`` is the end of everything the staging buffer holds).  With
+    `gpu_progressive`, ``progressive`` and ``progressive_plan`` do the same for the progressive JPEGs the GPU decodes
+    (``progressive_gpu_decodable``), behind the PNGs' range.
 
     With `tiling` = (rows, cols, overlap) every image is letterboxed as V = 1 + rows * cols views (``tiles.tile_windows``:
     the whole image, then its tiles): ``views`` = V, ``windows`` int32 [n * V, 4] (y0, x0, th, tw) and ``view_matrices``
     float64 [n * V, 6] (each window's own ``letterbox_params`` matrix), image-major.  Everything above stays per image: staging,
     the JPEG decode and the renderer see the originals."""
 
-    def __init__(self, images: Sequence, in_hw, tiling=None, gpu_png: bool = False):
+    def __init__(self, images: Sequence, in_hw, tiling=None, gpu_png: bool = False, gpu_progressive: bool = False):
         _check_images(images)
         n = len(images)
         self.in_hw = (int(in_hw[0]), int(in_hw[1]))
         self.arrays: List[Optional[np.ndarray]] = []
         self.jpeg = []
         self.png = []
+        self.progressive = []
         shapes = []
         for i, im in enumerate(images):
             if isinstance(im, ENCODED):
@@ -220,6 +268,8 @@ class BatchLayout:
                 to = self.jpeg
                 if info is None and gpu_png:
                     info, to = _png_route(buf), self.png
+                if info is None and gpu_progressive:
+                    info, to = _progressive_route(buf), self.progressive
                 if info is not None:
                     to.append((i, buf))
                     self.arrays.append(None)
@@ -246,6 +296,7 @@ class BatchLayout:
                                           dtype=np.float64)
         self.jpeg_plan = None
         self.png_plan = None
+        self.progressive_plan = None
         self.staged_end = self.nbytes
         if self.jpeg:
             self.jpeg_dst = self.offsets[[i for i, _ in self.jpeg]].astype(np.int64)
@@ -256,6 +307,11 @@ class BatchLayout:
             self.png_plan = _jpeg_layout([f for _, f in self.png], self.png_dst, (self.staged_end + ALIGN - 1) // ALIGN * ALIGN,
                                          _png_plan)
             self.staged_end = self.png_plan[3]
+        if self.progressive:
+            self.progressive_dst = self.offsets[[i for i, _ in self.progressive]].astype(np.int64)
+            self.progressive_plan = _jpeg_layout([f for _, f in self.progressive], self.progressive_dst,
+                                                 (self.staged_end + ALIGN - 1) // ALIGN * ALIGN, _progressive_plan)
+            self.staged_end = self.progressive_plan[3]
 
     def __len__(self) -> int:
         return len(self.hw)
@@ -297,6 +353,18 @@ class Staging:
         self.status: Optional[torch.Tensor] = None      # int32 [n, 4] per decoded JPEG (k2y_jpeg_decode)
         self.png_workspace: Optional[torch.Tensor] = None   # k2y_png_decode's
         self.png_status: Optional[torch.Tensor] = None      # int32 [n, 4] per decoded PNG (k2y_png_decode)
+        self.progressive_workspace: Optional[torch.Tensor] = None   # k2y_jpeg_progressive_decode's
+        self.progressive_status: Optional[torch.Tensor] = None      # int32 [n, 4] per decoded progressive JPEG
+
+    def reserve_progressive(self, workspace_bytes: int, n: int) -> None:
+        with torch.cuda.stream(self.stream):
+            ws, st = self.progressive_workspace, self.progressive_status
+            if ws is None or ws.numel() < workspace_bytes:
+                cap = max(workspace_bytes, 2 * ws.numel() if ws is not None else 0)
+                self.progressive_workspace = torch.empty((cap,), dtype=torch.uint8, device=self.device)
+            if st is None or st.shape[0] < n:
+                self.progressive_status = torch.empty((max(n, 2 * st.shape[0] if st is not None else 0), 4), dtype=torch.int32,
+                                                      device=self.device)
 
     def reserve_jpeg(self, workspace_bytes: int, n: int) -> None:
         with torch.cuda.stream(self.stream):
@@ -362,8 +430,23 @@ def _png_plan(files: Sequence[np.ndarray], src_offsets: np.ndarray, dst_offsets:
     return nbytes.value
 
 
+def _progressive_plan(files: Sequence[np.ndarray], src_offsets: np.ndarray, dst_offsets: np.ndarray, blob: Optional[np.ndarray]) -> int:
+    """k2y_jpeg_progressive_plan: the blob's size (blob None), or the blob written into `blob` (16-byte aligned)."""
+    n = len(files)
+    ptrs = (ctypes.c_void_p * n)(*[f.ctypes.data for f in files])
+    sizes = (ctypes.c_size_t * n)(*[f.size for f in files])
+    nbytes = ctypes.c_size_t()
+    ll = ctypes.POINTER(ctypes.c_longlong)
+    check(lib.k2y_jpeg_progressive_plan(ptrs, sizes, n, src_offsets.ctypes.data_as(ll), dst_offsets.ctypes.data_as(ll),
+                                        blob.ctypes.data if blob is not None else None, blob.size if blob is not None else 0,
+                                        ctypes.byref(nbytes)))
+    return nbytes.value
+
+
 _DECODERS = {"jpeg": (_jpeg_plan, "k2y_jpeg_workspace_bytes", "k2y_jpeg_decode", "reserve_jpeg", "workspace", "status"),
-             "png": (_png_plan, "k2y_png_workspace_bytes", "k2y_png_decode", "reserve_png", "png_workspace", "png_status")}
+             "png": (_png_plan, "k2y_png_workspace_bytes", "k2y_png_decode", "reserve_png", "png_workspace", "png_status"),
+             "progressive": (_progressive_plan, "k2y_jpeg_progressive_workspace_bytes", "k2y_jpeg_progressive_decode",
+                             "reserve_progressive", "progressive_workspace", "progressive_status")}
 
 
 def _fill(kind: str, files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: Staging, plan):
@@ -405,6 +488,12 @@ def stage_jpegs(files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: S
     _stage("jpeg", files, dst_offsets, staging, plan, dst)
 
 
+def stage_progressive_jpegs(files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: Staging, plan, dst: torch.Tensor) -> None:
+    """``stage_jpegs`` for GPU-decodable progressive JPEG files (`plan` from ``_jpeg_layout(..., _progressive_plan)``); status
+    words land in ``staging.progressive_status``."""
+    _stage("progressive", files, dst_offsets, staging, plan, dst)
+
+
 def stage_pngs(files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: Staging, plan, dst: torch.Tensor) -> None:
     """``stage_jpegs`` for GPU-decodable PNG files (`plan` from ``_jpeg_layout(..., _png_plan)``); status words land in
     ``staging.png_status``."""
@@ -413,8 +502,8 @@ def stage_pngs(files: Sequence[np.ndarray], dst_offsets: np.ndarray, staging: St
 
 def _jpeg_layout(files: Sequence[np.ndarray], dst_offsets: np.ndarray, base: int, planner=_jpeg_plan):
     """Offsets of the files and of the blob in the staging buffer from `base` on, the blob's size and the end of the range.
-    The blob's size query parses every header: a file the plan refuses raises ``ValueError`` here.  `planner`: ``_jpeg_plan``
-    or ``_png_plan``."""
+    The blob's size query parses every header: a file the plan refuses raises ``ValueError`` here.  `planner`: ``_jpeg_plan``,
+    ``_png_plan`` or ``_progressive_plan``."""
     sizes = np.array([f.size for f in files], np.int64)
     padded = (sizes + ALIGN - 1) // ALIGN * ALIGN
     src_offsets = (base + np.concatenate([[0], np.cumsum(padded)[:-1]])).astype(np.int64)
@@ -443,11 +532,13 @@ def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, ou
     with torch.cuda.stream(st):
         for b, e in layout.host_ranges():
             staging.dev[b:e].copy_(staging.host[b:e], non_blocking=True)
-        if layout.png:      # the JPEGs' and PNGs' files and blobs in one H2D copy, then both decodes
+        if layout.png or layout.progressive:   # every decoder's files and blobs in one H2D copy, then the decodes
             decodes = [_fill(k, [f for _, f in files], dst, staging, plan) for k, files, dst, plan in
                        (("jpeg", layout.jpeg, getattr(layout, "jpeg_dst", None), layout.jpeg_plan),
-                        ("png", layout.png, layout.png_dst, layout.png_plan)) if files]
-            b = int((layout.jpeg_plan or layout.png_plan)[0][0])
+                        ("png", layout.png, getattr(layout, "png_dst", None), layout.png_plan),
+                        ("progressive", layout.progressive, getattr(layout, "progressive_dst", None), layout.progressive_plan))
+                       if files]
+            b = int((layout.jpeg_plan or layout.png_plan or layout.progressive_plan)[0][0])
             staging.dev[b:layout.staged_end].copy_(staging.host[b:layout.staged_end], non_blocking=True)
             for decode in decodes:
                 decode(staging.dev)
@@ -475,7 +566,7 @@ def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, ou
 
 def letterbox_batch_device(images: List, in_hw, out: Optional[torch.Tensor] = None,
                            image_hw_out: Optional[torch.Tensor] = None, stream: Optional[torch.cuda.Stream] = None,
-                           gpu_png: bool = False) -> torch.Tensor:
+                           gpu_png: bool = False, gpu_progressive: bool = False) -> torch.Tensor:
     """images: host numpy uint8 [h, w, 3] RGB arrays of any sizes, or image files (``bytes``, ``bytearray``, ``memoryview``:
     see ``BatchLayout``) -> CUDA uint8 [n, in_h, in_w, 3] letterboxed (zero fill), the
     same bytes ``letterbox_device`` gives each image.  One pinned staging buffer, one H2D copy, one batched letterbox launch on
@@ -483,9 +574,10 @@ def letterbox_batch_device(images: List, in_hw, out: Optional[torch.Tensor] = No
     receives the images in its first n rows; `image_hw_out` ([N >= n, 2] float32), if given, receives each image's (h, w).
     When the batch holds JPEGs decoded on the GPU, the call synchronises `stream` to read their status words and raises
     ``K2YError`` if one of them was corrupt (``check_jpeg_status``).  With `gpu_png` the PNGs the GPU takes are decoded there
-    too (``BatchLayout``), and a damaged zlib stream PIL refuses raises the same way (``check_png_status``)."""
+    too (``BatchLayout``), and a damaged zlib stream PIL refuses raises the same way (``check_png_status``); so do the
+    progressive JPEGs with `gpu_progressive` (``check_progressive_status``)."""
     in_h, in_w = int(in_hw[0]), int(in_hw[1])
-    layout = BatchLayout(images, (in_h, in_w), gpu_png=gpu_png)
+    layout = BatchLayout(images, (in_h, in_w), gpu_png=gpu_png, gpu_progressive=gpu_progressive)
     n = len(layout)
     device = out.device if out is not None else torch.device("cuda", torch.cuda.current_device())
     _check_out(out, n, (in_h, in_w, 3), torch.uint8, "out", None)
@@ -497,14 +589,17 @@ def letterbox_batch_device(images: List, in_hw, out: Optional[torch.Tensor] = No
     staging = Staging(device, st)
     with torch.cuda.device(device):
         letterbox_packed(layout, images, staging, out, image_hw_out)
-        if layout.jpeg or layout.png:
+        if layout.jpeg or layout.png or layout.progressive:
             with torch.cuda.stream(st):
                 jst = staging.status[:len(layout.jpeg)].cpu().numpy() if layout.jpeg else None
                 pst = staging.png_status[:len(layout.png)].cpu().numpy() if layout.png else None
+                gst = staging.progressive_status[:len(layout.progressive)].cpu().numpy() if layout.progressive else None
             if layout.jpeg:
                 check_jpeg_status(jst, [i for i, _ in layout.jpeg])
             if layout.png:
                 check_png_status(pst, [i for i, _ in layout.png])
+            if layout.progressive:
+                check_progressive_status(gst, [i for i, _ in layout.progressive])
     return out
 
 
@@ -605,3 +700,53 @@ def check_png_status(status: np.ndarray, images) -> None:
     if bad:
         raise K2YError("corrupt PNG data: " + ", ".join(
             f"image {i}: " + ", ".join(v for k, v in PNG_ERRORS.items() if w & k) for i, w in bad))
+
+
+def decode_progressive_jpeg_batch(files: Sequence, stream: Optional[torch.cuda.Stream] = None, with_status: bool = False):
+    """GPU-decodable progressive JPEG files (``bytes``, ``bytearray``, ``memoryview``) -> list of CUDA uint8 [h, w, 3] RGB views
+    of one packed device buffer, byte for byte what ``Helper._read_img`` (PIL) gives.  One pinned staging buffer, one H2D copy,
+    one entropy-decode launch per level of the scan scripts and one IDCT and one colour launch on `stream` (default: the
+    current stream), then a synchronise to read the per-image status.  A file the GPU decoder does not take raises
+    ``ValueError`` before anything is enqueued; corrupt entropy data raises ``K2YError`` naming the images, unless
+    `with_status`, which returns (views, status int32 [n, 4]: error bits, 0, 0, segments decoded) instead."""
+    if not isinstance(files, (list, tuple)) or len(files) == 0:
+        raise ValueError("expected a non-empty list of progressive JPEG files")
+    bufs, shapes = [], []
+    for i, f in enumerate(files):
+        if not isinstance(f, ENCODED):
+            raise ValueError(f"file {i}: expected bytes, bytearray or memoryview, got {type(f).__name__}")
+        buf = _file_bytes(f)
+        info = _progressive_info(buf)
+        if info is None or not info.gpu_decodable:
+            why = info.reason.decode() if info is not None else "not a well-formed JPEG file"
+            raise ValueError(f"file {i}: not decodable on the GPU: {why}")
+        bufs.append(buf)
+        shapes.append((int(info.height), int(info.width)))
+    sizes = np.array([h * w * 3 for h, w in shapes], np.int64)
+    padded = (sizes + ALIGN - 1) // ALIGN * ALIGN
+    offsets = np.concatenate([[0], np.cumsum(padded)[:-1]]).astype(np.int64)
+    device = torch.device("cuda", torch.cuda.current_device())
+    st = stream if stream is not None else torch.cuda.current_stream(device)
+    staging = Staging(device, st)
+    plan = _jpeg_layout(bufs, offsets, int(padded.sum()), _progressive_plan)
+    staging.reserve(plan[3], len(bufs))
+    with torch.cuda.stream(st):
+        stage_progressive_jpegs(bufs, offsets, staging, plan, staging.dev)
+        status = staging.progressive_status[:len(bufs)].cpu().numpy()
+    out = [staging.dev[o:o + h * w * 3].view(h, w, 3) for o, (h, w) in zip(offsets, shapes)]
+    if with_status:
+        return out, status
+    check_progressive_status(status, range(len(bufs)))
+    return out
+
+
+PROGRESSIVE_ERRORS = {1: "invalid Huffman code", 2: "entropy-coded data ends early", 4: "DC value out of range"}
+
+
+def check_progressive_status(status: np.ndarray, images) -> None:
+    """Raises ``K2YError`` naming the progressive JPEGs whose entropy-coded data was corrupt or ended early.  `status`: the
+    decode's int32 [n, 4] words of the GPU-decoded progressive JPEGs, `images`: their positions in the caller's batch."""
+    bad = [(int(i), int(w)) for i, w in zip(images, status[:, 0]) if w]
+    if bad:
+        raise K2YError("corrupt progressive JPEG data: " + ", ".join(
+            f"image {i}: " + ", ".join(v for k, v in PROGRESSIVE_ERRORS.items() if w & k) for i, w in bad))

@@ -24,7 +24,9 @@ DetectionPipeline.enable_tiling): a batch then holds batch // (1 + ROWS * COLS) 
 and the lines keep their shape, with "index" // (boxes per network input) telling the view a detection came from.
 
 With --gpu_png the PNG files the GPU decoder takes (preprocess.png_gpu_decodable) stay compressed too and are decoded on the GPU
-(DetectionPipeline.enable_png_decode), with the pixels PIL gives; the lines are the same as without it.
+(DetectionPipeline.enable_png_decode), with the pixels PIL gives; the lines are the same as without it.  --gpu_progressive does
+the same for the progressive JPEGs the GPU decoder takes (preprocess.progressive_gpu_decodable,
+DetectionPipeline.enable_progressive_jpeg_decode).
 """
 import argparse
 import io
@@ -41,7 +43,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 from k210_yolo_framework_b200.dist import shard_range  # noqa: E402
 from k210_yolo_framework_b200.helper import read_image  # noqa: E402
-from k210_yolo_framework_b200.preprocess import gpu_decodable, png_gpu_decodable  # noqa: E402
+from k210_yolo_framework_b200.preprocess import gpu_decodable, png_gpu_decodable, progressive_gpu_decodable  # noqa: E402
 from k210_yolo_framework_b200.pipeline import DetectionPipeline  # noqa: E402
 
 EXTS = (".jpg", ".jpeg", ".png", ".bmp")
@@ -54,12 +56,12 @@ def list_images(path):
         return [l.strip() for l in fh if l.strip()]
 
 
-def load_image(path, gpu_png=False):
-    """The file's bytes when the GPU decodes it (PNGs only with `gpu_png`), else its pixels decoded on the host
-    (Helper._read_img)."""
+def load_image(path, gpu_png=False, gpu_progressive=False):
+    """The file's bytes when the GPU decodes it (PNGs only with `gpu_png`, progressive JPEGs only with `gpu_progressive`),
+    else its pixels decoded on the host (Helper._read_img)."""
     with open(path, "rb") as fh:
         data = fh.read()
-    if gpu_decodable(data) or (gpu_png and png_gpu_decodable(data)):
+    if gpu_decodable(data) or (gpu_png and png_gpu_decodable(data)) or (gpu_progressive and progressive_gpu_decodable(data)):
         return data
     return read_image(io.BytesIO(data))
 
@@ -82,6 +84,8 @@ def open_pipeline(args, max_per_class=30):
         pipe.enable_tiling(args.tiles[0], args.tiles[1], args.tile_overlap)
     if getattr(args, "gpu_png", False):
         pipe.enable_png_decode()
+    if getattr(args, "gpu_progressive", False):
+        pipe.enable_progressive_jpeg_decode()
     return pipe, world, rank
 
 
@@ -146,7 +150,8 @@ def serve(args, out_fh=None):
         pipe.enable_rendering(quality=args.draw_quality)
     n_out = 0
     B = pipe.images_per_batch
-    load = (lambda p: load_image(p, gpu_png=True)) if getattr(args, "gpu_png", False) else load_image
+    gpu_png, gpu_progressive = getattr(args, "gpu_png", False), getattr(args, "gpu_progressive", False)
+    load = (lambda p: load_image(p, gpu_png, gpu_progressive)) if gpu_png or gpu_progressive else load_image
     for g, item in enumerate(detect_files(pipe, files, getattr(args, "decode_threads", 4), load, rendered=bool(draw_dir))):
         chunk, dets, counts = item[:3]
         if draw_dir:        # this rank's files of the global batch
@@ -183,6 +188,9 @@ def add_model_args(ap):
     ap.add_argument("--tile_overlap", type=float, default=0.2, help="fraction of a tile shared with its neighbour (with --tiles)")
     ap.add_argument("--gpu_png", action="store_true",
                     help="decode the PNG files the GPU decoder takes on the GPU too (the same pixels as PIL), not in the host threads")
+    ap.add_argument("--gpu_progressive", action="store_true",
+                    help="decode the progressive JPEG files the GPU decoder takes on the GPU too (the same pixels as PIL), not in "
+                         "the host threads")
     ap.add_argument("--decode_threads", type=int, default=4, help="host threads reading the next batch's files and decoding those the GPU does not (PIL)")
 
 
