@@ -13,7 +13,6 @@ a file whose size differs from the file's height / width raises ValueError.  Cla
 smallest category id (the order of Darknet's coco.names), so the file must list class_num categories.  --results writes
 the detections as a COCO results file (what the COCO evaluation server takes); --out the stats and per-category AP.
 """
-import argparse
 import json
 import os
 import sys
@@ -23,7 +22,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 from evaluate_map import load_checked  # noqa: E402
-from serve import add_model_args, detect_files, open_pipeline  # noqa: E402
+from serve import ModelArgParser, add_model_args, detect_files, open_pipeline  # noqa: E402
 from k210_yolo_framework_b200.evaluate import CocoEval, coco_results, coco_summary, load_coco_annotations  # noqa: E402
 
 
@@ -72,7 +71,7 @@ def to_json(res, cats):
 
 
 def main():
-    ap = argparse.ArgumentParser()
+    ap = ModelArgParser()
     add_model_args(ap)
     ap.add_argument("ann", help="COCO instances JSON file")
     ap.add_argument("image_dir", help="directory holding the listed file_name of every image")

@@ -12,7 +12,6 @@ batches in flight), and rank 0 feeds every gathered record block to the evaluato
 matching at each --eval_iou threshold (the first also gives the VOC 2007 11-point AP), IoU without a "+1 pixel" term, and
 every object counts (the lists carry no "difficult" flag).  The defaults report AP at 0.5 and the mean over 0.50:0.05:0.95.
 """
-import argparse
 import json
 import os
 import sys
@@ -21,7 +20,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-from serve import add_model_args, detect_files, load_image, open_pipeline  # noqa: E402
+from serve import ModelArgParser, add_model_args, detect_files, load_image, open_pipeline  # noqa: E402
 from k210_yolo_framework_b200.evaluate import DetectionAP, load_voc_annotations  # noqa: E402
 from k210_yolo_framework_b200.preprocess import inspect_jpeg, inspect_png  # noqa: E402
 
@@ -80,7 +79,7 @@ def to_json(res, thresholds):
 
 
 def main():
-    ap = argparse.ArgumentParser()
+    ap = ModelArgParser()
     add_model_args(ap)
     ap.add_argument("ann", help="annotation list (.npy of (path, labels [n, 5] (class, x, y, w, h) relative, (h, w)) rows)")
     ap.add_argument("--obj_thresh", type=float, default=0.01)

@@ -184,11 +184,39 @@ int k2y_detect_keras_strided(const k2y_detect_cfg *cfg, const float *const *head
  * has IoU 0) until max_per_class are kept.  Outputs as k2y_detect_keras_strided's, for `rows` >= n_images images: rows past
  * n_images get count 0.  One launch, asynchronous on `stream`, no scratch memory.
  * K2Y_ERR_INVALID (nothing launched) when views * max_per_class exceeds k2y_merge_views_max_records() (1024: VOC's 30 per
- * class takes 34 views, COCO's 100 takes 10) or views * n_boxes exceeds INT32_MAX. */
+ * class takes 34 views, COCO's 100 takes 10) or views * n_boxes exceeds INT32_MAX.  It is k2y_merge_views_ex with uniform
+ * ranges and the default options (below). */
 int k2y_merge_views_max_records(void);
 int k2y_merge_views(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev, int n_images, int rows,
                     int views, int n_boxes, int class_num, int max_per_class, float iou_thresh, k2y_det *dets_dev,
                     int32_t *counts_dev, long long det_image_stride_words, long long count_image_stride_words, void *stream);
+
+/* k2y_merge_views with a number of views per image and the options of tiling by tile size (oracle/tiles_merge_ref.py states
+ * each one; k2y_merge_views is this call with null offsets and sides, K2Y_MATCH_IOU and K2Y_MERGE_SUPPRESS):
+ *   view_offsets_dev  int32 [n_images + 1] on the device: image b owns the views view_offsets[b] .. view_offsets[b+1] - 1 of
+ *                     the per-view blocks, at most max_views of them; view numbers (index = view * n_boxes + index) stay per
+ *                     image.  NULL: image b owns views b * max_views .. b * max_views + max_views - 1.
+ *   view_sides_dev    int32 [N] on the device, each view's interior sides (1 top, 2 left, 4 bottom, 8 right: that edge of
+ *                     the window is inside its image; the whole image has none).  With it, a record is dropped before the
+ *                     merge when, in window coordinates, fminf / fmaxf of its y (x) fields is < border at a top (left)
+ *                     interior side or > fl(th - border) (fl(tw - border)) at a bottom (right) one; th, tw from view_hw_dev
+ *                     ([N][2] float32, as k2y_letterbox_u8_views writes them) and border >= 0.  NULL: no record is dropped.
+ *   match             K2Y_MATCH_IOU (IoU > thresh) or K2Y_MATCH_IOS (intersection over the smaller area > thresh, float32,
+ *                     0 for a box of area <= 0).
+ *   merge             K2Y_MERGE_SUPPRESS (a record that matches a kept one is dropped) or K2Y_MERGE_UNION (the kept record's
+ *                     box becomes the field-wise min / max of itself and the records it suppressed; -0.0 below +0.0, NaN
+ *                     fields take no part).
+ * The same launch shape, limits (max_views * max_per_class <= k2y_merge_views_max_records()) and outputs as k2y_merge_views;
+ * no scratch memory. */
+#define K2Y_MATCH_IOU 0
+#define K2Y_MATCH_IOS 1
+#define K2Y_MERGE_SUPPRESS 0
+#define K2Y_MERGE_UNION 1
+int k2y_merge_views_ex(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev,
+                       const int32_t *view_offsets_dev, const int32_t *view_sides_dev, const float *view_hw_dev, float border,
+                       int match, int merge, int n_images, int rows, int max_views, int n_boxes, int class_num, int max_per_class,
+                       float thresh, k2y_det *dets_dev, int32_t *counts_dev, long long det_image_stride_words,
+                       long long count_image_stride_words, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * Multi-GPU collation: images shard across ranks (one process per GPU), and the one exchange on the path

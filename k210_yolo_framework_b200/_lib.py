@@ -106,6 +106,9 @@ _SIGNATURES = {
     "k2y_merge_views_max_records": (c_int, []),
     "k2y_merge_views": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p,
                                 ctypes.c_longlong, ctypes.c_longlong, c_void_p]),
+    "k2y_merge_views_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_int, c_int,
+                                   c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, ctypes.c_longlong, ctypes.c_longlong,
+                                   c_void_p]),
     "k2y_comm_unique_id": (c_int, [c_void_p]),
     "k2y_comm_create": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_void_p)]),
     "k2y_comm_destroy": (c_int, [c_void_p]),

@@ -1009,14 +1009,35 @@ __global__ void __launch_bounds__(32) nms_boxes_kernel(const float4 *__restrict_
 // in shared memory: keys (pack_key of the score and the new index) sorted by warp 0, every record's box scattered to its key's
 // rank (binary search; the keys are unique), then rounds of "first candidate still alive -> keep -> every thread tests its own
 // two candidates against it", one barrier per round, liveness exchanged as one ballot word per 32 candidates.
+//
+// k2y_merge_views_ex generalises it (k2y_merge_views is its case of uniform ranges and the defaults):
+//   view ranges   image b owns views [off[b], off[b+1]) of the per-view blocks (at most V of them); view numbers stay per image.
+//   border drop   with a border m >= 0, a record of a view is dropped while it is loaded if it lies within m pixels of one of
+//                 the view's interior sides (a side bit per view, computed on the host), in the window's own coordinates:
+//                 fminf / fmaxf of its two y (x) fields against m and fl(th - m) (fl(tw - m)).  Dropped records become
+//                 zero keys, which sort behind every real one; the CTA counts them with a shared atomic.
+//   MATCH         template: MATCH_IOU is the detector's test above, MATCH_IOS is inter / fminf(area_a, area_b) > thr with the
+//                 same inter (a box of area <= 0 has metric 0), by the exact IEEE division.
+//   UNION         template: the kept record's box becomes the field-wise union (min of ymin / xmin, max of ymax / xmax) of the
+//                 records that die in its round, itself included.  Each warp reduces the four extrema of its dying candidates
+//                 as order-preserving integer keys (union_key: -0.0 below +0.0, NaN fields skipped), one shared word per
+//                 warp and field, double-buffered like the liveness words; warp 0 folds the 16 warps' words behind the next
+//                 round's barrier and writes the record then, so a round still costs one barrier (plus one after the loop
+//                 when it ends at max_per_class).
 constexpr int MERGE_THREADS = 512;
 constexpr int MERGE_MAX = 2 * MERGE_THREADS;   // records of one (image, class) over all views
+constexpr int MERGE_WARPS = MERGE_THREADS / 32;
 static_assert(MERGE_MAX == 1024, "one liveness word per lane: 32 words of 32 candidates");
+enum { MATCH_IOU = 0, MATCH_IOS = 1 };
 
 struct MergeParams {
-    const k2y_det *vdets;   // [n * V][C][K]
-    const int *vcounts;     // [n * V][C]
-    const float *view_yx;   // [n * V][2] (y0, x0)
+    const k2y_det *vdets;   // [N][C][K] records of every view
+    const int *vcounts;     // [N][C]
+    const float *view_yx;   // [N][2] (y0, x0)
+    const int *off;         // [n + 1] first view of image b; null: b * V (uniform ranges)
+    const int *sides;       // [N] interior-side bits (1 top, 2 left, 4 bottom, 8 right); null: no border drop
+    const float *view_hw;   // [N][2] (th, tw), read with `sides`
+    float border;
     int n, V, C, K, nbox;
     float iou;
     k2y_det *dets;
@@ -1024,11 +1045,44 @@ struct MergeParams {
     long long det_stride, cnt_stride;
 };
 
+__device__ __forceinline__ bool ios_norm_gt(const float4 a, float area_a, const float4 b, float area_b, float thr) {
+    if (area_a <= 0.f || area_b <= 0.f) return 0.f > thr;
+    return __fdiv_rn(iou_terms(a, area_a, b, area_b).x, fminf(area_a, area_b)) > thr;
+}
+template <int MATCH>
+__device__ __forceinline__ bool merge_match(const float4 a, float area_a, const float4 b, float area_b, float thr) {
+    if constexpr (MATCH == MATCH_IOS) return ios_norm_gt(a, area_a, b, area_b, thr);
+    else return iou_norm_gt_eo(a, area_a, b, area_b, thr);
+}
+
+// order-preserving key of a non-NaN float (-0.0 below +0.0); a NaN gets the identity `nan_key` of the reduction it enters
+__device__ __forceinline__ unsigned union_key(float f, unsigned nan_key) {
+    const unsigned u = __float_as_uint(f);
+    return f != f ? nan_key : (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float union_field(unsigned key, unsigned nan_key, float own) {
+    return key == nan_key ? own : __uint_as_float((key & 0x80000000u) ? (key & 0x7fffffffu) : ~key);
+}
+
+// UNION: warp 0 writes record `slot`, the kept candidate `o` / `key`, with the union of the extrema its group left in `ext`
+__device__ __forceinline__ void merge_write_union(k2y_det *out, int slot, const float4 o, unsigned long long key, const uint4 *ext,
+                                                  int lane) {
+    const uint4 e = lane < MERGE_WARPS ? ext[lane] : make_uint4(0xffffffffu, 0xffffffffu, 0u, 0u);
+    const unsigned ymin = __reduce_min_sync(FULL, e.x), xmin = __reduce_min_sync(FULL, e.y);
+    const unsigned ymax = __reduce_max_sync(FULL, e.z), xmax = __reduce_max_sync(FULL, e.w);
+    if (lane == 0)
+        write_det(out, slot, make_float4(union_field(ymin, 0xffffffffu, o.x), union_field(xmin, 0xffffffffu, o.y),
+                                         union_field(ymax, 0u, o.z), union_field(xmax, 0u, o.w)), key_score(key), key_index(key));
+}
+
+template <int MATCH, bool UNION>
 __global__ void __launch_bounds__(MERGE_THREADS) merge_views_kernel(const MergeParams p) {
     __shared__ unsigned long long s_keys[MERGE_MAX];   // arrival order (view, then position in the view's list), then sorted
     __shared__ float4 s_box[MERGE_MAX];                // shifted boxes in sorted order
     __shared__ int s_off[MERGE_MAX + 1];               // first arrival position of view v (V <= MERGE_MAX)
     __shared__ unsigned s_alive[2][32];
+    __shared__ uint4 s_ext[UNION ? 2 : 1][MERGE_WARPS];   // UNION: per warp the extrema keys of the round's dying candidates
+    __shared__ int s_drop;
     const int c = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     k2y_det *out = reinterpret_cast<k2y_det *>(reinterpret_cast<int *>(p.dets) + (size_t)b * p.det_stride) + (size_t)c * p.K;
     int *count_out = p.counts + (size_t)b * p.cnt_stride + c;
@@ -1036,16 +1090,18 @@ __global__ void __launch_bounds__(MERGE_THREADS) merge_views_kernel(const MergeP
         if (tid == 0) *count_out = 0;
         return;
     }
-    const size_t view0 = (size_t)b * p.V;
-    for (int v = tid; v < p.V; v += MERGE_THREADS) s_off[v + 1] = min(max(p.vcounts[(view0 + v) * p.C + c], 0), p.K);
+    const size_t view0 = p.off ? (size_t)p.off[b] : (size_t)b * p.V;
+    const int V = p.off ? min(max(p.off[b + 1] - p.off[b], 0), p.V) : p.V;
+    for (int v = tid; v < V; v += MERGE_THREADS) s_off[v + 1] = min(max(p.vcounts[(view0 + v) * p.C + c], 0), p.K);
+    if (tid == 0) s_drop = 0;
     __syncthreads();
     if (tid == 0) {
         s_off[0] = 0;
-        for (int v = 0; v < p.V; ++v) s_off[v + 1] += s_off[v];
+        for (int v = 0; v < V; ++v) s_off[v + 1] += s_off[v];
     }
     __syncthreads();
-    const int n = s_off[p.V];
-    if (n == 0) {
+    const int loaded = s_off[V];
+    if (loaded == 0) {
         if (tid == 0) *count_out = 0;
         return;
     }
@@ -1055,18 +1111,35 @@ __global__ void __launch_bounds__(MERGE_THREADS) merge_views_kernel(const MergeP
 #pragma unroll
     for (int s = 0; s < 2; ++s) {
         const int i = tid + s * MERGE_THREADS, v = i / p.K, k = i - v * p.K;
-        if (v >= p.V || k >= s_off[v + 1] - s_off[v]) continue;
+        if (v >= V || k >= s_off[v + 1] - s_off[v]) continue;
         const k2y_det d = p.vdets[((view0 + v) * p.C + c) * p.K + k];
+        if (p.sides) {
+            const int side = p.sides[view0 + v];
+            const float m = p.border;
+            const bool drop = ((side & 1) && fminf(d.ymin, d.ymax) < m) || ((side & 2) && fminf(d.xmin, d.xmax) < m) ||
+                              ((side & 4) && fmaxf(d.ymin, d.ymax) > __fsub_rn(p.view_hw[2 * (view0 + v)], m)) ||
+                              ((side & 8) && fmaxf(d.xmin, d.xmax) > __fsub_rn(p.view_hw[2 * (view0 + v) + 1], m));
+            if (drop) {
+                s_keys[s_off[v] + k] = 0ull;
+                atomicAdd(&s_drop, 1);
+                continue;
+            }
+        }
         const float y0 = p.view_yx[2 * (view0 + v)], x0 = p.view_yx[2 * (view0 + v) + 1];
         mybox[s] = make_float4(__fadd_rn(d.ymin, y0), __fadd_rn(d.xmin, x0), __fadd_rn(d.ymax, y0), __fadd_rn(d.xmax, x0));
         s_keys[s_off[v] + k] = mykey[s] = pack_key(d.score, v * p.nbox + d.index);
     }
     int P = 32;
-    while (P < n) P <<= 1;
-    for (int i = n + tid; i < P; i += MERGE_THREADS) s_keys[i] = 0ull;
+    while (P < loaded) P <<= 1;
+    for (int i = loaded + tid; i < P; i += MERGE_THREADS) s_keys[i] = 0ull;
     __syncthreads();
+    const int n = loaded - s_drop;   // dropped records are zero keys, sorted behind the n real ones
+    if (n == 0) {
+        if (tid == 0) *count_out = 0;
+        return;
+    }
     if (warp == 0) {
-        if (n <= 32) s_keys[lane] = warp_sort_desc(s_keys[lane], lane);
+        if (P == 32) s_keys[lane] = warp_sort_desc(s_keys[lane], lane);   // every key, dropped ones included, is in s_keys[0, P)
         else warp_sort_desc_mem(s_keys, P, lane);
     }
     __syncthreads();
@@ -1092,7 +1165,7 @@ __global__ void __launch_bounds__(MERGE_THREADS) merge_views_kernel(const MergeP
         alive[s] = pos < n;
         nb[s] = norm_box(alive[s] ? s_box[pos] : make_float4(0.f, 0.f, 0.f, 0.f), ar[s]);
     }
-    int nsel = 0, par = 0;
+    int nsel = 0, par = 0, prev = -1;
     while (nsel < p.K) {
 #pragma unroll
         for (int s = 0; s < 2; ++s) {
@@ -1101,6 +1174,9 @@ __global__ void __launch_bounds__(MERGE_THREADS) merge_views_kernel(const MergeP
         }
         __syncthreads();
         const unsigned word = s_alive[par][lane];
+        if constexpr (UNION) {
+            if (warp == 0 && prev >= 0) merge_write_union(out, nsel - 1, s_box[prev], s_keys[prev], s_ext[par], lane);
+        }
         par ^= 1;
         const unsigned any = __ballot_sync(FULL, word != 0u);
         if (any == 0u) break;
@@ -1109,14 +1185,46 @@ __global__ void __launch_bounds__(MERGE_THREADS) merge_views_kernel(const MergeP
         const float4 ob = s_box[best];
         float ka;
         const float4 kb = norm_box(ob, ka);
-        if (tid == 0) {
-            const unsigned long long k = s_keys[best];
-            write_det(out, nsel, ob, key_score(k), key_index(k));
+        if constexpr (!UNION) {
+            if (tid == 0) {
+                const unsigned long long k = s_keys[best];
+                write_det(out, nsel, ob, key_score(k), key_index(k));
+            }
         }
+        unsigned died = 0u;
 #pragma unroll
-        for (int s = 0; s < 2; ++s)
-            if (alive[s] && (tid + s * MERGE_THREADS == best || iou_norm_gt_eo(kb, ka, nb[s], ar[s], p.iou))) alive[s] = false;
+        for (int s = 0; s < 2; ++s) {
+            if (alive[s] && (tid + s * MERGE_THREADS == best || merge_match<MATCH>(kb, ka, nb[s], ar[s], p.iou))) {
+                alive[s] = false;
+                died |= 1u << s;
+            }
+        }
+        if constexpr (UNION) {
+            uint4 e = make_uint4(0xffffffffu, 0xffffffffu, 0u, 0u);
+#pragma unroll
+            for (int s = 0; s < 2; ++s) {
+                if (died & (1u << s)) {
+                    const float4 r = s_box[tid + s * MERGE_THREADS];
+                    e.x = min(e.x, union_key(r.x, 0xffffffffu));
+                    e.y = min(e.y, union_key(r.y, 0xffffffffu));
+                    e.z = max(e.z, union_key(r.z, 0u));
+                    e.w = max(e.w, union_key(r.w, 0u));
+                }
+            }
+            e.x = __reduce_min_sync(FULL, e.x);
+            e.y = __reduce_min_sync(FULL, e.y);
+            e.z = __reduce_max_sync(FULL, e.z);
+            e.w = __reduce_max_sync(FULL, e.w);
+            if (lane == 0) s_ext[par][warp] = e;   // read behind the next round's barrier
+            prev = best;
+        }
         ++nsel;
+    }
+    if constexpr (UNION) {
+        if (nsel == p.K) {   // the loop ended at max_per_class, not at a barrier: the last round's extrema need one
+            __syncthreads();
+            if (warp == 0) merge_write_union(out, nsel - 1, s_box[prev], s_keys[prev], s_ext[par], lane);
+        }
     }
     if (tid == 0) *count_out = nsel;
 }
@@ -1276,45 +1384,83 @@ extern "C" int k2y_detect_keras_strided(const k2y_detect_cfg *cfg, const float *
 
 extern "C" int k2y_merge_views_max_records(void) { return MERGE_MAX; }
 
-extern "C" int k2y_merge_views(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev, int n_images,
-                               int rows, int views, int n_boxes, int class_num, int max_per_class, float iou_thresh, k2y_det *dets_dev,
-                               int32_t *counts_dev, long long det_image_stride_words, long long count_image_stride_words,
-                               void *stream) {
+namespace {
+int merge_views_launch(const char *fn, const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev,
+                       const int32_t *view_offsets_dev, const int32_t *view_sides_dev, const float *view_hw_dev, float border,
+                       int match, int merge, int n_images, int rows, int max_views, int n_boxes, int class_num, int max_per_class,
+                       float thresh, k2y_det *dets_dev, int32_t *counts_dev, long long det_image_stride_words,
+                       long long count_image_stride_words, void *stream) {
     if (!view_dets_dev || !view_counts_dev || !view_yx_dev || !dets_dev || !counts_dev || n_images < 0 || rows < 1 || rows < n_images ||
-        views < 1 || n_boxes < 1 || class_num < 1 || class_num > 65535 || max_per_class < 1) {
-        set_error("k2y_merge_views: null pointer, or not 0 <= n_images <= rows, rows, views, n_boxes, max_per_class >= 1, class_num 1..65535");
+        max_views < 1 || n_boxes < 1 || class_num < 1 || class_num > 65535 || max_per_class < 1) {
+        set_error("%s: null pointer, or not 0 <= n_images <= rows, rows, views, n_boxes, max_per_class >= 1, class_num 1..65535", fn);
         return K2Y_ERR_INVALID;
     }
-    if ((long long)views * max_per_class > MERGE_MAX) {
-        set_error("k2y_merge_views: %d views x %d records per class exceed the %d records one merge holds", views, max_per_class,
-                  MERGE_MAX);
+    if ((match != K2Y_MATCH_IOU && match != K2Y_MATCH_IOS) || (merge != K2Y_MERGE_SUPPRESS && merge != K2Y_MERGE_UNION)) {
+        set_error("%s: unknown match metric %d or merge action %d", fn, match, merge);
         return K2Y_ERR_INVALID;
     }
-    if ((long long)views * n_boxes > 0x7fffffffLL) {
-        set_error("k2y_merge_views: view * n_boxes + index does not fit the record's int32 index (%d views x %d boxes)", views, n_boxes);
+    if (view_sides_dev && (!view_hw_dev || !(border >= 0.f))) {
+        set_error("%s: a border drop needs the views' sizes and a border >= 0 (got %g)", fn, (double)border);
+        return K2Y_ERR_INVALID;
+    }
+    if ((long long)max_views * max_per_class > MERGE_MAX) {
+        set_error("%s: %d views x %d records per class exceed the %d records one merge holds", fn, max_views, max_per_class, MERGE_MAX);
+        return K2Y_ERR_INVALID;
+    }
+    if ((long long)max_views * n_boxes > 0x7fffffffLL) {
+        set_error("%s: view * n_boxes + index does not fit the record's int32 index (%d views x %d boxes)", fn, max_views, n_boxes);
         return K2Y_ERR_INVALID;
     }
     if (det_image_stride_words < (long long)class_num * max_per_class * 6 || count_image_stride_words < class_num) {
-        set_error("k2y_merge_views: image strides smaller than one image's records / counts");
+        set_error("%s: image strides smaller than one image's records / counts", fn);
         return K2Y_ERR_INVALID;
     }
     MergeParams p;
     p.vdets = view_dets_dev;
     p.vcounts = view_counts_dev;
     p.view_yx = view_yx_dev;
+    p.off = view_offsets_dev;
+    p.sides = view_sides_dev;
+    p.view_hw = view_hw_dev;
+    p.border = border;
     p.n = n_images;
-    p.V = views;
+    p.V = max_views;
     p.C = class_num;
     p.K = max_per_class;
     p.nbox = n_boxes;
-    p.iou = iou_thresh;
+    p.iou = thresh;
     p.dets = dets_dev;
     p.counts = counts_dev;
     p.det_stride = det_image_stride_words;
     p.cnt_stride = count_image_stride_words;
-    merge_views_kernel<<<dim3(class_num, rows), MERGE_THREADS, 0, (cudaStream_t)stream>>>(p);
+    const dim3 grid(class_num, rows);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (match == K2Y_MATCH_IOU && merge == K2Y_MERGE_SUPPRESS) merge_views_kernel<MATCH_IOU, false><<<grid, MERGE_THREADS, 0, st>>>(p);
+    else if (match == K2Y_MATCH_IOU) merge_views_kernel<MATCH_IOU, true><<<grid, MERGE_THREADS, 0, st>>>(p);
+    else if (merge == K2Y_MERGE_SUPPRESS) merge_views_kernel<MATCH_IOS, false><<<grid, MERGE_THREADS, 0, st>>>(p);
+    else merge_views_kernel<MATCH_IOS, true><<<grid, MERGE_THREADS, 0, st>>>(p);
     K2Y_CUDA_CHECK(cudaGetLastError());
     return K2Y_OK;
+}
+}  // namespace
+
+extern "C" int k2y_merge_views_ex(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev,
+                                  const int32_t *view_offsets_dev, const int32_t *view_sides_dev, const float *view_hw_dev,
+                                  float border, int match, int merge, int n_images, int rows, int max_views, int n_boxes,
+                                  int class_num, int max_per_class, float thresh, k2y_det *dets_dev, int32_t *counts_dev,
+                                  long long det_image_stride_words, long long count_image_stride_words, void *stream) {
+    return merge_views_launch("k2y_merge_views_ex", view_dets_dev, view_counts_dev, view_yx_dev, view_offsets_dev, view_sides_dev,
+                              view_hw_dev, border, match, merge, n_images, rows, max_views, n_boxes, class_num, max_per_class, thresh,
+                              dets_dev, counts_dev, det_image_stride_words, count_image_stride_words, stream);
+}
+
+extern "C" int k2y_merge_views(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev, int n_images,
+                               int rows, int views, int n_boxes, int class_num, int max_per_class, float iou_thresh, k2y_det *dets_dev,
+                               int32_t *counts_dev, long long det_image_stride_words, long long count_image_stride_words,
+                               void *stream) {
+    return merge_views_launch("k2y_merge_views", view_dets_dev, view_counts_dev, view_yx_dev, nullptr, nullptr, nullptr, -1.f, K2Y_MATCH_IOU,
+                              K2Y_MERGE_SUPPRESS, n_images, rows, views, n_boxes, class_num, max_per_class, iou_thresh, dets_dev,
+                              counts_dev, det_image_stride_words, count_image_stride_words, stream);
 }
 
 // Parity hook: the two pinned float32 exponentials, element-wise on device arrays.

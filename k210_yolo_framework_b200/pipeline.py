@@ -28,7 +28,10 @@ slot waits for the render before it overwrites the originals.
 ``enable_tiling`` makes ``submit_images`` detect on overlapping tiles of each image as well as on the whole image: a batch of
 n <= batch // V images is letterboxed as n * V views, the network and the decode run on those, and one more per-class NMS
 (``k2y_merge_views``, on the decode stream) merges each image's views into rows [0, n) of the gather slot, in image
-coordinates and in the usual block format, so everything behind it is unchanged.
+coordinates and in the usual block format, so everything behind it is unchanged.  With ``tile_size`` each image gets its own
+grid (``tiles.plan_grid``) and ``images_per_batch`` is the caller's; ``k2y_merge_views_ex`` then reads each image's view range
+and the windows' interior sides from a table that travels in the batch's H2D copy, and can match by intersection over the
+smaller box, fold the matched boxes into the kept one and drop records at the tiles' inner borders.
 
 ``enable_png_decode`` makes ``submit_images`` decode the PNG files the GPU takes there too (``preprocess.png_gpu_decodable``),
 in the same staging range and H2D copy as the batch's JPEGs; their status words travel beside the JPEGs'.
@@ -43,7 +46,7 @@ import ctypes
 import numpy as np
 import torch
 
-from . import yolonet
+from . import tiles, yolonet
 from ._lib import check, lib
 from .detect import DET_WORDS, KerasDetector
 from .dist import DetectionGather
@@ -107,20 +110,26 @@ class DetectionPipeline:
         self._render_done = [torch.cuda.Event() for _ in range(SLOTS)]   # files of gather slot ready to copy back
         self._render_free = [torch.cuda.Event() for _ in range(SLOTS)]   # render + encode finished with input slot's originals
         self._rendered_slot: List[bool] = [False] * SLOTS
-        # enable_tiling: (rows, cols, overlap), views per image, the per-view record block the decode writes and the merge reads
-        # (both on the decode stream, so one block serves every batch) and per input slot the device (y0, x0) of its views
+        # enable_tiling: (rows, cols, overlap) or a tiles.SizedTiling, the most views of an image, images per batch, the merge's
+        # options (None: k2y_merge_views), the per-view record block the decode writes and the merge reads (both on the decode
+        # stream, so one block serves every batch) and per input slot the device (y0, x0) of its views
         self._tiling = None
         self._views = 1
+        self._ipb = self.batch
+        self._merge = None
         self._view_dets: Optional[torch.Tensor] = None
         self._view_counts: Optional[torch.Tensor] = None
         self._slot_yx: Optional[List[torch.Tensor]] = None
 
     @property
     def images_per_batch(self) -> int:
-        """Images one ``submit_images`` takes: ``batch``, or ``batch // V`` with tiling."""
-        return self.batch // self._views
+        """Images one ``submit_images`` takes: ``batch``, ``batch // V`` with a rows x cols tiling, or the value given with
+        ``tile_size``."""
+        return self._ipb
 
-    def enable_tiling(self, rows: int, cols: int, overlap: float = 0.2) -> None:
+    def enable_tiling(self, rows: Optional[int] = None, cols: Optional[int] = None, overlap: float = 0.2, *, tile_size=None,
+                      images_per_batch: Optional[int] = None, match: str = "iou", merge: str = "suppress",
+                      match_thresh: Optional[float] = None, border: Optional[float] = None) -> None:
         """From now on ``submit_images`` detects every image as V = 1 + rows * cols views: the whole image and rows x cols
         overlapping tiles of it (``tiles.tile_windows``), each letterboxed and decoded as the crop submitted as an image of
         its own would be.  A batch holds at most ``images_per_batch`` = batch // V images; their n * V views fill the input
@@ -128,20 +137,67 @@ class DetectionPipeline:
         coordinates, ``index = view * nbox + index`` (``index // nbox`` tells the view), one more greedy NMS per class over
         the union.  ``collect`` returns the merged records in the usual format; rendering, the all-gather (rank r's images
         from row r * batch) and the flow control are unchanged.  Raises ``ValueError`` when V exceeds the batch or
-        V * max_per_class exceeds what one merge holds (``k2y_merge_views_max_records``)."""
-        rows, cols = int(rows), int(cols)
-        if rows < 1 or cols < 1:
-            raise ValueError(f"tiling {rows}x{cols}: at least one tile per axis")
+        V * max_per_class exceeds what one merge holds (``k2y_merge_views_max_records``).
+
+        ``tile_size=(th, tw)`` instead of rows and cols plans each image's grid from its own size (``tiles.plan_grid``): tiles
+        of at most th x tw pixels, one view for an image that fits one tile, and at most ``max_views`` = min(batch //
+        images_per_batch, k2y_merge_views_max_records() // max_per_class) views, so that a batch of `images_per_batch` images
+        (required here, refused without tile_size) always fits.  Images' view ranges differ, and ``k2y_merge_views_ex`` merges
+        them.  With either grid:
+          `match`         "iou" (the default) or "ios": a candidate matches a kept record when their IoU, or their
+                          intersection over the smaller box, exceeds `match_thresh` (default: the detector's iou_thresh);
+          `merge`         "suppress" (the default) drops a matching candidate, "union" also grows the kept record's box to the
+                          field-wise union of itself and the candidates it suppressed (score and index stay its own);
+          `border`        None (the default) or m >= 0: a tile's record within m pixels of a tile edge that lies inside the
+                          image is dropped before the merge (oracle/tiles_merge_ref.py states each rule exactly).
+        With none of these set, the merge is ``k2y_merge_views`` exactly.  Bad values raise ``ValueError`` and leave the
+        pipeline as it was."""
+        limit = int(lib.k2y_merge_views_max_records())
+        if match not in tiles.MATCHES:
+            raise ValueError(f"unknown match metric {match!r}: one of {', '.join(tiles.MATCHES)}")
+        if merge not in tiles.MERGES:
+            raise ValueError(f"unknown merge action {merge!r}: one of {', '.join(tiles.MERGES)}")
+        if border is not None and not float(border) >= 0:
+            raise ValueError(f"tile border {border}: at least 0 pixels")
         if not 0 <= overlap < 1:
             raise ValueError(f"tile overlap {overlap} is outside [0, 1)")
-        V = 1 + rows * cols
-        if V > self.batch:
-            raise ValueError(f"{V} views per image do not fit a batch of {self.batch}")
-        limit = int(lib.k2y_merge_views_max_records())
-        if V * self.gather.K > limit:
-            raise ValueError(f"{V} views x {self.gather.K} records per class exceed the {limit} records one merge holds")
+        if tile_size is None:
+            if rows is None or cols is None:
+                raise ValueError("enable_tiling needs rows and cols, or tile_size")
+            if images_per_batch is not None:
+                raise ValueError("images_per_batch goes with tile_size; a rows x cols grid holds batch // (1 + rows * cols) images")
+            rows, cols = int(rows), int(cols)
+            if rows < 1 or cols < 1:
+                raise ValueError(f"tiling {rows}x{cols}: at least one tile per axis")
+            V = 1 + rows * cols
+            if V > self.batch:
+                raise ValueError(f"{V} views per image do not fit a batch of {self.batch}")
+            if V * self.gather.K > limit:
+                raise ValueError(f"{V} views x {self.gather.K} records per class exceed the {limit} records one merge holds")
+            tiling, ipb = (rows, cols, overlap), self.batch // V
+        else:
+            if rows is not None or cols is not None:
+                raise ValueError("enable_tiling takes rows and cols, or tile_size, not both")
+            if images_per_batch is None:
+                raise ValueError("tile_size needs images_per_batch: the images one batch holds whatever their grids")
+            th, tw = (int(v) for v in tile_size)
+            if th < 1 or tw < 1:
+                raise ValueError(f"tile size {th}x{tw}: at least one pixel per side")
+            ipb = int(images_per_batch)
+            if not 1 <= ipb <= self.batch:
+                raise ValueError(f"images_per_batch {ipb} is outside 1..{self.batch}")
+            V = min(self.batch // ipb, limit // self.gather.K)
+            if V < 1:
+                raise ValueError(f"no view fits: {self.gather.K} records per class exceed the {limit} records one merge holds")
+            tiling = tiles.SizedTiling((th, tw), overlap, V)
+        options = dict(match=match, merge=merge, match_thresh=match_thresh, border=border)
+        legacy = tile_size is None and options == dict(match="iou", merge="suppress", match_thresh=None, border=None)
         dev = torch.device("cuda", self.device_index)
-        self._tiling, self._views = (rows, cols, overlap), V
+        self._tiling, self._views, self._ipb = tiling, V, ipb
+        self._merge = None if legacy else dict(
+            match=tiles.MATCHES.index(match), merge=tiles.MERGES.index(merge),
+            thresh=float(self.detector.cfg.iou_thresh if match_thresh is None else match_thresh),
+            border=None if border is None else float(border))
         self._nbox = sum(h * w for h, w in self.detector.out_hw) * self.detector.A      # boxes of one network input
         self._view_dets = torch.zeros((self.batch, self.gather.C, self.gather.K, DET_WORDS), dtype=torch.int32, device=dev)
         self._view_counts = torch.zeros((self.batch, self.gather.C), dtype=torch.int32, device=dev)
@@ -165,11 +221,12 @@ class DetectionPipeline:
         self._img_hw.copy_(torch.from_numpy(np.array(arr, dtype=np.float32, order="C", copy=True)))
 
     # -- device-resident step ---------------------------------------------------------------------------------------
-    def _step(self, n: int, image_hw: Optional[torch.Tensor] = None, view_yx: Optional[torch.Tensor] = None) -> int:
+    def _step(self, n: int, image_hw: Optional[torch.Tensor] = None, view_yx: Optional[torch.Tensor] = None, table=None) -> int:
         """Network on the current stream into head set s, decode/NMS on the decode stream into gather slot s, then
         (world > 1) the all-gather on the side stream.  `image_hw`: device [n, 2] original sizes (default: the shared
         ``set_image_shapes`` tensor).  With `view_yx` (device [n, 2] origins) the n inputs are the views of n // V images: the
-        decode writes the per-view block and the merge writes the gather slot.  Returns s."""
+        decode writes the per-view block and the merge writes the gather slot.  `table` = (device address of the view offsets,
+        of the view sides, images) switches to ``k2y_merge_views_ex`` with the tiling's options.  Returns s."""
         s = self._steps % SLOTS
         self._steps += 1
         compute = torch.cuda.current_stream(self.device_index)
@@ -186,6 +243,16 @@ class DetectionPipeline:
         dets, counts = self.gather.local(s)
         if view_yx is None:
             self.detector.run(heads, self._img_hw[:n] if image_hw is None else image_hw, dets_out=dets, counts_out=counts, stream=det)
+        elif table is not None:
+            self.detector.run(heads, image_hw, dets_out=self._view_dets, counts_out=self._view_counts, stream=det)
+            m = self._merge
+            off, sides, n_images = table
+            bordered = m["border"] is not None
+            check(lib.k2y_merge_views_ex(self._view_dets.data_ptr(), self._view_counts.data_ptr(), view_yx.data_ptr(), off,
+                                         sides if bordered else None, image_hw.data_ptr() if bordered else None,
+                                         m["border"] if bordered else -1.0, m["match"], m["merge"], n_images, self.batch, self._views,
+                                         self._nbox, self.gather.C, self.gather.K, m["thresh"], dets.data_ptr(), counts.data_ptr(),
+                                         dets.stride(0), counts.stride(0), ctypes.c_void_p(det.cuda_stream)))
         else:
             self.detector.run(heads, image_hw, dets_out=self._view_dets, counts_out=self._view_counts, stream=det)
             check(lib.k2y_merge_views(self._view_dets.data_ptr(), self._view_counts.data_ptr(), view_yx.data_ptr(), n // self._views,
@@ -311,7 +378,8 @@ class DetectionPipeline:
         before anything is enqueued."""
         if self._tiling is not None and isinstance(images, (list, tuple)) and len(images) > self.images_per_batch:
             raise ValueError(f"{len(images)} images of {self._views} views do not fit a batch of {self.batch}")
-        layout = BatchLayout(images, self.in_hw, self._tiling, gpu_png=self._gpu_png, gpu_progressive=self._gpu_progressive)
+        layout = BatchLayout(images, self.in_hw, self._tiling, gpu_png=self._gpu_png, gpu_progressive=self._gpu_progressive,
+                             merge_table=self._merge is not None)
         n = len(layout)
         if n > self.batch:
             raise ValueError(f"{n} images do not fit a batch of {self.batch}")
@@ -349,9 +417,13 @@ class DetectionPipeline:
                 with torch.cuda.stream(self._copy_stream):
                     self._prog_status[s][:np_].copy_(self._staging[slot].progressive_status[:np_], non_blocking=True)
         self._h2d_done[slot].record(self._copy_stream)
-        nv = n * layout.views
+        nv = layout.n_views
+        table = None
+        if layout.merge_table_at is not None:     # the view offsets and sides, where the H2D copy put them
+            at = self._staging[slot].dev.data_ptr() + layout.merge_table_at
+            table = (at, at + 4 * (n + 1), n)
         t = self._run_slot(slot, buf, nv, self._slot_hw[slot][:nv], n if self.world == 1 else None,
-                           self._slot_yx[slot][:nv] if self._tiling is not None else None)
+                           self._slot_yx[slot][:nv] if self._tiling is not None else None, table)
         self._rendered_slot[t] = self._render is not None
         if self._render is not None:
             with torch.cuda.device(dev):
@@ -359,12 +431,12 @@ class DetectionPipeline:
         return t
 
     def _run_slot(self, slot: int, buf: torch.Tensor, n: int, image_hw: Optional[torch.Tensor], rows: Optional[int],
-                  view_yx: Optional[torch.Tensor] = None) -> int:
+                  view_yx: Optional[torch.Tensor] = None, table=None) -> int:
         """Network + decode (+ all-gather) of input slot `slot` once its H2D is done, then the D2H of the records."""
         compute = torch.cuda.current_stream(self.device_index)
         compute.wait_event(self._h2d_done[slot])
         self.engine.bind_input(buf)
-        s = self._step(n, image_hw, view_yx)
+        s = self._step(n, image_hw, view_yx, table)
         self._in_free[slot].record(compute)
         self._hw_free[slot].record(self._det_stream)
         self._rows[s] = rows
@@ -518,10 +590,13 @@ class LanedPipeline:
         for ln in self.lanes:
             ln.enable_progressive_jpeg_decode()
 
-    def enable_tiling(self, rows: int, cols: int, overlap: float = 0.2) -> None:
+    def enable_tiling(self, rows: Optional[int] = None, cols: Optional[int] = None, overlap: float = 0.2, *, tile_size=None,
+                      images_per_batch: Optional[int] = None, match: str = "iou", merge: str = "suppress",
+                      match_thresh: Optional[float] = None, border: Optional[float] = None) -> None:
         """``DetectionPipeline.enable_tiling`` on every lane."""
         for ln in self.lanes:
-            ln.enable_tiling(rows, cols, overlap)
+            ln.enable_tiling(rows, cols, overlap, tile_size=tile_size, images_per_batch=images_per_batch, match=match, merge=merge,
+                             match_thresh=match_thresh, border=border)
 
     @property
     def images_per_batch(self) -> int:

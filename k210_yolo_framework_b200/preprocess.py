@@ -38,7 +38,7 @@ import torch
 
 from ._lib import JpegInfo, JpegProgressiveInfo, K2YError, PngInfo, check, lib
 from .helper import read_image
-from .tiles import tile_windows
+from .tiles import tile_windows, view_sides
 
 
 def letterbox_params(img_hw, in_hw):
@@ -250,9 +250,16 @@ class BatchLayout:
     With `tiling` = (rows, cols, overlap) every image is letterboxed as V = 1 + rows * cols views (``tiles.tile_windows``:
     the whole image, then its tiles): ``views`` = V, ``windows`` int32 [n * V, 4] (y0, x0, th, tw) and ``view_matrices``
     float64 [n * V, 6] (each window's own ``letterbox_params`` matrix), image-major.  Everything above stays per image: staging,
-    the JPEG decode and the renderer see the originals."""
+    the JPEG decode and the renderer see the originals.  `tiling` may also be a ``tiles.SizedTiling``, whose grid is planned
+    per image (``tiles.plan_windows``); ``views`` is then None.  Either way ``view_counts`` int32 [n] holds each image's number
+    of views, ``view_offsets`` int32 [n + 1] their running sum (image b's views are ``windows[view_offsets[b]:view_offsets[b+1]]``)
+    and ``view_sides`` int32 [N] each window's interior sides (``tiles.view_sides``).
 
-    def __init__(self, images: Sequence, in_hw, tiling=None, gpu_png: bool = False, gpu_progressive: bool = False):
+    With `merge_table` (and a tiling) ``view_offsets`` and ``view_sides`` also go into the staging buffer, behind everything
+    else, at ``merge_table_at``, so that the batch's H2D copy takes them to the device for ``k2y_merge_views_ex``."""
+
+    def __init__(self, images: Sequence, in_hw, tiling=None, gpu_png: bool = False, gpu_progressive: bool = False,
+                 merge_table: bool = False):
         _check_images(images)
         n = len(images)
         self.in_hw = (int(in_hw[0]), int(in_hw[1]))
@@ -285,13 +292,23 @@ class BatchLayout:
         self.nbytes = int(padded.sum())
         self.matrices = np.array([letterbox_params((int(h[0]), int(h[1])), self.in_hw)[2][:2].reshape(-1) for h in self.hw], dtype=np.float64)
         self.views, self.windows, self.view_matrices = 1, None, None
+        self.view_counts, self.view_offsets, self.view_sides = None, None, None
         if tiling is not None:
-            rows, cols, overlap = tiling
+            if isinstance(tiling, (tuple, list)):
+                rows, cols, overlap = tiling
+                what = f"tiling {rows}x{cols}"
+                plan = lambda h, w: tile_windows(h, w, rows, cols, overlap)     # noqa: E731
+            else:
+                what, plan = f"tiling by {tiling.tile_hw[0]}x{tiling.tile_hw[1]} tiles", tiling.windows
             try:
-                self.windows = np.concatenate([tile_windows(int(h), int(w), rows, cols, overlap) for h, w in self.hw])
+                per_image = [plan(int(h), int(w)) for h, w in self.hw]
             except ValueError as e:
-                raise ValueError(f"tiling {rows}x{cols}: {e}") from e
-            self.views = len(self.windows) // n
+                raise ValueError(f"{what}: {e}") from e
+            self.windows = np.concatenate(per_image)
+            self.view_counts = np.array([len(w) for w in per_image], np.int32)
+            self.view_offsets = np.concatenate([[0], np.cumsum(self.view_counts)]).astype(np.int32)
+            self.view_sides = np.concatenate([view_sides(w, int(h), int(wd)) for w, (h, wd) in zip(per_image, self.hw)])
+            self.views = len(self.windows) // n if isinstance(tiling, (tuple, list)) else None
             self.view_matrices = np.array([letterbox_params((int(t[2]), int(t[3])), self.in_hw)[2][:2].reshape(-1) for t in self.windows],
                                           dtype=np.float64)
         self.jpeg_plan = None
@@ -312,6 +329,16 @@ class BatchLayout:
             self.progressive_plan = _jpeg_layout([f for _, f in self.progressive], self.progressive_dst,
                                                  (self.staged_end + ALIGN - 1) // ALIGN * ALIGN, _progressive_plan)
             self.staged_end = self.progressive_plan[3]
+        self.merge_table_at = None
+        if merge_table and self.windows is not None:
+            self.merge_table = np.concatenate([self.view_offsets, self.view_sides]).astype(np.int32)
+            self.merge_table_at = (self.staged_end + ALIGN - 1) // ALIGN * ALIGN
+            self.staged_end = self.merge_table_at + self.merge_table.nbytes
+
+    @property
+    def n_views(self) -> int:
+        """Network inputs of the batch: one per image, or every image's views with a tiling."""
+        return len(self.hw) if self.windows is None else len(self.windows)
 
     def __len__(self) -> int:
         return len(self.hw)
@@ -521,18 +548,26 @@ def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, ou
     into ``image_hw_out[:n]``), all on ``staging.stream``.  GPU-decodable JPEGs travel compressed behind the packed pixels and
     are decoded into their place first (``stage_jpegs``), and so are the layout's GPU PNGs, whose range the same H2D copy moves
     (``stage_pngs``).  The host buffer is reused by the next call: wait for this copy
-    before packing into it again.  A layout with tiling letterboxes its n * V views instead (``k2y_letterbox_u8_views``),
-    image-major: ``out[:n * V]``, each view's (th, tw) into ``image_hw_out[:n * V]`` and its (y0, x0) into
-    ``view_yx_out[:n * V]`` (float32 [N, 2])."""
+    before packing into it again.  A layout with tiling letterboxes its N = ``layout.n_views`` views instead
+    (``k2y_letterbox_u8_views``), image-major: ``out[:N]``, each view's (th, tw) into ``image_hw_out[:N]`` and its (y0, x0) into
+    ``view_yx_out[:N]`` (float32 [N, 2]); a layout's merge table goes to ``staging.dev`` at ``layout.merge_table_at`` in the
+    same H2D copy as the rest."""
     n = len(layout)
-    staging.reserve(layout.staged_end, n * layout.views)
+    staging.reserve(layout.staged_end, layout.n_views)
     layout.pack(images, staging.host.numpy())
+    ranges = layout.host_ranges()
+    table = layout.merge_table_at is not None
+    if table:       # the merge table rides along with the last H2D copy: the decoders' range, else the last host range
+        at = layout.merge_table_at
+        staging.host.numpy()[at:at + layout.merge_table.nbytes] = layout.merge_table.view(np.uint8)
+        if not (layout.jpeg or layout.png or layout.progressive):
+            ranges[-1] = (ranges[-1][0], layout.staged_end)
     in_h, in_w = layout.in_hw
     st = staging.stream
     with torch.cuda.stream(st):
-        for b, e in layout.host_ranges():
+        for b, e in ranges:
             staging.dev[b:e].copy_(staging.host[b:e], non_blocking=True)
-        if layout.png or layout.progressive:   # every decoder's files and blobs in one H2D copy, then the decodes
+        if layout.png or layout.progressive or (layout.jpeg and table):   # every decoder's files and blobs in one H2D copy
             decodes = [_fill(k, [f for _, f in files], dst, staging, plan) for k, files, dst, plan in
                        (("jpeg", layout.jpeg, getattr(layout, "jpeg_dst", None), layout.jpeg_plan),
                         ("png", layout.png, getattr(layout, "png_dst", None), layout.png_plan),
@@ -546,10 +581,9 @@ def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, ou
             stage_jpegs([f for _, f in layout.jpeg], layout.jpeg_dst, staging, layout.jpeg_plan, staging.dev)
         offs = layout.offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong))
         if layout.windows is not None:
-            V = layout.views
-            offsets = np.repeat(layout.offsets, V)
-            hw = np.ascontiguousarray(np.repeat(layout.hw, V, axis=0))
-            check(lib.k2y_letterbox_u8_views(staging.dev.data_ptr(), n * V, offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
+            offsets = np.repeat(layout.offsets, layout.view_counts)
+            hw = np.ascontiguousarray(np.repeat(layout.hw, layout.view_counts, axis=0))
+            check(lib.k2y_letterbox_u8_views(staging.dev.data_ptr(), layout.n_views, offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
                                              hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
                                              layout.windows.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
                                              layout.view_matrices.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), out.data_ptr(), in_h,

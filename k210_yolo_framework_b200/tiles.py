@@ -6,6 +6,9 @@ in row-major order.  One axis of length ``L`` cut into ``k`` tiles with overlap 
 first tile starts at 0 and the last ends at ``L``.  The arithmetic is exact (``fractions.Fraction``; a float ``f`` is the rational
 it stores), so no rounding depends on the platform.  ``DetectionPipeline.enable_tiling`` runs the views through the network and
 ``k2y_merge_views`` merges their records.
+
+``plan_grid`` / ``plan_windows`` choose an image's grid from a tile size instead (``enable_tiling(tile_size=...)``), and
+``view_sides`` tells which edges of each window lie inside the image, for the border drop of ``k2y_merge_views_ex``.
 """
 from __future__ import annotations
 
@@ -34,3 +37,74 @@ def tile_windows(h: int, w: int, rows: int, cols: int, overlap=0.2) -> np.ndarra
     ``ValueError`` for rows or cols below 1, an overlap outside [0, 1) or an image with fewer rows / columns than tiles."""
     ys, xs = axis_tiles(h, rows, overlap), axis_tiles(w, cols, overlap)
     return np.array([(0, 0, int(h), int(w))] + [(y0, x0, th, tw) for y0, th in ys for x0, tw in xs], dtype=np.int32)
+
+
+def view_count(rows: int, cols: int) -> int:
+    """Views of an image cut rows x cols: one (the whole image) for 1x1, else the whole image and its rows * cols tiles."""
+    return 1 if rows * cols == 1 else 1 + rows * cols
+
+
+def axis_count(length: int, tile: int, overlap) -> int:
+    """Tiles of one axis of `length` pixels for a target tile length `tile`: the least k in 1..length whose tiles
+    (``axis_tiles``) are at most `tile` long, or `length` if there is none.  ``t(k) = ceil(L / (k (1 - f) + f))`` falls with k,
+    so k is the least one with ``k (1 - f) + f >= L / T``."""
+    length, tile = int(length), int(tile)
+    f = Fraction(overlap)
+    if length <= tile:
+        return 1
+    return min(length, max(1, math.ceil((Fraction(length, tile) - f) / (1 - f))))
+
+
+def plan_grid(h: int, w: int, tile_hw, overlap, max_views: int) -> tuple:
+    """(rows, cols) of an h x w image cut into tiles of at most tile_hw = (th, tw) pixels (``axis_count`` per axis), then,
+    while the image has more than `max_views` views (``view_count``), one tile fewer on the axis with more tiles (on a tie, the
+    rows).  1x1 is one view, so the loop ends there at the latest.  ``ValueError`` for a tile side below 1, an overlap
+    outside [0, 1) or `max_views` below 1."""
+    th, tw, max_views = int(tile_hw[0]), int(tile_hw[1]), int(max_views)
+    if th < 1 or tw < 1:
+        raise ValueError(f"tile size {th}x{tw}: at least one pixel per side")
+    if not 0 <= Fraction(overlap) < 1:
+        raise ValueError(f"tile overlap {overlap} is outside [0, 1)")
+    if max_views < 1:
+        raise ValueError(f"at most {max_views} views per image: at least one is needed")
+    rows, cols = axis_count(h, th, overlap), axis_count(w, tw, overlap)
+    while view_count(rows, cols) > max_views:
+        if rows >= cols:
+            rows -= 1
+        else:
+            cols -= 1
+    return rows, cols
+
+
+def plan_windows(h: int, w: int, tile_hw, overlap, max_views: int) -> np.ndarray:
+    """int32 [V, 4] windows of an h x w image under ``plan_grid``: the whole image alone for a 1x1 grid, else
+    ``tile_windows``."""
+    rows, cols = plan_grid(h, w, tile_hw, overlap, max_views)
+    if rows * cols == 1:
+        return np.array([(0, 0, int(h), int(w))], dtype=np.int32)
+    return tile_windows(h, w, rows, cols, overlap)
+
+
+def view_sides(windows: np.ndarray, h: int, w: int) -> np.ndarray:
+    """int32 [V] interior-side bits of an h x w image's windows: 1 top (y0 > 0), 2 left (x0 > 0), 4 bottom (y0 + th < h),
+    8 right (x0 + tw < w).  The merge's border drop tests a record only against the sides whose bit is set; the whole image
+    has none."""
+    win = np.asarray(windows, np.int64).reshape(-1, 4)
+    y0, x0, th, tw = win[:, 0], win[:, 1], win[:, 2], win[:, 3]
+    return ((y0 > 0) * 1 + (x0 > 0) * 2 + (y0 + th < h) * 4 + (x0 + tw < w) * 8).astype(np.int32)
+
+
+MATCHES = ("iou", "ios")
+MERGES = ("suppress", "union")
+
+
+class SizedTiling:
+    """A per-image grid: every image is cut into tiles of at most `tile_hw` pixels (``plan_windows``), with at most
+    `max_views` views.  ``BatchLayout`` takes it where it takes (rows, cols, overlap)."""
+
+    def __init__(self, tile_hw, overlap, max_views: int):
+        plan_grid(1, 1, tile_hw, overlap, max_views)        # validates the arguments
+        self.tile_hw, self.overlap, self.max_views = (int(tile_hw[0]), int(tile_hw[1])), overlap, int(max_views)
+
+    def windows(self, h: int, w: int) -> np.ndarray:
+        return plan_windows(h, w, self.tile_hw, self.overlap, self.max_views)

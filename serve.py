@@ -22,6 +22,8 @@ give; only the compressed files come back.  Duplicate stems are refused before a
 With --tiles ROWS COLS every image is detected on ROWS x COLS overlapping tiles as well as whole (--tile_overlap, default 0.2;
 DetectionPipeline.enable_tiling): a batch then holds batch // (1 + ROWS * COLS) images, the views' records are merged on the GPU
 and the lines keep their shape, with "index" // (boxes per network input) telling the view a detection came from.
+--tile_size H W --tile_images N plans each image's grid from its own size instead (tiles of at most H x W pixels, a batch of N
+images); --tile_match ios, --tile_merge union and --tile_border PX change how the views' records are merged (either grid).
 
 With --gpu_png the PNG files the GPU decoder takes (preprocess.png_gpu_decodable) stay compressed too and are decoded on the GPU
 (DetectionPipeline.enable_png_decode), with the pixels PIL gives; the lines are the same as without it.  --gpu_progressive does
@@ -80,8 +82,12 @@ def open_pipeline(args, max_per_class=30):
     pipe = DetectionPipeline(args.model_def, tuple(args.image_size), anchors, args.class_num, args.depth_multiplier, args.batch,
                              args.obj_thresh, args.iou_thresh, max_per_class, device=local, world=world, rank=rank)
     pipe.engine.load_weights(args.ckpt)
+    options = dict(match=getattr(args, "tile_match", "iou"), merge=getattr(args, "tile_merge", "suppress"),
+                   border=getattr(args, "tile_border", None))
     if getattr(args, "tiles", None):
-        pipe.enable_tiling(args.tiles[0], args.tiles[1], args.tile_overlap)
+        pipe.enable_tiling(args.tiles[0], args.tiles[1], args.tile_overlap, **options)
+    elif getattr(args, "tile_size", None):
+        pipe.enable_tiling(overlap=args.tile_overlap, tile_size=tuple(args.tile_size), images_per_batch=args.tile_images, **options)
     if getattr(args, "gpu_png", False):
         pipe.enable_png_decode()
     if getattr(args, "gpu_progressive", False):
@@ -182,16 +188,42 @@ def add_model_args(ap):
     ap.add_argument("--class_num", type=int, default=20)
     ap.add_argument("--anchors", default="data/voc_anchor.npy")
     ap.add_argument("--batch", type=int, default=32, help="images per GPU per step")
-    ap.add_argument("--tiles", type=int, nargs=2, default=None, metavar=("ROWS", "COLS"),
-                    help="also detect on ROWS x COLS overlapping tiles of every image and merge the views' records on the GPU; "
-                         "a batch then holds batch // (1 + ROWS * COLS) images")
+    grid = ap.add_mutually_exclusive_group()
+    grid.add_argument("--tiles", type=int, nargs=2, default=None, metavar=("ROWS", "COLS"),
+                      help="also detect on ROWS x COLS overlapping tiles of every image and merge the views' records on the GPU; "
+                           "a batch then holds batch // (1 + ROWS * COLS) images")
+    grid.add_argument("--tile_size", type=int, nargs=2, default=None, metavar=("H", "W"),
+                      help="also detect on overlapping tiles of at most H x W pixels, as many as each image's size needs (an "
+                           "image that fits one tile is detected whole only); needs --tile_images")
+    ap.add_argument("--tile_images", type=int, default=None, metavar="N",
+                    help="images per batch with --tile_size; each image gets at most batch // N views")
     ap.add_argument("--tile_overlap", type=float, default=0.2, help="fraction of a tile shared with its neighbour (with --tiles)")
+    ap.add_argument("--tile_match", choices=["iou", "ios"], default="iou",
+                    help="merge views' records matching by IoU or by intersection over the smaller box (threshold --iou_thresh)")
+    ap.add_argument("--tile_merge", choices=["suppress", "union"], default="suppress",
+                    help="drop a matching record, or also grow the kept record's box to the union of the records it suppressed")
+    ap.add_argument("--tile_border", type=float, default=None, metavar="PX",
+                    help="drop a tile's records within PX pixels of a tile edge inside the image before the merge")
     ap.add_argument("--gpu_png", action="store_true",
                     help="decode the PNG files the GPU decoder takes on the GPU too (the same pixels as PIL), not in the host threads")
     ap.add_argument("--gpu_progressive", action="store_true",
                     help="decode the progressive JPEG files the GPU decoder takes on the GPU too (the same pixels as PIL), not in "
                          "the host threads")
     ap.add_argument("--decode_threads", type=int, default=4, help="host threads reading the next batch's files and decoding those the GPU does not (PIL)")
+
+
+class ModelArgParser(argparse.ArgumentParser):
+    """An ArgumentParser that also refuses the add_model_args flags that need one another alone: --tile_size without
+    --tile_images, and --tile_images without --tile_size."""
+
+    def parse_known_args(self, args=None, namespace=None):
+        ns, rest = super().parse_known_args(args, namespace)
+        size, n = getattr(ns, "tile_size", None), getattr(ns, "tile_images", None)
+        if size is not None and n is None:
+            self.error("--tile_size needs --tile_images N: the images one batch holds")
+        if n is not None and size is None:
+            self.error("--tile_images goes with --tile_size")
+        return ns, rest
 
 
 def quality_arg(v):
@@ -202,7 +234,7 @@ def quality_arg(v):
 
 
 def build_parser():
-    ap = argparse.ArgumentParser()
+    ap = ModelArgParser()
     add_model_args(ap)
     ap.add_argument("images", help="directory of images, or a text file with one path per line")
     ap.add_argument("--obj_thresh", type=float, default=0.7)
