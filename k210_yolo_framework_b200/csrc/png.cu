@@ -13,7 +13,8 @@
 //                        decoding from a true block boundary is deterministic), resolves the references chunk by chunk into the
 //                        filtered rows and checks the Adler-32;
 //   png_inflate_kernel   one thread per image whose chain did not decode it inflates the stream serially (RFC 1950/1951),
-//                        stopping where zlib, as PIL drives it, stops (see inflate_image);
+//                        stopping where zlib, as PIL drives it, stops: PIL's reads of the IDAT data bound the tail it checks
+//                        (see inflate_image);
 //   png_unfilter_kernel  one CTA per image undoes the row filters as a diagonal wavefront (row r handles its unit x at step
 //                        x + r, so Up / Avg / Paeth always find their upper and upper-left bytes done) and writes HWC RGB at
 //                        the image's output offset, with sub-byte unpacking, palette, grey replication, 16-bit high bytes and
@@ -42,6 +43,7 @@ constexpr int CHUNK_THREADS = 32;
 constexpr int RESOLVE_THREADS = 1024;
 constexpr long long CHUNK_SYMBOLS = 4LL * CHUNK_BYTES + 131072;   // output capacity of a speculative chunk (symbols)
 constexpr long long MAX_RAW_BYTES = (1LL << 31) - 1;              // filtered bytes of one image the GPU takes
+constexpr long long PIL_READ = 65536;      // most IDAT bytes PIL hands zlib at once (ImageFile.MAXBLOCK)
 enum : int32_t { CHUNK_FINAL = 1, CHUNK_FAILED = 2 };
 
 enum : int32_t {
@@ -62,6 +64,7 @@ struct alignas(16) PngImg {
     long long prod_off;                 // workspace: int64 bytes inflated, int64 "the chunk chain decoded the image" flag
     long long chunk_bytes;              // compressed bytes per chunk
     int32_t chunk_first, nchunks;
+    long long piece_first, npiece;      // PIL's reads of the stream: their end offsets in the blob's piece array
     uint8_t plte[768];
 };
 
@@ -87,6 +90,7 @@ struct alignas(16) PngBlobHeader {
     uint32_t magic;
     int32_t n, nseg, nchunks;
     long long img_off, seg_off, chunk_off, blob_bytes, ws_bytes;
+    long long piece_off, npieces;
 };
 
 long long align16(long long v) { return (v + 15) & ~15LL; }
@@ -285,6 +289,7 @@ struct Huff {
     uint16_t fast[1 << FAST_BITS];
     uint16_t count[16];
     uint16_t sym[288];
+    uint16_t maxlen;        // longest code (0: no code)
 };
 
 // Returns 0 for a usable code, -1 for an over-subscribed one, 1 for an incomplete one (`left` > 0 codes unused).
@@ -292,6 +297,9 @@ __device__ int build_huff(Huff &hf, const uint8_t *len, int n) {
     for (int i = 0; i < 16; ++i) hf.count[i] = 0;
     for (int i = 0; i < n; ++i) hf.count[len[i]]++;
     hf.count[0] = 0;
+    hf.maxlen = 0;
+    for (int l = 1; l < 16; ++l)
+        if (hf.count[l]) hf.maxlen = (uint16_t)l;
     int left = 1;
     for (int l = 1; l < 16; ++l) {
         left = (left << 1) - hf.count[l];
@@ -315,7 +323,8 @@ __device__ int build_huff(Huff &hf, const uint8_t *len, int n) {
     return left > 0 ? 1 : 0;
 }
 
-// Next symbol: >= 0, -1 invalid code, -2 the code needs bits past the end of the stream.
+// Next symbol: >= 0, -1 invalid code, -2 the code needs bits past the end of the stream.  As in zlib, a code is invalid as soon
+// as the bits read rule out every code (the one-bit code's other bit, any first bit of an empty code), not only after 15 bits.
 __device__ __forceinline__ int decode_sym(Bits &br, const Huff &hf) {
     const uint32_t look = br.peek(15);
     const uint16_t e = hf.fast[look & ((1 << FAST_BITS) - 1)];
@@ -334,11 +343,12 @@ __device__ __forceinline__ int decode_sym(Bits &br, const Huff &hf) {
             br.drop(l);
             return hf.sym[index + (code - first)];
         }
+        if (l >= hf.maxlen) return br.has(l) ? -1 : -2;
         index += c;
         first = (first + c) << 1;
         code <<= 1;
     }
-    return br.has(15) ? -1 : -2;
+    return -1;
 }
 
 __constant__ uint16_t c_lbase[29] = {3, 4, 5, 6, 7, 8, 9, 10, 11, 13, 15, 17, 19, 23, 27, 31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
@@ -368,7 +378,10 @@ __device__ __forceinline__ int read_dynamic(Bits &br, Huff &lit, Huff &dist, uin
         cl[c_clorder[i]] = (uint8_t)br.peek(3);
         br.drop(3);
     }
-    if (build_huff(lit, cl, 19) != 0) return PNG_ERR_HEADER;    // the code-length code must be complete
+    const int rc = build_huff(lit, cl, 19);
+    if (rc < 0 || (rc > 0 && lit.maxlen)) return PNG_ERR_HEADER;    // the code-length code must be complete
+    // all zero: zlib reads every code length as a 0 of one bit, then finds no end-of-block code
+    if (rc > 0) return br.has(nlen + ndist) ? PNG_ERR_HEADER : -2;
     for (int i = 0; i < nlen + ndist;) {
         const int s = decode_sym(br, lit);
         if (s == -2) return -2;
@@ -379,8 +392,8 @@ __device__ __forceinline__ int read_dynamic(Bits &br, Huff &lit, Huff &dist, uin
         }
         int rep, val = 0;
         if (s == 16) {
+            if (!br.has(2)) return -2;      // zlib reads the repeat count before it refuses a first repeat
             if (i == 0) return PNG_ERR_HEADER;
-            if (!br.has(2)) return -2;
             val = lens[i - 1];
             rep = 3 + (int)br.peek(2);
             br.drop(2);
@@ -415,21 +428,23 @@ __device__ void fixed_tables(Huff &lit, Huff &dist, uint8_t *lens) {
     build_huff(dist, lens, 32);
 }
 
-// Inflates one image's zlib stream into its `total` filtered bytes.  The stop rule is zlib's as PIL drives it: once the image's
-// last byte is written, decoding goes on until it would have to write another byte (a literal, a match with a valid distance
-// code, or a non-empty stored block), still checking end-of-block codes, block headers, stored LEN / NLEN and, at the end of
-// the stream, the Adler-32; an invalid code there is an error, a distance too far back is not (zlib checks it only when it has
-// room to copy), and nothing after that point is read.  A stream that ends
-// early leaves the rest of the image unwritten: PIL accepts that only from a stream that ended cleanly (final block, Adler-32)
-// on a row boundary after at least one row.  Status: [0] error bits, [1] blocks,
-// [2] bytes written, [3] stream bytes consumed.
-__device__ void inflate_image(const PngImg &im, const uint8_t *stream, uint8_t *out, int32_t *status, long long *produced,
-                              uint8_t *win, Huff &lit, Huff &dist, uint8_t *lens) {
+// Inflates one image's zlib stream into its `total` filtered bytes, stopping where zlib stops as PIL drives it.  PIL hands zlib
+// the stream one read at a time (each IDAT in pieces of at most 64 KiB from its start: `ends`) with one row of output room per
+// call, and stops after the call that completes the last row.  So once the image's last byte is written, decoding goes on only
+// through the rest of the read that call was fed and only until zlib would have to write another byte (a literal, a match with
+// a valid distance code, or a non-empty stored block), still checking end-of-block codes, block headers, stored LEN / NLEN and
+// the Adler-32; an invalid code there is an error, a distance too far back is not (zlib checks it only when it has room to
+// copy).  A symbol decoded in the call that filled a row waits for the next call, which is fed the next read when that call
+// used up its own; with no read left PIL finds the file truncated.  A stream that ends early leaves the rest of the image
+// unwritten: PIL accepts that only when the call that wrote the last row also read the final block's Adler-32, after at least
+// one row.  Status: [0] error bits, [3] bytes written.
+__device__ void inflate_image(const PngImg &im, const uint8_t *stream, const long long *ends, uint8_t *out, int32_t *status,
+                              long long *produced, uint8_t *win, Huff &lit, Huff &dist, uint8_t *lens) {
     Bits br;
     br.start(stream, im.stream_len * 8, 16);     // past the zlib header, which the host checked
-    const long long total = im.raw_len;
+    const long long total = im.raw_len, row = 1 + (long long)im.rowbytes;
     long long o = 0;
-    int err = 0, blocks = 0;
+    int err = 0;
     uint32_t a1 = 1, a2 = 0;     // Adler-32 of everything written (bytes past `total` are never written)
     int since = 0;               // bytes added to a1 / a2 since the last modulo reduction
     auto put = [&](uint8_t b) {
@@ -444,6 +459,23 @@ __device__ void inflate_image(const PngImg &im, const uint8_t *stream, uint8_t *
             since = 0;
         }
     };
+    long long pc = 0, lim = ends[0];     // the read the zlib call writing at `o` is fed, and its end in the stream
+    bool stranded = false;               // a call waited for a read that does not exist
+    // Before a symbol's first byte at `o` (n bytes, of which those past `total` are never written): the read its call is fed.
+    auto place = [&](long long n) {
+        const long long q = (br.pos + 7) >> 3;     // bytes zlib has taken in
+        const bool fresh = q > lim;                 // decoded in a later read's call, which has room
+        while (q > lim) lim = ends[++pc];
+        const bool waits = (!fresh && o > 0 && o % row == 0) || (o / row + 1) * row < o + min(n, total - o);
+        if (waits && q == lim) {
+            if (pc + 1 < im.npiece) lim = ends[++pc];
+            else stranded = true;
+        }
+    };
+    // once the image is complete, nothing past the read that completed it is checked
+    auto done = [&]() {
+        if (o == total) br.total = min(br.total, lim * 8);
+    };
     bool last = false, ended = false;     // ended: the final block and a matching Adler-32 were read
     while (!err) {
         if (last) {             // end of the stream: the Adler-32, big-endian, byte aligned
@@ -455,7 +487,7 @@ __device__ void inflate_image(const PngImg &im, const uint8_t *stream, uint8_t *
                     br.drop(8);
                 }
                 if (v != ((a2 % 65521u) << 16 | (a1 % 65521u))) err |= PNG_ERR_ADLER;
-                ended = true;
+                ended = (br.pos >> 3) <= lim;
             }
             break;
         }
@@ -463,7 +495,6 @@ __device__ void inflate_image(const PngImg &im, const uint8_t *stream, uint8_t *
         last = br.peek(1);
         const int type = (int)(br.peek(3) >> 1);
         br.drop(3);
-        ++blocks;
         if (type == 3) {
             err |= PNG_ERR_HEADER;
             break;
@@ -486,8 +517,11 @@ __device__ void inflate_image(const PngImg &im, const uint8_t *stream, uint8_t *
                     cut = true;
                     break;
                 }
+                // a stored byte is written by the call fed the read that holds it
+                while ((br.pos >> 3) + 1 > lim) lim = ends[++pc];
                 put((uint8_t)br.peek(8));
                 br.drop(8);
+                done();
             }
             if (cut) break;
             continue;
@@ -518,7 +552,9 @@ __device__ void inflate_image(const PngImg &im, const uint8_t *stream, uint8_t *
                     stop = true;
                     break;
                 }
+                place(1);
                 put((uint8_t)s);
+                done();
                 continue;
             }
             if (s == 256) break;
@@ -552,8 +588,10 @@ __device__ void inflate_image(const PngImg &im, const uint8_t *stream, uint8_t *
                 err |= PNG_ERR_DISTANCE;
                 break;
             }
+            place(length);
             const int n = (int)min((long long)length, total - o);
             for (int k = 0; k < n; ++k) put(win[(o - d) & (WINDOW - 1)]);
+            done();
             if (n < length) {
                 stop = true;
                 break;
@@ -561,10 +599,8 @@ __device__ void inflate_image(const PngImg &im, const uint8_t *stream, uint8_t *
         }
         if (stop) break;
     }
-    const long long row = 1 + (long long)im.rowbytes;
     // an image left incomplete decodes only when its stream ended cleanly after at least one whole row (and on a row boundary)
-    if (!err && o < total && (!ended || o == 0 || o % row)) err |= PNG_ERR_TRUNCATED;
-    (void)blocks;
+    if (!err && (stranded || (o < total && (!ended || o == 0 || o % row)))) err |= PNG_ERR_TRUNCATED;
     status[0] |= err;
     status[3] = (int32_t)o;     // every byte decoded serially (o < 2^31: the host refuses larger images)
     *produced = o;
@@ -948,7 +984,8 @@ __global__ void __launch_bounds__(1) png_inflate_kernel(const uint8_t *__restric
     const PngImg &im = reinterpret_cast<const PngImg *>(blob + H.img_off)[blockIdx.x];
     long long *prod = reinterpret_cast<long long *>(ws + im.prod_off);
     if (prod[1]) return;        // the chunk chain decoded it
-    inflate_image(im, ws + im.stream_off, ws + im.raw_off, status + 4 * blockIdx.x, prod, win, lit, dist, lens);
+    const long long *ends = reinterpret_cast<const long long *>(blob + H.piece_off) + im.piece_first;
+    inflate_image(im, ws + im.stream_off, ends, ws + im.raw_off, status + 4 * blockIdx.x, prod, win, lit, dist, lens);
 }
 
 __device__ __forceinline__ uint8_t paeth(int a, int b, int c) {
@@ -1104,6 +1141,13 @@ extern "C" int k2y_png_plan(const unsigned char *const *files, const size_t *siz
         }
         nseg += (long long)ps[i].idat.size();
     }
+    // PIL's reads: every non-empty IDAT in pieces of at most PIL_READ bytes from its start
+    std::vector<long long> npiece(n, 0);
+    long long npieces = 0;
+    for (int i = 0; i < n; ++i) {
+        for (auto &c : ps[i].idat) npiece[i] += (c.second + PIL_READ - 1) / PIL_READ;
+        npieces += npiece[i];
+    }
     std::vector<long long> chunk_bytes(n);
     std::vector<int> nchunks(n);
     long long nch = 0;
@@ -1116,7 +1160,8 @@ extern "C" int k2y_png_plan(const unsigned char *const *files, const size_t *siz
     const long long img_off = align16(sizeof(PngBlobHeader));
     const long long seg_off = img_off + (long long)sizeof(PngImg) * n;
     const long long chunk_off = seg_off + (long long)sizeof(PngSeg) * nseg;
-    const long long total = chunk_off + (long long)sizeof(PngChunk) * nch;
+    const long long piece_off = chunk_off + (long long)sizeof(PngChunk) * nch;
+    const long long total = piece_off + (long long)sizeof(long long) * npieces;
     *blob_bytes = (size_t)total;
     if (!blob) return K2Y_OK;
     if (blob_capacity < (size_t)total || ((uintptr_t)blob & 15)) {
@@ -1129,7 +1174,8 @@ extern "C" int k2y_png_plan(const unsigned char *const *files, const size_t *siz
     PngImg *I = reinterpret_cast<PngImg *>(B + img_off);
     PngSeg *S = reinterpret_cast<PngSeg *>(B + seg_off);
     PngChunk *C = reinterpret_cast<PngChunk *>(B + chunk_off);
-    long long ws = 0;
+    long long *P = reinterpret_cast<long long *>(B + piece_off);
+    long long ws = 0, pg = 0;
     int sg = 0, cg = 0;
     for (int i = 0; i < n; ++i) {
         const PngParsed &p = ps[i];
@@ -1165,11 +1211,14 @@ extern "C" int k2y_png_plan(const unsigned char *const *files, const size_t *siz
         }
         im.seg_first = sg;
         im.nseg = (int)p.idat.size();
+        im.piece_first = pg;
+        im.npiece = npiece[i];
         long long at = 0;
         for (auto &c : p.idat) {
             S[sg].src = src_offsets[i] + c.first;
             S[sg].len = c.second;
             S[sg].dst = at;
+            for (long long k = 0; k < c.second; k += PIL_READ) P[pg++] = at + std::min(c.second, k + PIL_READ);
             at += c.second;
             ++sg;
         }
@@ -1181,6 +1230,8 @@ extern "C" int k2y_png_plan(const unsigned char *const *files, const size_t *siz
     H.seg_off = seg_off;
     H.chunk_off = chunk_off;
     H.nchunks = (int)nch;
+    H.piece_off = piece_off;
+    H.npieces = npieces;
     H.blob_bytes = total;
     H.ws_bytes = ws;
     return K2Y_OK;

@@ -2,7 +2,9 @@
 
 A stream is built from blocks; each block holds tokens: an int (a literal byte) or a tuple (length, distance) for a match.
 ``stored`` / ``fixed`` / ``dynamic`` write one block each; ``dynamic`` takes explicit code lengths, so tests can make one-code and
-empty distance codes, 15-bit codes and other shapes zlib's encoder does not choose.  ``zlib_wrap`` adds the header and Adler-32.
+empty distance codes, 15-bit codes and other shapes zlib's encoder does not choose.  ``dynamic_header`` writes a dynamic block's
+header field by field (HLIT 287 / 288, HDIST 31 / 32, any code-length code, any repeat), for headers zlib must refuse.
+``BitWriter.tell`` gives the bit a block starts at.  ``zlib_wrap`` adds the header and Adler-32.
 """
 from __future__ import annotations
 
@@ -43,6 +45,10 @@ class BitWriter:
     def align(self) -> None:
         if self.n:
             self.bits(0, 8 - self.n)
+
+    def tell(self) -> int:
+        """Bits written so far: the position of the next bit in the raw DEFLATE stream."""
+        return 8 * len(self.out) + self.n
 
     def getvalue(self) -> bytes:
         return bytes(self.out) + (bytes([self.acc]) if self.n else b"")
@@ -182,6 +188,36 @@ def dynamic(w: BitWriter, tokens: Sequence[Token], final: bool, lit_lens: Option
     for l in lens:
         w.code(cl_codes[l], cl[l])
     _write_tokens(w, tokens, canonical(lit_lens), lit_lens, canonical((dist_lens + [0] * 30)[:30]), (dist_lens + [0] * 30)[:30])
+
+
+def dynamic_header(w: BitWriter, final: bool, nlen: int, ndist: int, cl_lens: Sequence[int], lengths: Sequence,
+                   ncode: int = 19) -> None:
+    """A dynamic block header as written, checked by nothing: HLIT = nlen - 257 and HDIST = ndist - 1 (5 bits each, so 287 /
+    288 and 31 / 32 are allowed), the first `ncode` of `cl_lens` (indexed by code-length symbol) in CL_ORDER, then `lengths`
+    coded with the code of `cl_lens`: a length 0..15, a repeat (16 | 17 | 18, extra bits), or ("raw", value, bits)."""
+    w.bits(int(final), 1)
+    w.bits(2, 2)
+    w.bits(nlen - 257, 5)
+    w.bits(ndist - 1, 5)
+    w.bits(ncode - 4, 4)
+    for i in range(ncode):
+        w.bits(cl_lens[CL_ORDER[i]], 3)
+    codes = canonical(cl_lens)
+    nbits = {16: 2, 17: 3, 18: 7}
+    for x in lengths:
+        if isinstance(x, tuple) and x[0] == "raw":
+            w.bits(x[1], x[2])
+        elif isinstance(x, tuple):
+            w.code(codes[x[0]], cl_lens[x[0]])
+            w.bits(x[1], nbits[x[0]])
+        else:
+            w.code(codes[x], cl_lens[x])
+
+
+def tokens_with(w: BitWriter, tokens: Sequence[Token], lit_lens: Sequence[int], dist_lens: Sequence[int]) -> None:
+    """The tokens and the end-of-block code, with explicit literal/length and distance code lengths (behind ``dynamic_header``)."""
+    dist_lens = (list(dist_lens) + [0] * 30)[:30]
+    _write_tokens(w, tokens, canonical(lit_lens), lit_lens, canonical(dist_lens), dist_lens)
 
 
 def zlib_wrap(deflate: bytes, data: bytes) -> bytes:
