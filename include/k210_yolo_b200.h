@@ -217,6 +217,19 @@ int k2y_merge_views_ex(const k2y_det *view_dets_dev, const int32_t *view_counts_
                        int match, int merge, int n_images, int rows, int max_views, int n_boxes, int class_num, int max_per_class,
                        float thresh, k2y_det *dets_dev, int32_t *counts_dev, long long det_image_stride_words,
                        long long count_image_stride_words, void *stream);
+/* k2y_merge_views_ex with mirrored views (test-time flip; k2y_merge_views_ex is this call with a null view_mirror_dev):
+ *   view_mirror_dev   int32 [N] on the device, nonzero for a view that is its window flipped left to right
+ *                     (k2y_letterbox_u8_views_mirror), whose records are in mirrored window coordinates.  Each such record is
+ *                     mapped back while it is loaded: xmin = fl(fl(tw - xmax) + x0), xmax = fl(fl(tw - xmin) + x0), y fields
+ *                     shifted as for any view (a NaN result is the canonical NaN); index = view * n_boxes + index as for any
+ *                     view.  The border drop tests the record in the mirrored coordinates it comes in, with the window's
+ *                     left and right side bits (2 and 8, as view_sides_dev gives them for the window) swapped.  Needs
+ *                     view_hw_dev (tw), with or without a border drop.  NULL: no view is mirrored. */
+int k2y_merge_views_mirror(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev,
+                           const int32_t *view_offsets_dev, const int32_t *view_sides_dev, const int32_t *view_mirror_dev,
+                           const float *view_hw_dev, float border, int match, int merge, int n_images, int rows, int max_views,
+                           int n_boxes, int class_num, int max_per_class, float thresh, k2y_det *dets_dev, int32_t *counts_dev,
+                           long long det_image_stride_words, long long count_image_stride_words, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * Multi-GPU collation: images shard across ranks (one process per GPU), and the one exchange on the path
@@ -314,6 +327,12 @@ int k2y_letterbox_u8_batch(const unsigned char *src_dev, int n, const long long 
 int k2y_letterbox_u8_views(const unsigned char *src_dev, int n_views, const long long *offsets_host, const int *hw_host,
                            const int *windows_host, const double *inv_matrices_host, unsigned char *dst_dev, int dst_h, int dst_w,
                            float *image_hw_dev, float *view_yx_dev, int *minmax_dev, void *stream);
+/* k2y_letterbox_u8_views with mirrored views: mirror_host[i] nonzero letterboxes view i as np.fliplr of its window, bit for bit
+ * (the same matrix, min and max; only the fetched column changes).  NULL: no view is mirrored, k2y_letterbox_u8_views. */
+int k2y_letterbox_u8_views_mirror(const unsigned char *src_dev, int n_views, const long long *offsets_host, const int *hw_host,
+                                  const int *windows_host, const int *mirror_host, const double *inv_matrices_host,
+                                  unsigned char *dst_dev, int dst_h, int dst_w, float *image_hw_dev, float *view_yx_dev,
+                                  int *minmax_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * Baseline JPEG decode on the device, in front of k2y_letterbox_u8_batch: replaces the file decode of

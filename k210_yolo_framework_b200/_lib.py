@@ -109,6 +109,9 @@ _SIGNATURES = {
     "k2y_merge_views_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int, c_int, c_int,
                                    c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, ctypes.c_longlong, ctypes.c_longlong,
                                    c_void_p]),
+    "k2y_merge_views_mirror": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float, c_int, c_int,
+                                       c_int, c_int, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p, ctypes.c_longlong,
+                                       ctypes.c_longlong, c_void_p]),
     "k2y_comm_unique_id": (c_int, [c_void_p]),
     "k2y_comm_create": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_void_p)]),
     "k2y_comm_destroy": (c_int, [c_void_p]),
@@ -130,6 +133,8 @@ _SIGNATURES = {
                                        c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "k2y_letterbox_u8_views": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong), POINTER(c_int), POINTER(c_int), POINTER(ctypes.c_double),
                                        c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "k2y_letterbox_u8_views_mirror": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong), POINTER(c_int), POINTER(c_int), POINTER(c_int),
+                                              POINTER(ctypes.c_double), c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "k2y_jpeg_inspect": (c_int, [c_void_p, c_size_t, POINTER(JpegInfo)]),
     "k2y_jpeg_plan": (c_int, [POINTER(c_void_p), POINTER(c_size_t), c_int, POINTER(ctypes.c_longlong), POINTER(ctypes.c_longlong),
                               c_void_p, c_size_t, POINTER(c_size_t)]),

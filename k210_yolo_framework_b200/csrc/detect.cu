@@ -1024,6 +1024,9 @@ __global__ void __launch_bounds__(32) nms_boxes_kernel(const float4 *__restrict_
 //                 warp and field, double-buffered like the liveness words; warp 0 folds the 16 warps' words behind the next
 //                 round's barrier and writes the record then, so a round still costs one barrier (plus one after the loop
 //                 when it ends at max_per_class).
+// k2y_merge_views_mirror adds mirrored views (the window flipped left to right, k2y_letterbox_u8_views_mirror), whose records
+// are in mirrored window coordinates: the load maps them back, xmin = fl(fl(tw - xmax) + x0), xmax = fl(fl(tw - xmin) + x0),
+// and the border drop, which tests the record as it comes, swaps the window's left and right side bits (2 and 8).
 constexpr int MERGE_THREADS = 512;
 constexpr int MERGE_MAX = 2 * MERGE_THREADS;   // records of one (image, class) over all views
 constexpr int MERGE_WARPS = MERGE_THREADS / 32;
@@ -1036,7 +1039,8 @@ struct MergeParams {
     const float *view_yx;   // [N][2] (y0, x0)
     const int *off;         // [n + 1] first view of image b; null: b * V (uniform ranges)
     const int *sides;       // [N] interior-side bits (1 top, 2 left, 4 bottom, 8 right); null: no border drop
-    const float *view_hw;   // [N][2] (th, tw), read with `sides`
+    const int *mirror;      // [N] nonzero: view mirrored left to right; null: none is
+    const float *view_hw;   // [N][2] (th, tw), read with `sides` or `mirror`
     float border;
     int n, V, C, K, nbox;
     float iou;
@@ -1113,8 +1117,10 @@ __global__ void __launch_bounds__(MERGE_THREADS) merge_views_kernel(const MergeP
         const int i = tid + s * MERGE_THREADS, v = i / p.K, k = i - v * p.K;
         if (v >= V || k >= s_off[v + 1] - s_off[v]) continue;
         const k2y_det d = p.vdets[((view0 + v) * p.C + c) * p.K + k];
+        const bool mirrored = p.mirror && p.mirror[view0 + v];
         if (p.sides) {
-            const int side = p.sides[view0 + v];
+            int side = p.sides[view0 + v];
+            if (mirrored) side = (side & 5) | ((side & 2) << 2) | ((side & 8) >> 2);   // the window's left edge is the view's right
             const float m = p.border;
             const bool drop = ((side & 1) && fminf(d.ymin, d.ymax) < m) || ((side & 2) && fminf(d.xmin, d.xmax) < m) ||
                               ((side & 4) && fmaxf(d.ymin, d.ymax) > __fsub_rn(p.view_hw[2 * (view0 + v)], m)) ||
@@ -1126,7 +1132,13 @@ __global__ void __launch_bounds__(MERGE_THREADS) merge_views_kernel(const MergeP
             }
         }
         const float y0 = p.view_yx[2 * (view0 + v)], x0 = p.view_yx[2 * (view0 + v) + 1];
-        mybox[s] = make_float4(__fadd_rn(d.ymin, y0), __fadd_rn(d.xmin, x0), __fadd_rn(d.ymax, y0), __fadd_rn(d.xmax, x0));
+        float xmin = d.xmin, xmax = d.xmax;
+        if (mirrored) {
+            const float tw = p.view_hw[2 * (view0 + v) + 1];
+            xmin = __fsub_rn(tw, d.xmax);
+            xmax = __fsub_rn(tw, d.xmin);
+        }
+        mybox[s] = make_float4(__fadd_rn(d.ymin, y0), __fadd_rn(xmin, x0), __fadd_rn(d.ymax, y0), __fadd_rn(xmax, x0));
         s_keys[s_off[v] + k] = mykey[s] = pack_key(d.score, v * p.nbox + d.index);
     }
     int P = 32;
@@ -1386,10 +1398,10 @@ extern "C" int k2y_merge_views_max_records(void) { return MERGE_MAX; }
 
 namespace {
 int merge_views_launch(const char *fn, const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev,
-                       const int32_t *view_offsets_dev, const int32_t *view_sides_dev, const float *view_hw_dev, float border,
-                       int match, int merge, int n_images, int rows, int max_views, int n_boxes, int class_num, int max_per_class,
-                       float thresh, k2y_det *dets_dev, int32_t *counts_dev, long long det_image_stride_words,
-                       long long count_image_stride_words, void *stream) {
+                       const int32_t *view_offsets_dev, const int32_t *view_sides_dev, const int32_t *view_mirror_dev,
+                       const float *view_hw_dev, float border, int match, int merge, int n_images, int rows, int max_views,
+                       int n_boxes, int class_num, int max_per_class, float thresh, k2y_det *dets_dev, int32_t *counts_dev,
+                       long long det_image_stride_words, long long count_image_stride_words, void *stream) {
     if (!view_dets_dev || !view_counts_dev || !view_yx_dev || !dets_dev || !counts_dev || n_images < 0 || rows < 1 || rows < n_images ||
         max_views < 1 || n_boxes < 1 || class_num < 1 || class_num > 65535 || max_per_class < 1) {
         set_error("%s: null pointer, or not 0 <= n_images <= rows, rows, views, n_boxes, max_per_class >= 1, class_num 1..65535", fn);
@@ -1401,6 +1413,10 @@ int merge_views_launch(const char *fn, const k2y_det *view_dets_dev, const int32
     }
     if (view_sides_dev && (!view_hw_dev || !(border >= 0.f))) {
         set_error("%s: a border drop needs the views' sizes and a border >= 0 (got %g)", fn, (double)border);
+        return K2Y_ERR_INVALID;
+    }
+    if (view_mirror_dev && !view_hw_dev) {
+        set_error("%s: mirrored views need the views' sizes", fn);
         return K2Y_ERR_INVALID;
     }
     if ((long long)max_views * max_per_class > MERGE_MAX) {
@@ -1421,6 +1437,7 @@ int merge_views_launch(const char *fn, const k2y_det *view_dets_dev, const int32
     p.view_yx = view_yx_dev;
     p.off = view_offsets_dev;
     p.sides = view_sides_dev;
+    p.mirror = view_mirror_dev;
     p.view_hw = view_hw_dev;
     p.border = border;
     p.n = n_images;
@@ -1444,13 +1461,24 @@ int merge_views_launch(const char *fn, const k2y_det *view_dets_dev, const int32
 }
 }  // namespace
 
+extern "C" int k2y_merge_views_mirror(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev,
+                                      const int32_t *view_offsets_dev, const int32_t *view_sides_dev, const int32_t *view_mirror_dev,
+                                      const float *view_hw_dev, float border, int match, int merge, int n_images, int rows,
+                                      int max_views, int n_boxes, int class_num, int max_per_class, float thresh, k2y_det *dets_dev,
+                                      int32_t *counts_dev, long long det_image_stride_words, long long count_image_stride_words,
+                                      void *stream) {
+    return merge_views_launch("k2y_merge_views_mirror", view_dets_dev, view_counts_dev, view_yx_dev, view_offsets_dev, view_sides_dev,
+                              view_mirror_dev, view_hw_dev, border, match, merge, n_images, rows, max_views, n_boxes, class_num,
+                              max_per_class, thresh, dets_dev, counts_dev, det_image_stride_words, count_image_stride_words, stream);
+}
+
 extern "C" int k2y_merge_views_ex(const k2y_det *view_dets_dev, const int32_t *view_counts_dev, const float *view_yx_dev,
                                   const int32_t *view_offsets_dev, const int32_t *view_sides_dev, const float *view_hw_dev,
                                   float border, int match, int merge, int n_images, int rows, int max_views, int n_boxes,
                                   int class_num, int max_per_class, float thresh, k2y_det *dets_dev, int32_t *counts_dev,
                                   long long det_image_stride_words, long long count_image_stride_words, void *stream) {
     return merge_views_launch("k2y_merge_views_ex", view_dets_dev, view_counts_dev, view_yx_dev, view_offsets_dev, view_sides_dev,
-                              view_hw_dev, border, match, merge, n_images, rows, max_views, n_boxes, class_num, max_per_class, thresh,
+                              nullptr, view_hw_dev, border, match, merge, n_images, rows, max_views, n_boxes, class_num, max_per_class, thresh,
                               dets_dev, counts_dev, det_image_stride_words, count_image_stride_words, stream);
 }
 
@@ -1458,7 +1486,8 @@ extern "C" int k2y_merge_views(const k2y_det *view_dets_dev, const int32_t *view
                                int rows, int views, int n_boxes, int class_num, int max_per_class, float iou_thresh, k2y_det *dets_dev,
                                int32_t *counts_dev, long long det_image_stride_words, long long count_image_stride_words,
                                void *stream) {
-    return merge_views_launch("k2y_merge_views", view_dets_dev, view_counts_dev, view_yx_dev, nullptr, nullptr, nullptr, -1.f, K2Y_MATCH_IOU,
+    return merge_views_launch("k2y_merge_views", view_dets_dev, view_counts_dev, view_yx_dev, nullptr, nullptr, nullptr, nullptr, -1.f,
+                              K2Y_MATCH_IOU,
                               K2Y_MERGE_SUPPRESS, n_images, rows, views, n_boxes, class_num, max_per_class, iou_thresh, dets_dev,
                               counts_dev, det_image_stride_words, count_image_stride_words, stream);
 }

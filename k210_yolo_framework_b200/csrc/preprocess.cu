@@ -14,7 +14,9 @@
 
 // A batch is n images of different sizes packed back to back in one device buffer.  What is letterboxed is a VIEW: a window
 // (y0, x0, th, tw) of one of those images, treated as an image of its own (the whole image is the window (0, 0, h, w)); several
-// views may share an image.  The descriptors travel by value in the kernel parameters (__grid_constant__: indexed in place,
+// views may share an image.  A mirrored view is the window flipped left to right: the warp samples the same positions and
+// fetches column tw - 1 - c where it would fetch c, so it equals the letterbox of np.fliplr(window) bit for bit (folding the
+// flip into the inverse matrix instead would round tw - 1 - x differently).  The descriptors travel by value in the kernel parameters (__grid_constant__: indexed in place,
 // never copied to local memory), LB_MAX_IMAGES views per launch.  Pass 1 reduces each window's min and max into the scratch as
 // (255 - min, max), both with atomicMax, so that one memset to zero initialises it; pass 2 is the bilinear warp, one thread
 // per output pixel, grid (pixel tile, view).
@@ -30,6 +32,7 @@ struct LbImage {
     int pitch;          // pixels per row of the image the window lies in
     int h, w;           // the window's size
     int y0, x0;         // its origin in the image (only reported, view_yx)
+    int mirror;         // nonzero: the window flipped left to right
     double m[6];        // the first two rows of the inverse affine matrix, in window coordinates
 };
 
@@ -117,9 +120,12 @@ __global__ void __launch_bounds__(LB_THREADS) letterbox_minmax_kernel(const __gr
     }
 }
 
-__device__ __forceinline__ double pix_or_zero(const unsigned char *src, int sh, int sw, int pitch, double r, double c, int ch) {
+// the bounds test is on the sampled column c; a mirrored view fetches the window's column sw - 1 - c
+__device__ __forceinline__ double pix_or_zero(const unsigned char *src, int sh, int sw, int pitch, bool mirror, double r, double c,
+                                              int ch) {
     if (!(r >= 0.0 && r < (double)sh && c >= 0.0 && c < (double)sw)) return 0.0;
-    return (double)src[((size_t)(int)r * pitch + (int)c) * 3 + ch];
+    const int col = mirror ? sw - 1 - (int)c : (int)c;
+    return (double)src[((size_t)(int)r * pitch + col) * 3 + ch];
 }
 
 __global__ void __launch_bounds__(LB_THREADS) letterbox_warp_kernel(const __grid_constant__ LbBatch p) {
@@ -137,6 +143,7 @@ __global__ void __launch_bounds__(LB_THREADS) letterbox_warp_kernel(const __grid
     if (idx >= p.dh * p.dw) return;
     const unsigned char *src = p.src + im.offset;
     const int sh = im.h, sw = im.w, pitch = im.pitch;
+    const bool mir = im.mirror != 0;
     const double r = (double)(idx / p.dw), c = (double)(idx % p.dw);
     const double x = __dadd_rn(__dadd_rn(__dmul_rn(im.m[0], c), __dmul_rn(im.m[1], r)), im.m[2]);
     const double y = __dadd_rn(__dadd_rn(__dmul_rn(im.m[3], c), __dmul_rn(im.m[4], r)), im.m[5]);
@@ -148,8 +155,8 @@ __global__ void __launch_bounds__(LB_THREADS) letterbox_warp_kernel(const __grid
     unsigned char *dst = p.dst + ((size_t)b * p.dh * p.dw + idx) * 3;
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
-        const double p00 = pix_or_zero(src, sh, sw, pitch, minr, minc, ch), p01 = pix_or_zero(src, sh, sw, pitch, minr, maxc, ch);
-        const double p10 = pix_or_zero(src, sh, sw, pitch, maxr, minc, ch), p11 = pix_or_zero(src, sh, sw, pitch, maxr, maxc, ch);
+        const double p00 = pix_or_zero(src, sh, sw, pitch, mir, minr, minc, ch), p01 = pix_or_zero(src, sh, sw, pitch, mir, minr, maxc, ch);
+        const double p10 = pix_or_zero(src, sh, sw, pitch, mir, maxr, minc, ch), p11 = pix_or_zero(src, sh, sw, pitch, mir, maxr, maxc, ch);
         const double top = __dadd_rn(__dmul_rn(wc, p00), __dmul_rn(dc, p01));
         const double bot = __dadd_rn(__dmul_rn(wc, p10), __dmul_rn(dc, p11));
         double o = __dadd_rn(__dmul_rn(wr, top), __dmul_rn(dr, bot));
@@ -161,9 +168,10 @@ __global__ void __launch_bounds__(LB_THREADS) letterbox_warp_kernel(const __grid
 }  // namespace
 }  // namespace k2y
 
-extern "C" int k2y_letterbox_u8_views(const unsigned char *src_dev, int n_views, const long long *offsets_host, const int *hw_host,
-                                      const int *windows_host, const double *inv_matrices_host, unsigned char *dst_dev, int dst_h,
-                                      int dst_w, float *image_hw_dev, float *view_yx_dev, int *minmax_dev, void *stream) {
+extern "C" int k2y_letterbox_u8_views_mirror(const unsigned char *src_dev, int n_views, const long long *offsets_host,
+                                             const int *hw_host, const int *windows_host, const int *mirror_host,
+                                             const double *inv_matrices_host, unsigned char *dst_dev, int dst_h, int dst_w,
+                                             float *image_hw_dev, float *view_yx_dev, int *minmax_dev, void *stream) {
     using namespace k2y;
     if (!src_dev || n_views <= 0 || !offsets_host || !hw_host || !windows_host || !inv_matrices_host || !dst_dev || !minmax_dev ||
         dst_h <= 0 || dst_w <= 0 || (long long)dst_h * dst_w > (1LL << 30)) {
@@ -205,6 +213,7 @@ extern "C" int k2y_letterbox_u8_views(const unsigned char *src_dev, int n_views,
             im.x0 = win[1];
             im.h = win[2];
             im.w = win[3];
+            im.mirror = mirror_host ? (mirror_host[g0 + i] != 0) : 0;
             im.offset = offsets_host[g0 + i] + ((long long)im.y0 * im.pitch + im.x0) * 3;
             for (int k = 0; k < 6; ++k) im.m[k] = inv_matrices_host[6 * (g0 + i) + k];
             const size_t blocks = LbRuns(im).blocks();
@@ -215,6 +224,13 @@ extern "C" int k2y_letterbox_u8_views(const unsigned char *src_dev, int n_views,
         K2Y_CUDA_CHECK(cudaGetLastError());
     }
     return K2Y_OK;
+}
+
+extern "C" int k2y_letterbox_u8_views(const unsigned char *src_dev, int n_views, const long long *offsets_host, const int *hw_host,
+                                      const int *windows_host, const double *inv_matrices_host, unsigned char *dst_dev, int dst_h,
+                                      int dst_w, float *image_hw_dev, float *view_yx_dev, int *minmax_dev, void *stream) {
+    return k2y_letterbox_u8_views_mirror(src_dev, n_views, offsets_host, hw_host, windows_host, nullptr, inv_matrices_host, dst_dev,
+                                         dst_h, dst_w, image_hw_dev, view_yx_dev, minmax_dev, stream);
 }
 
 extern "C" int k2y_letterbox_u8_batch(const unsigned char *src_dev, int n, const long long *offsets_host, const int *hw_host,

@@ -33,6 +33,10 @@ grid (``tiles.plan_grid``) and ``images_per_batch`` is the caller's; ``k2y_merge
 and the windows' interior sides from a table that travels in the batch's H2D copy, and can match by intersection over the
 smaller box, fold the matched boxes into the kept one and drop records at the tiles' inner borders.
 
+``enable_flip`` makes ``submit_images`` detect every view a second time, mirrored left to right (the flip the reference trains
+with): the letterbox fetches the mirrored columns, and ``k2y_merge_views_mirror`` maps the mirrored views' records back into
+the image while it loads them, then merges all views as above.  It combines with either grid, in either order.
+
 ``enable_png_decode`` makes ``submit_images`` decode the PNG files the GPU takes there too (``preprocess.png_gpu_decodable``),
 in the same staging range and H2D copy as the batch's JPEGs; their status words travel beside the JPEGs'.
 ``enable_progressive_jpeg_decode`` does the same for progressive JPEGs (``preprocess.progressive_gpu_decodable``).
@@ -53,6 +57,15 @@ from .dist import DetectionGather
 from .preprocess import BatchLayout, Staging, check_jpeg_status, check_png_status, check_progressive_status, letterbox_packed
 
 SLOTS = 2
+
+
+def _check_merge_options(match, merge, border) -> None:
+    if match not in tiles.MATCHES:
+        raise ValueError(f"unknown match metric {match!r}: one of {', '.join(tiles.MATCHES)}")
+    if merge not in tiles.MERGES:
+        raise ValueError(f"unknown merge action {merge!r}: one of {', '.join(tiles.MERGES)}")
+    if border is not None and not float(border) >= 0:
+        raise ValueError(f"tile border {border}: at least 0 pixels")
 
 
 class DetectionPipeline:
@@ -110,9 +123,13 @@ class DetectionPipeline:
         self._render_done = [torch.cuda.Event() for _ in range(SLOTS)]   # files of gather slot ready to copy back
         self._render_free = [torch.cuda.Event() for _ in range(SLOTS)]   # render + encode finished with input slot's originals
         self._rendered_slot: List[bool] = [False] * SLOTS
-        # enable_tiling: (rows, cols, overlap) or a tiles.SizedTiling, the most views of an image, images per batch, the merge's
+        # enable_tiling / enable_flip: the grid and merge options asked for and the flip, from which tiles.plan_views derives
+        # the rest: (rows, cols, overlap) or a tiles.SizedTiling, the most views of an image, images per batch, the merge's
         # options (None: k2y_merge_views), the per-view record block the decode writes and the merge reads (both on the decode
         # stream, so one block serves every batch) and per input slot the device (y0, x0) of its views
+        self._grid = None
+        self._merge_options = dict(match="iou", merge="suppress", match_thresh=None, border=None)
+        self._flip = False
         self._tiling = None
         self._views = 1
         self._ipb = self.batch
@@ -150,15 +167,10 @@ class DetectionPipeline:
                           field-wise union of itself and the candidates it suppressed (score and index stay its own);
           `border`        None (the default) or m >= 0: a tile's record within m pixels of a tile edge that lies inside the
                           image is dropped before the merge (oracle/tiles_merge_ref.py states each rule exactly).
-        With none of these set, the merge is ``k2y_merge_views`` exactly.  Bad values raise ``ValueError`` and leave the
-        pipeline as it was."""
-        limit = int(lib.k2y_merge_views_max_records())
-        if match not in tiles.MATCHES:
-            raise ValueError(f"unknown match metric {match!r}: one of {', '.join(tiles.MATCHES)}")
-        if merge not in tiles.MERGES:
-            raise ValueError(f"unknown merge action {merge!r}: one of {', '.join(tiles.MERGES)}")
-        if border is not None and not float(border) >= 0:
-            raise ValueError(f"tile border {border}: at least 0 pixels")
+        With none of these set (and no ``enable_flip``), the merge is ``k2y_merge_views`` exactly.  With ``enable_flip``, before
+        or after this call, every window is detected mirrored as well: V and max_views above count the mirrored views, and a
+        tile_size grid is planned under max_views // 2.  Bad values raise ``ValueError`` and leave the pipeline as it was."""
+        _check_merge_options(match, merge, border)
         if not 0 <= overlap < 1:
             raise ValueError(f"tile overlap {overlap} is outside [0, 1)")
         if tile_size is None:
@@ -169,12 +181,7 @@ class DetectionPipeline:
             rows, cols = int(rows), int(cols)
             if rows < 1 or cols < 1:
                 raise ValueError(f"tiling {rows}x{cols}: at least one tile per axis")
-            V = 1 + rows * cols
-            if V > self.batch:
-                raise ValueError(f"{V} views per image do not fit a batch of {self.batch}")
-            if V * self.gather.K > limit:
-                raise ValueError(f"{V} views x {self.gather.K} records per class exceed the {limit} records one merge holds")
-            tiling, ipb = (rows, cols, overlap), self.batch // V
+            grid = ("grid", rows, cols, overlap)
         else:
             if rows is not None or cols is not None:
                 raise ValueError("enable_tiling takes rows and cols, or tile_size, not both")
@@ -186,22 +193,43 @@ class DetectionPipeline:
             ipb = int(images_per_batch)
             if not 1 <= ipb <= self.batch:
                 raise ValueError(f"images_per_batch {ipb} is outside 1..{self.batch}")
-            V = min(self.batch // ipb, limit // self.gather.K)
-            if V < 1:
-                raise ValueError(f"no view fits: {self.gather.K} records per class exceed the {limit} records one merge holds")
-            tiling = tiles.SizedTiling((th, tw), overlap, V)
-        options = dict(match=match, merge=merge, match_thresh=match_thresh, border=border)
-        legacy = tile_size is None and options == dict(match="iou", merge="suppress", match_thresh=None, border=None)
+            grid = ("size", (th, tw), overlap, ipb)
+        self._set_views(grid, dict(match=match, merge=merge, match_thresh=match_thresh, border=border), self._flip)
+
+    def enable_flip(self, *, match: Optional[str] = None, merge: Optional[str] = None, match_thresh: Optional[float] = None,
+                    border: Optional[float] = None) -> None:
+        """From now on ``submit_images`` detects every view of an image a second time, mirrored left to right: the whole image
+        then its mirror without tiling, or with W windows per image (``enable_tiling``, before or after this call) views 0 .. W-1
+        as without flip and view W + v window v mirrored.  A mirrored view is letterboxed and decoded as ``np.fliplr`` of its
+        crop submitted as an image of its own would be, and the merge maps its records back into the image
+        (xmin = fl(fl(tw - xmax_m) + x0), xmax = fl(fl(tw - xmin_m) + x0); index = (W + v) * nbox + index) before merging every
+        view as ``enable_tiling`` describes, with its options.  A batch holds batch // V images (V = 2, or 2 (1 + rows * cols));
+        a tile_size grid plans its windows under max_views // 2.  `match`, `merge`, `match_thresh` and `border` are
+        ``enable_tiling``'s merge options; each one not given keeps its value (from ``enable_tiling``, else the default), so the
+        merge of a flip without tiling can take them too.  Raises ``ValueError`` when the views do not fit the batch or one
+        merge, or for a bad option, and leaves the pipeline as it was."""
+        given = dict(match=match, merge=merge, match_thresh=match_thresh, border=border)
+        options = dict(self._merge_options, **{k: v for k, v in given.items() if v is not None})
+        _check_merge_options(options["match"], options["merge"], options["border"])
+        self._set_views(self._grid, options, True)
+
+    def _set_views(self, grid, options: dict, flip: bool) -> None:
+        """The one place the views follow from the grid, the merge options and the flip (``tiles.plan_views``); nothing changes
+        when it raises."""
+        tiling, V, ipb = tiles.plan_views(self.batch, self.gather.K, int(lib.k2y_merge_views_max_records()), grid, flip)
+        legacy = not flip and grid[0] == "grid" and options == dict(match="iou", merge="suppress", match_thresh=None, border=None)
         dev = torch.device("cuda", self.device_index)
+        self._grid, self._merge_options, self._flip = grid, options, flip
         self._tiling, self._views, self._ipb = tiling, V, ipb
         self._merge = None if legacy else dict(
-            match=tiles.MATCHES.index(match), merge=tiles.MERGES.index(merge),
-            thresh=float(self.detector.cfg.iou_thresh if match_thresh is None else match_thresh),
-            border=None if border is None else float(border))
+            match=tiles.MATCHES.index(options["match"]), merge=tiles.MERGES.index(options["merge"]),
+            thresh=float(self.detector.cfg.iou_thresh if options["match_thresh"] is None else options["match_thresh"]),
+            border=None if options["border"] is None else float(options["border"]))
         self._nbox = sum(h * w for h, w in self.detector.out_hw) * self.detector.A      # boxes of one network input
-        self._view_dets = torch.zeros((self.batch, self.gather.C, self.gather.K, DET_WORDS), dtype=torch.int32, device=dev)
-        self._view_counts = torch.zeros((self.batch, self.gather.C), dtype=torch.int32, device=dev)
-        self._slot_yx = [torch.zeros((self.batch, 2), dtype=torch.float32, device=dev) for _ in range(SLOTS)]
+        if self._view_dets is None:
+            self._view_dets = torch.zeros((self.batch, self.gather.C, self.gather.K, DET_WORDS), dtype=torch.int32, device=dev)
+            self._view_counts = torch.zeros((self.batch, self.gather.C), dtype=torch.int32, device=dev)
+            self._slot_yx = [torch.zeros((self.batch, 2), dtype=torch.float32, device=dev) for _ in range(SLOTS)]
 
     def enable_png_decode(self) -> None:
         """From now on ``submit_images`` decodes the PNG files the GPU takes (``preprocess.png_gpu_decodable``: non-interlaced,
@@ -226,7 +254,8 @@ class DetectionPipeline:
         (world > 1) the all-gather on the side stream.  `image_hw`: device [n, 2] original sizes (default: the shared
         ``set_image_shapes`` tensor).  With `view_yx` (device [n, 2] origins) the n inputs are the views of n // V images: the
         decode writes the per-view block and the merge writes the gather slot.  `table` = (device address of the view offsets,
-        of the view sides, images) switches to ``k2y_merge_views_ex`` with the tiling's options.  Returns s."""
+        of the view sides, of the mirror flags or None, images) switches to ``k2y_merge_views_mirror`` with the tiling's options.
+        Returns s."""
         s = self._steps % SLOTS
         self._steps += 1
         compute = torch.cuda.current_stream(self.device_index)
@@ -246,13 +275,14 @@ class DetectionPipeline:
         elif table is not None:
             self.detector.run(heads, image_hw, dets_out=self._view_dets, counts_out=self._view_counts, stream=det)
             m = self._merge
-            off, sides, n_images = table
+            off, sides, mirror, n_images = table
             bordered = m["border"] is not None
-            check(lib.k2y_merge_views_ex(self._view_dets.data_ptr(), self._view_counts.data_ptr(), view_yx.data_ptr(), off,
-                                         sides if bordered else None, image_hw.data_ptr() if bordered else None,
-                                         m["border"] if bordered else -1.0, m["match"], m["merge"], n_images, self.batch, self._views,
-                                         self._nbox, self.gather.C, self.gather.K, m["thresh"], dets.data_ptr(), counts.data_ptr(),
-                                         dets.stride(0), counts.stride(0), ctypes.c_void_p(det.cuda_stream)))
+            check(lib.k2y_merge_views_mirror(self._view_dets.data_ptr(), self._view_counts.data_ptr(), view_yx.data_ptr(), off,
+                                             sides if bordered else None, mirror,
+                                             image_hw.data_ptr() if bordered or mirror is not None else None,
+                                             m["border"] if bordered else -1.0, m["match"], m["merge"], n_images, self.batch,
+                                             self._views, self._nbox, self.gather.C, self.gather.K, m["thresh"], dets.data_ptr(),
+                                             counts.data_ptr(), dets.stride(0), counts.stride(0), ctypes.c_void_p(det.cuda_stream)))
         else:
             self.detector.run(heads, image_hw, dets_out=self._view_dets, counts_out=self._view_counts, stream=det)
             check(lib.k2y_merge_views(self._view_dets.data_ptr(), self._view_counts.data_ptr(), view_yx.data_ptr(), n // self._views,
@@ -376,10 +406,11 @@ class DetectionPipeline:
         rank, rank r's images from row r * batch), or raises ``K2YError`` naming the JPEGs whose entropy-coded data was corrupt
         (their records would come from undefined pixels).  Same flow control as ``submit``.  Bad input raises ``ValueError``
         before anything is enqueued."""
-        if self._tiling is not None and isinstance(images, (list, tuple)) and len(images) > self.images_per_batch:
+        viewed = self._tiling is not None or self._flip
+        if viewed and isinstance(images, (list, tuple)) and len(images) > self.images_per_batch:
             raise ValueError(f"{len(images)} images of {self._views} views do not fit a batch of {self.batch}")
         layout = BatchLayout(images, self.in_hw, self._tiling, gpu_png=self._gpu_png, gpu_progressive=self._gpu_progressive,
-                             merge_table=self._merge is not None)
+                             merge_table=self._merge is not None, flip=self._flip)
         n = len(layout)
         if n > self.batch:
             raise ValueError(f"{n} images do not fit a batch of {self.batch}")
@@ -402,7 +433,7 @@ class DetectionPipeline:
         s = self._steps % SLOTS                  # the gather slot this batch's step will use
         with torch.cuda.device(dev):
             letterbox_packed(layout, images, self._staging[slot], buf, self._slot_hw[slot],
-                             self._slot_yx[slot] if self._tiling is not None else None)
+                             self._slot_yx[slot] if viewed else None)
             self._jpeg_idx[s] = [i for i, _ in layout.jpeg]
             if layout.jpeg:             # the status words travel to the host before the network starts on this slot
                 with torch.cuda.stream(self._copy_stream):
@@ -419,11 +450,11 @@ class DetectionPipeline:
         self._h2d_done[slot].record(self._copy_stream)
         nv = layout.n_views
         table = None
-        if layout.merge_table_at is not None:     # the view offsets and sides, where the H2D copy put them
+        if layout.merge_table_at is not None:     # the view offsets, sides and mirror flags, where the H2D copy put them
             at = self._staging[slot].dev.data_ptr() + layout.merge_table_at
-            table = (at, at + 4 * (n + 1), n)
+            table = (at, at + 4 * (n + 1), at + 4 * (n + 1 + nv) if self._flip else None, n)
         t = self._run_slot(slot, buf, nv, self._slot_hw[slot][:nv], n if self.world == 1 else None,
-                           self._slot_yx[slot][:nv] if self._tiling is not None else None, table)
+                           self._slot_yx[slot][:nv] if viewed else None, table)
         self._rendered_slot[t] = self._render is not None
         if self._render is not None:
             with torch.cuda.device(dev):
@@ -597,6 +628,12 @@ class LanedPipeline:
         for ln in self.lanes:
             ln.enable_tiling(rows, cols, overlap, tile_size=tile_size, images_per_batch=images_per_batch, match=match, merge=merge,
                              match_thresh=match_thresh, border=border)
+
+    def enable_flip(self, *, match: Optional[str] = None, merge: Optional[str] = None, match_thresh: Optional[float] = None,
+                    border: Optional[float] = None) -> None:
+        """``DetectionPipeline.enable_flip`` on every lane."""
+        for ln in self.lanes:
+            ln.enable_flip(match=match, merge=merge, match_thresh=match_thresh, border=border)
 
     @property
     def images_per_batch(self) -> int:

@@ -38,7 +38,7 @@ import torch
 
 from ._lib import JpegInfo, JpegProgressiveInfo, K2YError, PngInfo, check, lib
 from .helper import read_image
-from .tiles import tile_windows, view_sides
+from .tiles import SizedTiling, mirror_views, tile_windows, view_sides
 
 
 def letterbox_params(img_hw, in_hw):
@@ -255,11 +255,16 @@ class BatchLayout:
     of views, ``view_offsets`` int32 [n + 1] their running sum (image b's views are ``windows[view_offsets[b]:view_offsets[b+1]]``)
     and ``view_sides`` int32 [N] each window's interior sides (``tiles.view_sides``).
 
-    With `merge_table` (and a tiling) ``view_offsets`` and ``view_sides`` also go into the staging buffer, behind everything
-    else, at ``merge_table_at``, so that the batch's H2D copy takes them to the device for ``k2y_merge_views_ex``."""
+    With `flip` (with or without a tiling) each image's W windows (the whole image alone without a tiling) are followed by
+    the same W windows mirrored (``tiles.mirror_views``): ``view_mirror`` int32 [N] flags them, and their ``view_sides`` are
+    their windows' (the merge swaps left and right for a mirrored view).  Without `flip` ``view_mirror`` is None.
+
+    With `merge_table` (and a tiling or flip) ``view_offsets``, ``view_sides`` and, with `flip`, ``view_mirror`` also go into
+    the staging buffer, behind everything else, at ``merge_table_at``, so that the batch's H2D copy takes them to the device
+    for ``k2y_merge_views_ex`` / ``k2y_merge_views_mirror``."""
 
     def __init__(self, images: Sequence, in_hw, tiling=None, gpu_png: bool = False, gpu_progressive: bool = False,
-                 merge_table: bool = False):
+                 merge_table: bool = False, flip: bool = False):
         _check_images(images)
         n = len(images)
         self.in_hw = (int(in_hw[0]), int(in_hw[1]))
@@ -292,9 +297,11 @@ class BatchLayout:
         self.nbytes = int(padded.sum())
         self.matrices = np.array([letterbox_params((int(h[0]), int(h[1])), self.in_hw)[2][:2].reshape(-1) for h in self.hw], dtype=np.float64)
         self.views, self.windows, self.view_matrices = 1, None, None
-        self.view_counts, self.view_offsets, self.view_sides = None, None, None
-        if tiling is not None:
-            if isinstance(tiling, (tuple, list)):
+        self.view_counts, self.view_offsets, self.view_sides, self.view_mirror = None, None, None, None
+        if tiling is not None or flip:
+            if tiling is None:
+                what, plan = "flip", lambda h, w: np.array([(0, 0, h, w)], np.int32)      # noqa: E731
+            elif isinstance(tiling, (tuple, list)):
                 rows, cols, overlap = tiling
                 what = f"tiling {rows}x{cols}"
                 plan = lambda h, w: tile_windows(h, w, rows, cols, overlap)     # noqa: E731
@@ -304,11 +311,14 @@ class BatchLayout:
                 per_image = [plan(int(h), int(w)) for h, w in self.hw]
             except ValueError as e:
                 raise ValueError(f"{what}: {e}") from e
+            if flip:
+                per_image, mirror = zip(*[mirror_views(w) for w in per_image])
+                self.view_mirror = np.concatenate(mirror)
             self.windows = np.concatenate(per_image)
             self.view_counts = np.array([len(w) for w in per_image], np.int32)
             self.view_offsets = np.concatenate([[0], np.cumsum(self.view_counts)]).astype(np.int32)
             self.view_sides = np.concatenate([view_sides(w, int(h), int(wd)) for w, (h, wd) in zip(per_image, self.hw)])
-            self.views = len(self.windows) // n if isinstance(tiling, (tuple, list)) else None
+            self.views = None if isinstance(tiling, SizedTiling) else len(self.windows) // n
             self.view_matrices = np.array([letterbox_params((int(t[2]), int(t[3])), self.in_hw)[2][:2].reshape(-1) for t in self.windows],
                                           dtype=np.float64)
         self.jpeg_plan = None
@@ -331,7 +341,8 @@ class BatchLayout:
             self.staged_end = self.progressive_plan[3]
         self.merge_table_at = None
         if merge_table and self.windows is not None:
-            self.merge_table = np.concatenate([self.view_offsets, self.view_sides]).astype(np.int32)
+            self.merge_table = np.concatenate([self.view_offsets, self.view_sides] +
+                                              ([] if self.view_mirror is None else [self.view_mirror])).astype(np.int32)
             self.merge_table_at = (self.staged_end + ALIGN - 1) // ALIGN * ALIGN
             self.staged_end = self.merge_table_at + self.merge_table.nbytes
 
@@ -549,7 +560,7 @@ def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, ou
     are decoded into their place first (``stage_jpegs``), and so are the layout's GPU PNGs, whose range the same H2D copy moves
     (``stage_pngs``).  The host buffer is reused by the next call: wait for this copy
     before packing into it again.  A layout with tiling letterboxes its N = ``layout.n_views`` views instead
-    (``k2y_letterbox_u8_views``), image-major: ``out[:N]``, each view's (th, tw) into ``image_hw_out[:N]`` and its (y0, x0) into
+    (``k2y_letterbox_u8_views_mirror``, the mirrored ones flipped left to right), image-major: ``out[:N]``, each view's (th, tw) into ``image_hw_out[:N]`` and its (y0, x0) into
     ``view_yx_out[:N]`` (float32 [N, 2]); a layout's merge table goes to ``staging.dev`` at ``layout.merge_table_at`` in the
     same H2D copy as the rest."""
     n = len(layout)
@@ -583,13 +594,15 @@ def letterbox_packed(layout: BatchLayout, images: Sequence, staging: Staging, ou
         if layout.windows is not None:
             offsets = np.repeat(layout.offsets, layout.view_counts)
             hw = np.ascontiguousarray(np.repeat(layout.hw, layout.view_counts, axis=0))
-            check(lib.k2y_letterbox_u8_views(staging.dev.data_ptr(), layout.n_views, offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
-                                             hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
-                                             layout.windows.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
-                                             layout.view_matrices.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), out.data_ptr(), in_h,
-                                             in_w, image_hw_out.data_ptr() if image_hw_out is not None else None,
-                                             view_yx_out.data_ptr() if view_yx_out is not None else None, staging.minmax.data_ptr(),
-                                             ctypes.c_void_p(st.cuda_stream)))
+            mirror = None if layout.view_mirror is None else layout.view_mirror.ctypes.data_as(ctypes.POINTER(ctypes.c_int))
+            check(lib.k2y_letterbox_u8_views_mirror(staging.dev.data_ptr(), layout.n_views,
+                                                    offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
+                                                    hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+                                                    layout.windows.ctypes.data_as(ctypes.POINTER(ctypes.c_int)), mirror,
+                                                    layout.view_matrices.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), out.data_ptr(),
+                                                    in_h, in_w, image_hw_out.data_ptr() if image_hw_out is not None else None,
+                                                    view_yx_out.data_ptr() if view_yx_out is not None else None,
+                                                    staging.minmax.data_ptr(), ctypes.c_void_p(st.cuda_stream)))
             return
         hw = layout.hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int))
         mats = layout.matrices.ctypes.data_as(ctypes.POINTER(ctypes.c_double))

@@ -9,6 +9,10 @@ it stores), so no rounding depends on the platform.  ``DetectionPipeline.enable_
 
 ``plan_grid`` / ``plan_windows`` choose an image's grid from a tile size instead (``enable_tiling(tile_size=...)``), and
 ``view_sides`` tells which edges of each window lie inside the image, for the border drop of ``k2y_merge_views_ex``.
+
+With flip (``DetectionPipeline.enable_flip``) an image of W windows has 2W views: view ``v < W`` is window v, view ``W + v`` is
+window v mirrored left to right (``mirror_views``).  ``plan_views`` derives the views of every image, the images one batch
+holds and what the merge needs from the grid and the flip, in one place.
 """
 from __future__ import annotations
 
@@ -94,6 +98,13 @@ def view_sides(windows: np.ndarray, h: int, w: int) -> np.ndarray:
     return ((y0 > 0) * 1 + (x0 > 0) * 2 + (y0 + th < h) * 4 + (x0 + tw < w) * 8).astype(np.int32)
 
 
+def mirror_views(windows: np.ndarray):
+    """(int32 [2W, 4] windows, int32 [2W] mirror flags) of an image's W windows with flip: the windows as they are, then each
+    one again, mirrored."""
+    win = np.asarray(windows, np.int32).reshape(-1, 4)
+    return np.concatenate([win, win]), np.repeat(np.array([0, 1], np.int32), len(win))
+
+
 MATCHES = ("iou", "ios")
 MERGES = ("suppress", "union")
 
@@ -108,3 +119,30 @@ class SizedTiling:
 
     def windows(self, h: int, w: int) -> np.ndarray:
         return plan_windows(h, w, self.tile_hw, self.overlap, self.max_views)
+
+
+def plan_views(batch: int, max_per_class: int, max_records: int, grid=None, flip: bool = False):
+    """The views a pipeline of `batch` inputs detects each image as: (tiling, views, images_per_batch), where `tiling` is what
+    ``BatchLayout`` takes (None, (rows, cols, overlap) or a ``SizedTiling``), `views` the most views of one image (the merge's
+    max_views) and `images_per_batch` the images one batch holds.  `grid` is None (the whole image only), ("grid", rows, cols,
+    overlap) or ("size", (th, tw), overlap, images_per_batch); with `flip` every window is detected mirrored as well.
+      fixed grid (or none): V = (1 + rows * cols, or 1) * (2 with flip), images_per_batch = batch // V;
+      sized grid: max_views = min(batch // images_per_batch, max_records // max_per_class), windows planned under max_views
+                  (max_views // 2 with flip), views = that cap (doubled with flip).
+    ``ValueError`` when V exceeds the batch or V * max_per_class exceeds `max_records` (the records one merge holds), or when no
+    window fits a sized grid's cap."""
+    batch, K, limit, mult = int(batch), int(max_per_class), int(max_records), 2 if flip else 1
+    if grid is None or grid[0] == "grid":
+        rows, cols, overlap = (1, 1, 0) if grid is None else grid[1:]
+        V = (1 if grid is None else 1 + rows * cols) * mult
+        if V > batch:
+            raise ValueError(f"{V} views per image do not fit a batch of {batch}")
+        if V * K > limit:
+            raise ValueError(f"{V} views x {K} records per class exceed the {limit} records one merge holds")
+        return (None if grid is None else (rows, cols, overlap)), V, batch // V
+    _, tile_hw, overlap, ipb = grid
+    cap = min(batch // ipb, limit // K)
+    if cap // mult < 1:
+        raise ValueError(f"no view fits: {K} records per class exceed the {limit} records one merge holds" if cap < 1 else
+                         f"a flipped window takes 2 views and an image may have {cap}")
+    return SizedTiling(tile_hw, overlap, cap // mult), cap // mult * mult, ipb

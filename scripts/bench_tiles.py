@@ -12,11 +12,15 @@ whole image costs, on the bench_ingest photos as decoded pixels and as quality-9
   * with --tile_size H W --tile_images N, one more arm ("size"): each image cut into tiles of at most H x W pixels
     (``enable_tiling(tile_size=..., images_per_batch=N)``), timed like the others, checked against oracle/tiles_merge_ref.py,
     and ``k2y_merge_views_ex`` timed on one of its batches in every metric / action mode, and with a border.
+  * with --flip, two more arms: "flip" (every image and its mirror, ``enable_flip``) and "2x2+flip" (2x2 tiles and the whole
+    image, each also mirrored), timed like the others, checked against the composed reference of oracle/flip_ref.py
+    (the crops and their np.fliplr through the untiled pipeline, then the merge with the mirror flags), and the mirrored
+    letterbox (``k2y_letterbox_u8_views_mirror``) and merge (``k2y_merge_views_mirror``) timed on one of their batches.
 
 The card's name, power limit and SM clock are read in the same run.  Prints one JSON line.
 
     python scripts/bench_tiles.py [--images 192 --batch 32 --windows 3 --passes 4 --launches 200 --tile_size 224 320
-                                   --tile_images 6]
+                                   --tile_images 6 --flip]
 """
 import argparse
 import ctypes
@@ -90,6 +94,31 @@ def composed(plain, images, rows, cols, overlap, iou):
     return out
 
 
+def composed_flip(plain, images, images_per_batch, rows_cols, overlap, iou):
+    """The crops of every view and their mirrors through the untiled pipeline, one flipped batch's views per batch, then the
+    numpy merge with the mirror flags."""
+    from oracle import flip_ref
+    out = []
+    for i in range(0, len(images), images_per_batch):
+        chunk = images[i:i + images_per_batch]
+        per = [tiles.tile_windows(im.shape[0], im.shape[1], *rows_cols, overlap) if rows_cols else
+               np.array([(0, 0, im.shape[0], im.shape[1])], np.int32) for im in chunk]
+        crops, windows, mirror = [], [], []
+        for im, w in zip(chunk, per):
+            cut = [np.ascontiguousarray(im[y0:y0 + th, x0:x0 + tw]) for y0, x0, th, tw in w.tolist()]
+            crops += cut + [np.ascontiguousarray(np.fliplr(c)) for c in cut]
+            windows += [w, w]
+            mirror += [0] * len(w) + [1] * len(w)
+        windows = np.concatenate(windows)
+        offsets = np.concatenate([[0], np.cumsum([2 * len(w) for w in per])])
+        d, c = plain.collect(plain.submit_images(crops))
+        dets, counts = flip_ref.merge_views(d.numpy(), c.numpy(), windows[:, :2], offsets, NBOX, iou, view_hw=windows[:, 2:],
+                                       mirrored=np.array(mirror))
+        out += [[(cls, int(r["index"]), float(r["score"]), float(r["ymin"]), float(r["xmin"]), float(r["ymax"]), float(r["xmax"]))
+                 for cls in range(dets.shape[1]) for r in dets[b, cls, :counts[b, cls]]] for b in range(len(chunk))]
+    return out
+
+
 def events_ms(fn, launches):
     """Milliseconds per call of `fn` over `launches` calls on the current stream, after 10 warm-up calls."""
     for _ in range(10):
@@ -108,7 +137,8 @@ def kernel_times(pipe, images, launches):
     pipeline tiled by size the merge time is a dict: ``k2y_merge_views_ex`` in every metric / action mode, and with a border."""
     imgs = images[:pipe.images_per_batch]
     sized = pipe._merge is not None
-    layout = preprocess.BatchLayout(imgs, pipe.in_hw, pipe._tiling, merge_table=sized)
+    flip = pipe._flip
+    layout = preprocess.BatchLayout(imgs, pipe.in_hw, pipe._tiling, merge_table=sized, flip=flip)
     n, N, V = len(layout), layout.n_views, pipe._views
     dev = torch.device("cuda", pipe.device_index)
     st = torch.cuda.current_stream()
@@ -119,6 +149,14 @@ def kernel_times(pipe, images, launches):
     preprocess.letterbox_packed(layout, imgs, staging, out, hw, yx)     # packs and copies the batch; the loop below only letterboxes
     offsets = np.repeat(layout.offsets, layout.view_counts)
     full = np.ascontiguousarray(np.repeat(layout.hw, layout.view_counts, axis=0))
+
+    def letterbox_mirror():
+        check(lib.k2y_letterbox_u8_views_mirror(
+            staging.dev.data_ptr(), N, offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
+            full.ctypes.data_as(ctypes.POINTER(ctypes.c_int)), layout.windows.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+            layout.view_mirror.ctypes.data_as(ctypes.POINTER(ctypes.c_int)),
+            layout.view_matrices.ctypes.data_as(ctypes.POINTER(ctypes.c_double)), out.data_ptr(), pipe.in_hw[0], pipe.in_hw[1],
+            hw.data_ptr(), yx.data_ptr(), staging.minmax.data_ptr(), ctypes.c_void_p(st.cuda_stream)))
 
     def letterbox():
         check(lib.k2y_letterbox_u8_views(staging.dev.data_ptr(), N, offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_longlong)),
@@ -147,6 +185,15 @@ def kernel_times(pipe, images, launches):
             pipe.gather.K, pipe.detector.cfg.iou_thresh, dets.data_ptr(), counts.data_ptr(), dets.stride(0), counts.stride(0),
             ctypes.c_void_p(st.cuda_stream)))
 
+    def merge_mirror():
+        table = staging.dev.data_ptr() + layout.merge_table_at
+        check(lib.k2y_merge_views_mirror(
+            pipe._view_dets.data_ptr(), pipe._view_counts.data_ptr(), yx.data_ptr(), table, None, table + 4 * (n + 1 + N),
+            hw.data_ptr(), -1.0, 0, 0, n, pipe.batch, V, NBOX, pipe.gather.C, pipe.gather.K, pipe.detector.cfg.iou_thresh,
+            dets.data_ptr(), counts.data_ptr(), dets.stride(0), counts.stride(0), ctypes.c_void_p(st.cuda_stream)))
+
+    if flip:
+        return events_ms(letterbox_mirror, launches), events_ms(merge_mirror, launches), N
     if not sized:
         return events_ms(letterbox, launches), events_ms(merge, launches), N
     modes = {f"{m}/{a}": (i, j, None) for i, m in enumerate(("iou", "ios")) for j, a in enumerate(("suppress", "union"))}
@@ -164,6 +211,7 @@ def main():
     ap.add_argument("--obj_thresh", type=float, default=0.3)
     ap.add_argument("--tile_size", type=int, nargs=2, default=None, metavar=("H", "W"), help="add an arm tiled by tile size")
     ap.add_argument("--tile_images", type=int, default=6, help="images per batch of the --tile_size arm")
+    ap.add_argument("--flip", action="store_true", help="add the arms flip (each image and its mirror) and 2x2+flip")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_tiles measures on a GPU"
     from PIL import Image
@@ -175,13 +223,19 @@ def main():
     tilings = dict(TILINGS)
     if args.tile_size:
         tilings["size"] = "size"
+    if args.flip:
+        tilings["flip"], tilings["2x2+flip"] = "flip", (2, 2, "flip")
     for name, t in tilings.items():
         pipes[name] = DetectionPipeline("yolo_mobilev1", (H, W), anchors, 20, 0.75, args.batch, obj_thresh=args.obj_thresh, iou_thresh=0.5)
         pipes[name].engine.set_weights(weights)
         if t == "size":
             pipes[name].enable_tiling(tile_size=tuple(args.tile_size), images_per_batch=args.tile_images)
+        elif t == "flip":
+            pipes[name].enable_flip()
         elif t:
-            pipes[name].enable_tiling(*t)
+            pipes[name].enable_tiling(*t[:2])
+            if t[2:] == ("flip",):
+                pipes[name].enable_flip()
     pixels = photos(args.images)
     files = []
     for img in pixels:
@@ -205,6 +259,12 @@ def main():
                                                                          p.images_per_batch, p._views, 0.2, 0.5)
         views_per_image["size"] = float(np.mean([len(tiles.plan_windows(im.shape[0], im.shape[1], tuple(args.tile_size), 0.2, p._views))
                                                  for im in pixels]))
+    if args.flip:
+        for name, rc in (("flip", None), ("2x2+flip", (2, 2))):
+            p = pipes[name]
+            k = 4 * p.images_per_batch
+            equal[name] = first[(name, "pixels")][:k] == composed_flip(pipes["off"], pixels[:k], p.images_per_batch, rc, 0.2, 0.5)
+            views_per_image[name] = p._views
     records = {f"{name}/{r}": sum(len(x) for x in v) for (name, r), v in first.items()}
 
     times = {k: [] for k in first}
@@ -228,7 +288,7 @@ def main():
         "network_inputs_per_s": {f"{n}/{r}": round(v * views_per_image[n], 1) for (n, r), v in rate.items()},
         "views_per_image": views_per_image, "tile_size": args.tile_size, "tile_images": args.tile_images if args.tile_size else None,
         "windows_s": {f"{n}/{r}": [round(t, 4) for t in v] for (n, r), v in times.items()},
-        "records": records, "kernels": kernels, "launches": args.launches, "equals_composed_reference": equal, "gpu": gpu_info()}))
+        "flip": args.flip, "records": records, "kernels": kernels, "launches": args.launches, "equals_composed_reference": equal, "gpu": gpu_info()}))
     if not all(equal.values()):
         sys.exit("tiled records differ from the composed reference")
 

@@ -24,6 +24,9 @@ DetectionPipeline.enable_tiling): a batch then holds batch // (1 + ROWS * COLS) 
 and the lines keep their shape, with "index" // (boxes per network input) telling the view a detection came from.
 --tile_size H W --tile_images N plans each image's grid from its own size instead (tiles of at most H x W pixels, a batch of N
 images); --tile_match ios, --tile_merge union and --tile_border PX change how the views' records are merged (either grid).
+With --flip every view (the whole image, or each of its tiles) is also detected mirrored left to right, the test-time
+augmentation of a detector trained with random flips (DetectionPipeline.enable_flip): a batch then holds half the images, and the
+mirrored views' records are mapped back and merged with the rest on the GPU.  It combines with every tiling flag.
 
 With --gpu_png the PNG files the GPU decoder takes (preprocess.png_gpu_decodable) stay compressed too and are decoded on the GPU
 (DetectionPipeline.enable_png_decode), with the pixels PIL gives; the lines are the same as without it.  --gpu_progressive does
@@ -88,6 +91,8 @@ def open_pipeline(args, max_per_class=30):
         pipe.enable_tiling(args.tiles[0], args.tiles[1], args.tile_overlap, **options)
     elif getattr(args, "tile_size", None):
         pipe.enable_tiling(overlap=args.tile_overlap, tile_size=tuple(args.tile_size), images_per_batch=args.tile_images, **options)
+    if getattr(args, "flip", False):
+        pipe.enable_flip(**options)
     if getattr(args, "gpu_png", False):
         pipe.enable_png_decode()
     if getattr(args, "gpu_progressive", False):
@@ -204,6 +209,8 @@ def add_model_args(ap):
                     help="drop a matching record, or also grow the kept record's box to the union of the records it suppressed")
     ap.add_argument("--tile_border", type=float, default=None, metavar="PX",
                     help="drop a tile's records within PX pixels of a tile edge inside the image before the merge")
+    ap.add_argument("--flip", action="store_true",
+                    help="also detect every view mirrored left to right and merge both on the GPU (a batch holds half the images)")
     ap.add_argument("--gpu_png", action="store_true",
                     help="decode the PNG files the GPU decoder takes on the GPU too (the same pixels as PIL), not in the host threads")
     ap.add_argument("--gpu_progressive", action="store_true",
