@@ -7,7 +7,9 @@
 // puts the blob next to the compressed bytes in pinned memory, so one H2D copy moves both.
 //
 // Device side, one launch per stage whatever the image count:
-//   1. jpeg_unstuff_kernel   (CTA per image)   drops the 0x00 after each 0xFF, cuts the entropy data at RSTn markers
+//   1. jpeg_unstuff_kernel   (CTA per image)   drops the 0x00 after each 0xFF, cuts the entropy data at RSTn markers and
+//                            checks their numbers (the k-th between intervals must be RST(k mod 8)); a marker past the
+//                            last interval ends the data
 //   2. jpeg_huffman_kernel   (CTA per segment) self-synchronising Huffman decode (Weissenberger & Schmidt): each thread owns
 //                            a fixed-length subsequence of the segment's bits, decodes it from a guessed state, then restarts
 //                            from its left neighbour's exact end state until its own end state stops changing; an exclusive
@@ -229,9 +231,9 @@ __device__ __forceinline__ const JpegBlobHeader &hdr(const uint8_t *blob) { retu
 __device__ __forceinline__ const JpegImg *imgs(const uint8_t *blob) { return reinterpret_cast<const JpegImg *>(blob + hdr(blob).img_off); }
 
 __global__ void __launch_bounds__(UNSTUFF_THREADS) jpeg_unstuff_kernel(const uint8_t *__restrict__ blob, const uint8_t *__restrict__ src,
-                                                                       uint8_t *__restrict__ ws) {
+                                                                       uint8_t *__restrict__ ws, int *__restrict__ status) {
     __shared__ int sh[32];
-    __shared__ int s_term;
+    __shared__ int s_term, s_last, s_order;
     const JpegImg &im = imgs(blob)[blockIdx.x];
     const uint8_t *s = src + im.src_offset;
     const long long n = im.src_end - im.src_offset;
@@ -241,6 +243,10 @@ __global__ void __launch_bounds__(UNSTUFF_THREADS) jpeg_unstuff_kernel(const uin
     long long term = n;
     int out_total = 0, rst_total = 0;
     const int tile = UNSTUFF_THREADS * UNSTUFF_BYTES;
+    if (threadIdx.x == 0) {
+        s_last = 0x7fffffff;
+        s_order = 0;
+    }
     for (long long base = 0; base < term; base += tile) {
         const long long b0 = base + (long long)threadIdx.x * UNSTUFF_BYTES;
         const long long b1 = min(b0 + UNSTUFF_BYTES, n);
@@ -281,7 +287,12 @@ __global__ void __launch_bounds__(UNSTUFF_THREADS) jpeg_unstuff_kernel(const uin
             } else if (prev == 0xFF && (cur == 0x00 || (cur >= 0xD0 && cur <= 0xD7))) {
                 if (cur != 0x00) {
                     ++r;
-                    if (r < nseg) seg[r] = o;
+                    if (r < nseg) {
+                        seg[r] = o;
+                        if ((cur & 7) != ((r - 1) & 7)) s_order = 1;
+                    } else if (r == nseg) {
+                        s_last = o;
+                    }
                 }
             } else {
                 u[o++] = (uint8_t)cur;
@@ -295,11 +306,15 @@ __global__ void __launch_bounds__(UNSTUFF_THREADS) jpeg_unstuff_kernel(const uin
     for (int k = rst_total + 1 + threadIdx.x; k < nseg; k += blockDim.x) seg[k] = out_total;
     if (threadIdx.x == 0) {
         seg[0] = 0;
-        seg[nseg] = out_total;
+        // a marker past the last interval (or any with no restart interval) ends the data, where libjpeg stops reading it
+        seg[nseg] = min(out_total, s_last);
+        // a marker between intervals out of sequence: libjpeg-turbo resynchronises, which this decode does not model
+        if (s_order) atomicOr(status + 4 * blockIdx.x, 4);
     }
 }
 
-// status words per image: [0] error bits (1 bad Huffman code, 2 premature end of data), [1] max sync rounds of a window,
+// status words per image: [0] error bits (1 bad Huffman code, 2 premature end of data, 4 a restart marker between intervals
+// out of sequence), [1] max sync rounds of a window,
 // [2] sum of sync rounds over windows, [3] windows
 __global__ void __launch_bounds__(SYNC_THREADS) jpeg_huffman_kernel(const uint8_t *__restrict__ blob, uint8_t *__restrict__ ws,
                                                                     int *__restrict__ status) {
@@ -662,7 +677,7 @@ extern "C" int k2y_jpeg_decode(const void *blob_host, const void *blob_dev, cons
     uint8_t *ws = static_cast<uint8_t *>(workspace_dev);
     K2Y_CUDA_CHECK(cudaMemsetAsync(status_dev, 0, sizeof(int32_t) * 4 * (size_t)H->n, st));
     K2Y_CUDA_CHECK(cudaMemsetAsync(ws + H->ws_coef, 0, (size_t)(H->ws_plane - H->ws_coef), st));
-    jpeg_unstuff_kernel<<<H->n, UNSTUFF_THREADS, 0, st>>>(blob, src_dev, ws);
+    jpeg_unstuff_kernel<<<H->n, UNSTUFF_THREADS, 0, st>>>(blob, src_dev, ws, status_dev);
     jpeg_huffman_kernel<<<H->nseg, SYNC_THREADS, 0, st>>>(blob, ws, status_dev);
     jpeg_dc_kernel<<<H->nseg, DC_THREADS, 0, st>>>(blob, ws);
     jpeg_idct_kernel<<<dim3((unsigned)((H->max_blocks + IDCT_THREADS - 1) / IDCT_THREADS), H->n), IDCT_THREADS, 0, st>>>(blob, ws);

@@ -7,16 +7,20 @@
 // force at the scan.  Quantisation tables are latched at each component's first scan, as jdinput.c latches them.  A file
 // stays on the host when libjpeg-turbo would decode it with a JWRN_BOGUS_PROGRESSION warning, when its script leaves
 // libjpeg-turbo to block-smooth the output (jdcoefct.c smoothing_ok: a component's DC is known but one of its zig-zag
-// coefficients 1..9 is not fully known), or when it has more than PROG_MAX_SCANS scans.
+// coefficients 1..9 is not fully known), when it has more than PROG_MAX_SCANS scans, or when a scan's restart markers are
+// out of sequence (the k-th marker between its intervals not RST(k mod 8), too few of them, or any with no restart interval:
+// libjpeg-turbo's resynchronisation then drops or rereads data, which the decoder does not model).
 //
 // The descriptor blob (ProgBlobHeader, ProgImg[n], ProgScan[scans], ProgSeg[segments], JpegHuff[tables]) lists every
-// (scan, restart interval) segment with its byte range in the file.  Each scan gets a level: 0 when no earlier scan touched
-// any of its (component, coefficient) pairs, else one more than the highest level of those that did.  Scans of one level
-// write disjoint coefficient bits and read none another scan of the level writes, so they decode concurrently; the segments
-// are sorted by level.
+// (scan, restart interval) segment with its byte range in the file.  Each scan gets a level from the (component,
+// coefficient) pairs it may write: 0 when no earlier scan may write any of them, else one more than the highest level of
+// those that may.  A scan may write past its band: jdphuff.c indexes the natural order (whose last sixteen entries are 63)
+// at k after a run, so an AC first scan may write zig-zag Ss..min(63, Se + 15) and an AC refinement Ss..min(63, Se + 1).
+// Scans that may write a common coefficient thus decode in file order, and scans of one level write disjoint coefficients
+// and read none another scan of the level writes, so they decode concurrently; the segments are sorted by level.
 //
 // Device side:
-//   1. prog_entropy_kernel  one launch per level (a default libjpeg script has three), one thread per segment in a CTA of
+//   1. prog_entropy_kernel  one launch per level (a default libjpeg script has four), one thread per segment in a CTA of
 //                           its own, decoding the segment serially from its bytes as they lie in the file (stuffing and
 //                           fill bytes dropped on the fly): DC first (prediction in the unshifted domain, stored as
 //                           (JCOEF)((unsigned)v << Al)), DC refine (one raw bit per block), AC first (EOB runs across
@@ -163,7 +167,6 @@ struct ProgHook : ScanHook {
         }
         // the progression as jdphuff.c tracks it: scripts it warns about (JWRN_BOGUS_PROGRESSION) stay on the host, and so
         // does a first scan of a coefficient that was already sent
-        int level = 0;
         for (int k = 0; k < p.ns; ++k) {
             const int c = p.scan_comp[k];
             r.comp[k] = c;
@@ -175,13 +178,37 @@ struct ProgHook : ScanHook {
                 if (p.ah != 0 && p.ah != coef_bits[c][z] && !bogus[0])
                     snprintf(bogus, sizeof(bogus), "scan %d: refinement Ah=%d of coefficient %d of component %d", si, p.ah, z, c);
                 coef_bits[c][z] = p.al;
-                level = std::max(level, last_level[c][z] + 1);
             }
         }
+        // the level, from the coefficients the scan may write rather than its band: jdphuff.c writes a run that ends past Se
+        // through the natural order's trailing 63s, up to Se + 15 in an AC first scan and Se + 1 in an AC refinement
+        const int reach = dc ? 0 : std::min(63, p.se + (p.ah == 0 ? 15 : 1));
+        int level = 0;
         for (int k = 0; k < p.ns; ++k)
-            for (int z = p.ss; z <= p.se; ++z) last_level[r.comp[k]][z] = level;
+            for (int z = p.ss; z <= reach; ++z) level = std::max(level, last_level[r.comp[k]][z] + 1);
+        for (int k = 0; k < p.ns; ++k)
+            for (int z = p.ss; z <= reach; ++z) last_level[r.comp[k]][z] = level;
         r.level = level;
         nlevel = std::max(nlevel, level + 1);
+        // restart intervals the scan needs; libjpeg-turbo resynchronises on a marker out of sequence, which the decoder does
+        // not model, so such a file stays on the host
+        long long mcus = 0;
+        {
+            int hmax = 1, vmax = 1;
+            for (int c = 0; c < p.ncomp && p.ncomp > 1; ++c) {
+                hmax = std::max(hmax, p.hs[c]);
+                vmax = std::max(vmax, p.vs[c]);
+            }
+            if (p.ns == 1) {
+                const int c = r.comp[0], hc = p.ncomp > 1 ? p.hs[c] : 1, vc = p.ncomp > 1 ? p.vs[c] : 1;
+                const long long dw = ((long long)p.w * hc + hmax - 1) / hmax, dh = ((long long)p.h * vc + vmax - 1) / vmax;
+                mcus = ((dw + 7) / 8) * ((dh + 7) / 8);
+            } else {
+                mcus = (long long)((p.w + 8 * hmax - 1) / (8 * hmax)) * ((p.h + 8 * vmax - 1) / (8 * vmax));
+            }
+        }
+        const long long need = p.restart && mcus > 0 ? (mcus + p.restart - 1) / p.restart - 1 : 0;   // markers between intervals
+        long long seen = 0;
         // the entropy-coded data: up to the first marker that is neither a stuffed zero, a fill byte nor RSTn
         size_t j = data_at;
         r.bounds.push_back((long long)j);
@@ -202,6 +229,12 @@ struct ProgHook : ScanHook {
             } else if (nx == 0xFF) {
                 j += 1;
             } else if (nx >= 0xD0 && nx <= 0xD7) {
+                if (!p.restart && !bogus[0])
+                    snprintf(bogus, sizeof(bogus), "scan %d: RST%d with no restart interval", si, nx - 0xD0);
+                else if (seen < need && nx - 0xD0 != (int)(seen % 8) && !bogus[0])
+                    snprintf(bogus, sizeof(bogus), "scan %d: restart marker %lld is RST%d, not RST%d", si, seen, nx - 0xD0,
+                             (int)(seen % 8));
+                ++seen;
                 r.bounds.push_back((long long)j);
                 r.bounds.push_back((long long)j + 2);
                 j += 2;
@@ -209,6 +242,7 @@ struct ProgHook : ScanHook {
                 break;
             }
         }
+        if (seen < need && !bogus[0]) snprintf(bogus, sizeof(bogus), "scan %d: %lld restart markers of %lld", si, seen, need);
         r.bounds.push_back((long long)j);
         resume = j;
         if (si < PROG_MAX_SCANS) scans.push_back(std::move(r));

@@ -689,12 +689,16 @@ def decode_jpeg_batch(files: Sequence, stream: Optional[torch.cuda.Stream] = Non
 
 
 def check_jpeg_status(status: np.ndarray, images) -> None:
-    """Raises ``K2YError`` naming the images whose entropy-coded data was corrupt or ended early.  `status`: the decode's
-    int32 [n, 4] words of the GPU-decoded JPEGs, `images`: their positions in the caller's batch."""
+    """Raises ``K2YError`` naming the images whose entropy-coded data was corrupt, ended early or had its restart markers out
+    of sequence.  `status`: the decode's int32 [n, 4] words of the GPU-decoded JPEGs, `images`: their positions in the
+    caller's batch."""
     bad = [(int(i), int(w)) for i, w in zip(images, status[:, 0]) if w]
     if bad:
-        what = {1: "invalid Huffman code", 2: "entropy-coded data ends early", 3: "invalid Huffman code, data ends early"}
-        raise K2YError("corrupt JPEG data: " + ", ".join(f"image {i}: {what.get(w, w)}" for i, w in bad))
+        raise K2YError("corrupt JPEG data: " + ", ".join(
+            f"image {i}: " + ", ".join(v for k, v in JPEG_ERRORS.items() if w & k) for i, w in bad))
+
+
+JPEG_ERRORS = {1: "invalid Huffman code", 2: "entropy-coded data ends early", 4: "restart marker out of sequence"}
 
 
 def decode_png_batch(files: Sequence, stream: Optional[torch.cuda.Stream] = None, with_status: bool = False):

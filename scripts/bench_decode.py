@@ -15,7 +15,8 @@ and the card's name, power limit and SM clock, read in the same run.  Prints one
 
 With --progressive the files are the same photos saved by PIL as progressive JPEGs (quality 90, 4:2:0, libjpeg's default
 scan script), the decode is k2y_jpeg_progressive_decode (the pipeline's enable_progressive_jpeg_decode), the kernel split
-gives each entropy-decode level on its own (level 0: every first scan; levels 1 and 2: the refinements), and the JSON adds
+gives each entropy-decode level on its own (level 0: the DC, chroma and luma 1..5 first scans; level 1: the luma 6..63
+first scan and the DC and chroma refinements; levels 2 and 3: the luma refinements), and the JSON adds
 the host milliseconds BatchLayout takes to parse and plan a batch of the files and to write its descriptor blob.
 
     python scripts/bench_decode.py [--progressive] [--images 256 --batch 32 --windows 3 --passes 4 --decode_reps 50]

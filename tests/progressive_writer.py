@@ -11,6 +11,10 @@ jcphuff.c's MAX_CORR_BITS).  EOB runs end at each restart marker and at the end 
 every scan or one per scan (a DRI marker goes before each scan whose interval differs from the one in force).  `huffman`:
 "optimal" (jpeg_gen_optimal_table per scan, as libjpeg-turbo's progressive mode does) or "flat" (every symbol a scan uses
 at one length).  Each scan's tables are defined by a DHT right before its SOS.
+
+`write_scans(qtables, height=, width=, sampling=, scans=)` writes a frame from explicit entropy-coded items instead: per scan
+and restart segment, the Huffman symbols and raw bit fields `_Seg` holds, with tables built from the symbols each scan uses
+(or given), any RSTn numbering, markers left out or added, fill bytes before markers and in the data, and zero padding.
 """
 from __future__ import annotations
 
@@ -238,3 +242,80 @@ def known_coefs(coefs: Sequence[np.ndarray], script, ncomp: int) -> List[np.ndar
                 x[:, pos] = np.sign(x[:, pos]) * ((np.abs(x[:, pos]) >> s) << s)
         out.append(x.reshape(np.asarray(coefs[c]).shape))
     return out
+
+
+def write_scans(qtables: Dict[int, np.ndarray], *, height: int, width: int, sampling: Sequence[Tuple[int, int]],
+                scans: Sequence[dict], tq: Sequence[int] = None, ids: Sequence[int] = None, jfif: bool = True) -> bytes:
+    """A progressive file from explicit entropy-coded items, for bitstreams jcphuff.c never writes.
+
+    Each scan is a dict: ``comps``, ``ss``, ``se``, ``ah``, ``al`` as in a script entry; ``segs``: one item list per restart
+    segment, items ("s", table, symbol) (table: index of the component in a DC first scan, else 0) or ("b", value, nbits)
+    as ``_Seg`` holds them; optional:
+      huffman  "flat" (default), "optimal", or {table: (bits, values)}; a DHT with the scan's tables goes right before its SOS
+      restart  the DRI interval in force (a DRI marker goes before the scan when it differs from the one in force; default 0)
+      markers  the number n of the RSTn written after each segment but the last (default k % 8), None to leave a marker out
+      extra    the number of one more RSTn after the last segment (default none)
+      pad      "ones" (default) or "zeros" to the byte boundary at each segment's end
+      fill     0xFF fill bytes before each RSTn and before the next marker after the scan
+      fill_data  0xFF fill bytes before each stuffed 0xFF 0x00 in the data
+    """
+    n = len(sampling)
+    tq = list(tq) if tq is not None else [0] + [1] * (n - 1)
+    ids = list(ids) if ids is not None else list(range(1, n + 1))
+    out = b"\xff\xd8"
+    if jfif:
+        out += J._segment(0xE0, b"JFIF\x00\x01\x01\x00\x00\x01\x00\x01\x00\x00")
+    qt = {t: np.asarray(q, np.int64).reshape(64) for t, q in qtables.items()}
+    out += J._segment(0xDB, J._dqt(qt, {t: int(q.max() > 255) for t, q in qt.items()}))
+    sof = bytes([8]) + height.to_bytes(2, "big") + width.to_bytes(2, "big") + bytes([n])
+    for c in range(n):
+        sof += bytes([ids[c], (sampling[c][0] << 4) | sampling[c][1], tq[c]])
+    out += J._segment(0xC2, sof)
+    dri = 0
+    for sc in scans:
+        comps, ss, se, ah, al = list(sc["comps"]), sc["ss"], sc["se"], sc["ah"], sc["al"]
+        segs = sc["segs"]
+        ntab = len(comps) if ss == 0 else 1
+        cls = "dc" if ss == 0 else "ac"
+        htabs = {}
+        if not (ss == 0 and ah != 0):
+            freq = [dict() for _ in range(ntab)]
+            for items in segs:
+                for it in items:
+                    if it[0] == "s":
+                        freq[it[1]][it[2]] = freq[it[1]].get(it[2], 0) + 1
+            huff = sc.get("huffman", "flat")
+            for t in range(ntab):
+                f = freq[t] or {0: 1}
+                if isinstance(huff, dict):
+                    htabs[(cls, t)] = huff[t]
+                elif huff == "optimal":
+                    htabs[(cls, t)] = J.optimal_table(f)
+                else:
+                    htabs[(cls, t)] = J.flat_table(sorted(f), max(1, len(f).bit_length()))
+            out += J._segment(0xC4, J._dht(htabs))
+        rst = sc.get("restart", 0)
+        if rst != dri:
+            out += J._segment(0xDD, rst.to_bytes(2, "big"))
+            dri = rst
+        sos = bytes([len(comps)])
+        for k, c in enumerate(comps):
+            sos += bytes([ids[c], (k << 4) if ss == 0 else 0])
+        out += J._segment(0xDA, sos + bytes([ss, se, (ah << 4) | al]))
+        codes = {t: J._codes(htabs[(cls, t)]) for t in range(ntab)} if htabs else {}
+        markers = sc.get("markers") or [k % 8 for k in range(len(segs) - 1)]
+        fill, pad = b"\xff" * sc.get("fill", 0), sc.get("pad", "ones")
+        for si, items in enumerate(segs):
+            words = [codes[t][sym] if kind == "s" else (t, sym) for kind, t, sym in items]
+            bits = J._bit_array(np.array([a for a, _ in words], np.int64), np.array([b for _, b in words], np.int64))
+            npad = (-len(bits)) % 8
+            bits = np.concatenate([bits, np.ones(npad, np.uint8) if pad == "ones" else np.zeros(npad, np.uint8)])
+            data = J._stuff(bits)
+            if sc.get("fill_data"):
+                data = data.replace(b"\xff\x00", b"\xff" * sc["fill_data"] + b"\xff\x00")
+            out += data
+            num = markers[si] if si + 1 < len(segs) else sc.get("extra")
+            if num is not None:
+                out += fill + bytes([0xFF, 0xD0 + num])
+        out += fill
+    return out + b"\xff\xd9"

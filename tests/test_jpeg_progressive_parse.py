@@ -64,14 +64,14 @@ def patch_scan(data, index, ss=None, se=None, ah=None, al=None):
     return bytes(d)
 
 
-def test_pil_progressive_files_are_gpu_decodable_and_the_baseline_view_is_unchanged():
+def test_pil_progressive_files_decode_in_four_levels_and_the_baseline_view_is_unchanged():
     img = photo(37, 53, 2)
     for kw in ({}, {"subsampling": 0}, {"subsampling": 1}, {"restart_marker_blocks": 1}, {"restart_marker_rows": 1}):
         f = pil_progressive(img, **kw)
         assert preprocess.inspect_jpeg_progressive(f) == (37, 53, True, "")
         assert preprocess.progressive_gpu_decodable(f)
         i = info(f)
-        assert (i.scans, i.levels, i.sof_marker) == (10, 3, 0xC2)    # libjpeg's default script: three entropy launches
+        assert (i.scans, i.levels, i.sof_marker) == (10, 4, 0xC2)    # libjpeg's default script: four entropy launches
         assert preprocess.inspect_jpeg(f) == (37, 53, False, "progressive (SOF 0xC2)")
         assert not preprocess.gpu_decodable(f)
         with pytest.raises(K2YError, match="not decodable on the GPU: progressive"):
