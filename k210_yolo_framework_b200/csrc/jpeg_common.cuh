@@ -3,6 +3,7 @@
 // and ycc_rgb_convert) as device functions over an image descriptor with the same field names in both decoders.
 #pragma once
 #include "common.h"
+#include "jpeg_std_huff.cuh"
 
 #include <algorithm>
 #include <cstdarg>
@@ -310,6 +311,20 @@ int parse_jpeg(const uint8_t *d, size_t n, Parsed &p, const char *who, ScanHook 
         const int rc = hook->finish(p, eoi, who);
         if (rc != K2Y_OK || p.reason[0]) return rc;
     }
+    // jdhuff.c jinit_huff_decoder -> std_huff_tables: a sequential scan's DC / AC slots 0 and 1 that no DHT defined take the
+    // Annex K.3 tables, each slot on its own (Motion-JPEG frames leave them out); an undefined slot 2 or 3 stays an error
+    for (int s = 0; !hook && s < 2; ++s)
+        for (int ac = 0; ac < 2; ++ac) {
+            HuffSpec &hs = ac ? p.ac[s] : p.dc[s];
+            if (hs.defined) continue;
+            const int t = 2 * s + ac;
+            int count = 0;
+            hs.defined = true;
+            hs.bits[0] = 0;
+            for (int l = 1; l <= 16; ++l) count += hs.bits[l] = kHuffBits[t][l - 1];
+            memset(hs.vals, 0, sizeof(hs.vals));
+            memcpy(hs.vals, huff_vals(t), count);
+        }
     for (int k = 0; !hook && k < p.ns; ++k) {
         if (!p.dc[p.td[k]].defined || !p.ac[p.ta[k]].defined)
             return set_reason(p, "Huffman table not defined before the scan"), K2Y_OK;

@@ -32,6 +32,13 @@ With --gpu_png the PNG files the GPU decoder takes (preprocess.png_gpu_decodable
 (DetectionPipeline.enable_png_decode), with the pixels PIL gives; the lines are the same as without it.  --gpu_progressive does
 the same for the progressive JPEGs the GPU decoder takes (preprocess.progressive_gpu_decodable,
 DetectionPipeline.enable_progressive_jpeg_decode).
+
+IMAGE_DIR may also be a video file, recognised by its content (RIFF AVI, MP4 / MOV, Matroska / WebM; video files inside a
+directory are not picked up).  Its frames go through the same loop, one JSON line per frame in frame order,
+{"video": PATH, "frame": i, "time": seconds, "detections": [...]}, and every flag works per frame.  Motion-JPEG frames in an AVI
+are read by index (k210_yolo_framework_b200.video) and routed as JPEG files are; every other video is decoded in order by
+OpenCV's FFmpeg backend on the decode threads of every rank, each rank keeping its own frames.  --draw DIR then writes
+DIR/<stem>.avi, a Motion-JPEG AVI of the drawn frames at the source frame rate, on rank 0.
 """
 import argparse
 import io
@@ -50,6 +57,7 @@ from k210_yolo_framework_b200.dist import shard_range  # noqa: E402
 from k210_yolo_framework_b200.helper import read_image  # noqa: E402
 from k210_yolo_framework_b200.preprocess import gpu_decodable, png_gpu_decodable, progressive_gpu_decodable  # noqa: E402
 from k210_yolo_framework_b200.pipeline import DetectionPipeline  # noqa: E402
+from k210_yolo_framework_b200.video import AviWriter, jpeg_hw, open_video, sniff_video  # noqa: E402
 
 EXTS = (".jpg", ".jpeg", ".png", ".bmp")
 
@@ -61,14 +69,27 @@ def list_images(path):
         return [l.strip() for l in fh if l.strip()]
 
 
-def load_image(path, gpu_png=False, gpu_progressive=False):
-    """The file's bytes when the GPU decodes it (PNGs only with `gpu_png`, progressive JPEGs only with `gpu_progressive`),
-    else its pixels decoded on the host (Helper._read_img)."""
+def is_video(path):
+    """True when `path` is a file whose content is a video container (RIFF AVI, ISO-BMFF or Matroska / WebM); directories and
+    text lists of images are not."""
+    if not os.path.isfile(path):
+        return False
     with open(path, "rb") as fh:
-        data = fh.read()
+        return sniff_video(fh.read(12))
+
+
+def route_image(data, gpu_png=False, gpu_progressive=False):
+    """A file's bytes when the GPU decodes it (PNGs only with `gpu_png`, progressive JPEGs only with `gpu_progressive`), else
+    its pixels decoded on the host (Helper._read_img)."""
     if gpu_decodable(data) or (gpu_png and png_gpu_decodable(data)) or (gpu_progressive and progressive_gpu_decodable(data)):
         return data
     return read_image(io.BytesIO(data))
+
+
+def load_image(path, gpu_png=False, gpu_progressive=False):
+    """``route_image`` of the file at `path`."""
+    with open(path, "rb") as fh:
+        return route_image(fh.read(), gpu_png, gpu_progressive)
 
 
 def open_pipeline(args, max_per_class=30):
@@ -150,8 +171,16 @@ def detect_files(pipe, files, decode_threads=4, load=None, rendered=False):
             yield result(*pending.popleft())
 
 
+def detections(recs):
+    """The "detections" field of a JSON line: one image's (or frame's) records."""
+    return [{"class": int(c), "score": round(float(s), 6), "box_tlbr": [float(t), float(l), float(b), float(r)], "index": int(i)}
+            for c, i, s, t, l, b, r in recs]
+
+
 def serve(args, out_fh=None):
     import torch.distributed as dist
+    if is_video(args.images):
+        return serve_video(args, out_fh)
     files = list_images(args.images)
     draw_dir = getattr(args, "draw", None)
     targets = draw_paths(files, draw_dir) if draw_dir else None     # refuses duplicate stems before any work
@@ -174,11 +203,57 @@ def serve(args, out_fh=None):
             continue
         recs = DetectionPipeline.records(dets, counts)
         for j, path in enumerate(chunk):
-            line = {"image": path, "detections": [{"class": int(c), "score": round(float(s), 6), "box_tlbr": [float(t), float(l), float(b), float(r)],
-                                                   "index": int(i)} for c, i, s, t, l, b, r in recs[j]]}
+            line = {"image": path, "detections": detections(recs[j])}
             if out_fh is not None:
                 out_fh.write(json.dumps(line) + "\n")
             n_out += 1
+    if world > 1:
+        dist.barrier()
+    return n_out
+
+
+def serve_video(args, out_fh=None):
+    """``serve`` for a video file: one JSON line per frame, {"video", "frame" (its position in the stream), "time" (seconds),
+    "detections"}, in frame order.  Frames are batched and sharded over the ranks as files are (``detect_files``); Motion-JPEG
+    AVI frames are read by index and routed as image files are, other videos are decoded in order by OpenCV's FFmpeg backend on
+    every rank, each keeping its own frames.  With --draw DIR rank 0 writes DIR/<stem>.avi at the source frame rate from the
+    GPU-drawn JPEG frames, which the other ranks send it once per global batch."""
+    import torch.distributed as dist
+    src = open_video(args.images)
+    draw_dir = getattr(args, "draw", None)
+    pipe, world, rank = open_pipeline(args)
+    if draw_dir:
+        os.makedirs(draw_dir, exist_ok=True)
+        pipe.enable_rendering(quality=args.draw_quality)
+    B, G = pipe.images_per_batch, pipe.world * pipe.images_per_batch
+    gpu_png, gpu_progressive = getattr(args, "gpu_png", False), getattr(args, "gpu_progressive", False)
+    load = src.loader(keep=lambda k: (k % G) // B == rank, route=lambda data: route_image(data, gpu_png, gpu_progressive))
+    target = os.path.join(draw_dir, os.path.splitext(os.path.basename(args.images))[0] + ".avi") if draw_dir else None
+    writer, n_out = None, 0
+    try:
+        for item in detect_files(pipe, list(range(src.n_frames)), getattr(args, "decode_threads", 4), load, rendered=bool(draw_dir)):
+            chunk, dets, counts = item[:3]
+            if draw_dir:
+                drawn = item[3]
+                if world > 1:       # the frames vary in size: the records' fixed-size all-gather cannot carry them
+                    parts = [None] * world if rank == 0 else None
+                    dist.gather_object(drawn, parts, dst=0)
+                    drawn = [d for part in parts for d in part] if rank == 0 else []
+                for data in drawn:
+                    if writer is None:
+                        writer = AviWriter(target, src.fps, jpeg_hw(data))
+                    writer.write(data)
+            if rank != 0:
+                continue
+            recs = DetectionPipeline.records(dets, counts)
+            for j, k in enumerate(chunk):
+                line = {"video": args.images, "frame": src.position(k), "time": src.time(k), "detections": detections(recs[j])}
+                if out_fh is not None:
+                    out_fh.write(json.dumps(line) + "\n")
+                n_out += 1
+    finally:
+        if writer is not None:
+            writer.close()
     if world > 1:
         dist.barrier()
     return n_out
@@ -243,13 +318,14 @@ def quality_arg(v):
 def build_parser():
     ap = ModelArgParser()
     add_model_args(ap)
-    ap.add_argument("images", help="directory of images, or a text file with one path per line")
+    ap.add_argument("images", help="directory of images, a text file with one path per line, or a video file (recognised by its "
+                                    "content: AVI, MP4 / MOV or Matroska / WebM)")
     ap.add_argument("--obj_thresh", type=float, default=0.7)
     ap.add_argument("--iou_thresh", type=float, default=0.5)
     ap.add_argument("--out", default="-")
     ap.add_argument("--draw", default=None, metavar="DIR",
                     help="also write every image with its detections drawn (as keras_inference.py draws them) to DIR/<stem>.jpg, "
-                         "rendered and JPEG-encoded on the GPU")
+                         "rendered and JPEG-encoded on the GPU; for a video, its drawn frames as the Motion-JPEG AVI DIR/<stem>.avi")
     ap.add_argument("--draw_quality", type=quality_arg, default=75, help="JPEG quality of the --draw files (1..100)")
     return ap
 
@@ -261,7 +337,7 @@ def main():
     n = serve(args, fh)
     if rank == 0 and fh is not sys.stdout:
         fh.close()
-        print(f"{n} images -> {args.out}", file=sys.stderr)
+        print(f"{n} {'frames' if is_video(args.images) else 'images'} -> {args.out}", file=sys.stderr)
 
 
 if __name__ == "__main__":
