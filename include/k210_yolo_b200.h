@@ -231,6 +231,27 @@ int k2y_merge_views_mirror(const k2y_det *view_dets_dev, const int32_t *view_cou
                            int n_boxes, int class_num, int max_per_class, float thresh, k2y_det *dets_dev, int32_t *counts_dev,
                            long long det_image_stride_words, long long count_image_stride_words, void *stream);
 
+/* SORT tracking (oracle/sort_ref.py states every rule, and this call follows it bit for bit): per class, a Kalman filter per
+ * track, IoU association by scipy's optimal assignment, SORT's birth, reporting and death, ids from one counter per stream.
+ *   state_dev       k2y_track_state_bytes() bytes on the device, zeroed to start a stream; the tracks, the frame count, the
+ *                   last position and the ids taken carry over from one call to the next, so calls of one stream must be
+ *                   ordered (one stream, or events).
+ *   dets_dev, counts_dev  a gathered record block: row r's records of class c at dets_dev + r * row_stride_words words
+ *                   (k2y_det, max_per_class per class), its counts at counts_dev + r * row_stride_words + c.
+ *   rows_dev        int32 [n_frames]: the block row of each frame, frames in stream order.
+ *   positions_dev   int64 [n_frames]: each frame's position in the stream, increasing (the caller checks it).  A jump of g > 1
+ *                   runs g - 1 updates without detections first.
+ *   ids_out_dev     int32 [n_frames, class_num, max_per_class]: each record's track id, -1 when it has none reported.
+ *   boxes_out_dev   float32 [n_frames, class_num, max_per_class, 4]: for a record with an id, its track's post-update state
+ *                   box (ymin, xmin, ymax, xmax); zeros elsewhere.
+ * One launch of one CTA per call, whatever n_frames, asynchronous on `stream`.  K2Y_ERR_INVALID (nothing launched) for
+ * class_num outside 1..1024, max_age < 0, min_hits < 0, iou_thresh outside [0, 1], or max_per_class * (max_age + 1) over the
+ * 1024 tracks one class holds. */
+int k2y_track_state_bytes(int class_num, int max_per_class, int max_age, size_t *bytes);
+int k2y_track_update(void *state_dev, const k2y_det *dets_dev, const int32_t *counts_dev, long long row_stride_words,
+                     const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num, int max_per_class,
+                     int max_age, int min_hits, double iou_thresh, int32_t *ids_out_dev, float *boxes_out_dev, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Multi-GPU collation: images shard across ranks (one process per GPU), and the one exchange on the path
  * is ONE ncclAllGather of the fixed-size record blocks.  The reference is single-process (keras_inference.py:12-17), so

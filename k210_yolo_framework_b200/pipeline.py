@@ -37,6 +37,11 @@ smaller box, fold the matched boxes into the kept one and drop records at the ti
 with): the letterbox fetches the mirrored columns, and ``k2y_merge_views_mirror`` maps the mirrored views' records back into
 the image while it loads them, then merges all views as above.  It combines with either grid, in either order.
 
+``enable_tracking`` tracks objects across the frames of a stream, SORT-style (``track.Tracker``, oracle/sort_ref.py):
+``submit_images(frames=...)`` gives each image's position in the stream, one ``k2y_track_update`` launch per batch runs behind the
+NMS / all-gather on the stream that holds the gathered block, before its D2H, and ``tracks(ticket)`` returns each record's track
+id and box.  The records are unchanged.
+
 ``enable_png_decode`` makes ``submit_images`` decode the PNG files the GPU takes there too (``preprocess.png_gpu_decodable``),
 in the same staging range and H2D copy as the batch's JPEGs; their status words travel beside the JPEGs'.
 ``enable_progressive_jpeg_decode`` does the same for progressive JPEGs (``preprocess.progressive_gpu_decodable``).
@@ -137,6 +142,10 @@ class DetectionPipeline:
         self._view_dets: Optional[torch.Tensor] = None
         self._view_counts: Optional[torch.Tensor] = None
         self._slot_yx: Optional[List[torch.Tensor]] = None
+        # enable_tracking: the tracker, its pinned per-slot inputs and outputs and their device copies; per gather slot the
+        # frames its batch tracked (None: not tracked)
+        self._track = None
+        self._track_n: List[Optional[int]] = [None] * SLOTS
 
     @property
     def images_per_batch(self) -> int:
@@ -230,6 +239,63 @@ class DetectionPipeline:
             self._view_dets = torch.zeros((self.batch, self.gather.C, self.gather.K, DET_WORDS), dtype=torch.int32, device=dev)
             self._view_counts = torch.zeros((self.batch, self.gather.C), dtype=torch.int32, device=dev)
             self._slot_yx = [torch.zeros((self.batch, 2), dtype=torch.float32, device=dev) for _ in range(SLOTS)]
+
+    def enable_tracking(self, max_age: int = 1, min_hits: int = 3, iou_thresh: float = 0.3) -> None:
+        """From now on ``submit_images`` takes `frames`, each image's position in a stream of frames, and tracks the objects of
+        the stream as SORT does (oracle/sort_ref.py states every rule): per class, a Kalman filter per track, IoU association
+        by optimal assignment, a track born for each unmatched detection and removed once it missed more than `max_age`
+        frames, and reported once it was matched in `min_hits` frames in a row (or in the stream's first `min_hits` frames).
+        ``tracks(ticket)`` returns each record's id and track box.  A new call starts a new stream, as ``reset_tracks`` does.
+        Raises ``ValueError``, leaving the pipeline as it was, for a bad setting or when max_per_class * (max_age + 1)
+        exceeds the 1024 tracks one class holds (max_age <= 33 at max_per_class 30, <= 9 at 100)."""
+        from .track import Tracker
+        tracker = Tracker(self.gather.C, self.gather.K, max_age, min_hits, iou_thresh, self.device_index)
+        dev = torch.device("cuda", self.device_index)
+        n, C, K = self.world * self.batch, self.gather.C, self.gather.K
+        self._track = dict(
+            tracker=tracker, rows=torch.empty(n, dtype=torch.int32, device=dev), pos=torch.empty(n, dtype=torch.int64, device=dev),
+            ids=torch.empty((n, C, K), dtype=torch.int32, device=dev), boxes=torch.empty((n, C, K, 4), dtype=torch.float32, device=dev),
+            rows_host=[torch.empty(n, dtype=torch.int32).pin_memory() for _ in range(SLOTS)],
+            pos_host=[torch.empty(n, dtype=torch.int64).pin_memory() for _ in range(SLOTS)],
+            ids_host=[torch.empty((n, C, K), dtype=torch.int32).pin_memory() for _ in range(SLOTS)],
+            boxes_host=[torch.empty((n, C, K, 4), dtype=torch.float32).pin_memory() for _ in range(SLOTS)])
+        self._track_n = [None] * SLOTS
+
+    def reset_tracks(self) -> None:
+        """Starts a new stream: no tracks, frame count 0, ids from 1, any first position.  Ordered after the batches already
+        submitted."""
+        if self._track is None:
+            raise RuntimeError("reset_tracks() needs enable_tracking()")
+        self._track["tracker"].reset(self._side if self.world > 1 else self._det_stream)
+
+    def tracks(self, ticket: int):
+        """(ids int32 [F, C, K], boxes float32 [F, C, K, 4]) of the F frames of the ``submit_images`` batch behind `ticket`, in
+        the order of its `frames`: each record's track id (-1: no track, or one not reported in this frame) and, where it
+        has an id, its track's state box (ymin, xmin, ymax, xmax) after the frame; pinned host views, valid after
+        ``collect(ticket)`` until the ticket's slot is reused.  Frame q is global image q: with several ranks, rank q //
+        images_per_batch's image q % images_per_batch."""
+        if self._track is None or self._track_n[ticket] is None:
+            raise RuntimeError("no tracks for this ticket: call enable_tracking() and give submit_images() its frames")
+        self._d2h_done[ticket].synchronize()
+        m = self._track_n[ticket]
+        return self._track["ids_host"][ticket][:m], self._track["boxes_host"][ticket][:m]
+
+    def _track_slot(self, s: int, st: torch.cuda.Stream, frames: list) -> None:
+        """Enqueues the tracking of gather slot s's frames on `st`, behind its gathered block: rows and positions H2D, one
+        k2y_track_update, ids and boxes D2H."""
+        tk, m, B = self._track, len(frames), self._ipb
+        self._track_n[s] = m
+        if m == 0:
+            return
+        self._d2h_done[s].synchronize()       # the slot's last copies out of its pinned inputs have finished
+        tk["rows_host"][s].numpy()[:m] = [(q // B) * self.batch + q % B for q in range(m)]
+        tk["pos_host"][s].numpy()[:m] = frames
+        tk["rows"][:m].copy_(tk["rows_host"][s][:m], non_blocking=True)
+        tk["pos"][:m].copy_(tk["pos_host"][s][:m], non_blocking=True)
+        dets, counts = self.gather.views(s)
+        tk["tracker"].update(dets, counts, tk["rows"], tk["pos"], m, tk["ids"], tk["boxes"], st, frames[-1])
+        tk["ids_host"][s][:m].copy_(tk["ids"][:m], non_blocking=True)
+        tk["boxes_host"][s][:m].copy_(tk["boxes"][:m], non_blocking=True)
 
     def enable_png_decode(self) -> None:
         """From now on ``submit_images`` decodes the PNG files the GPU takes (``preprocess.png_gpu_decodable``: non-interlaced,
@@ -350,6 +416,7 @@ class DetectionPipeline:
         self._prog_idx[self._steps % SLOTS] = []
         t = self._run_slot(slot, buf, n, None, None)
         self._rendered_slot[t] = False
+        self._track_n[t] = None
         return t
 
     def enable_rendering(self, quality: int = 75, font_path: str = "asset/FiraMono-Medium.otf", colormap=None) -> None:
@@ -395,7 +462,7 @@ class DetectionPipeline:
         self._render_done[s].record(det)
         self._render_free[slot].record(det)
 
-    def submit_images(self, images: Sequence[np.ndarray]) -> int:
+    def submit_images(self, images: Sequence[np.ndarray], frames: Optional[Sequence[int]] = None) -> int:
         """Streaming form for raw images: `images` is a list of n <= ``images_per_batch`` host numpy uint8 [h, w, 3] RGB arrays of any sizes, or
         image files (``bytes``, ``bytearray``, ``memoryview``): baseline JPEGs are decoded on the GPU on the copy stream in front
         of the letterbox, other files on the host inside this call (``preprocess.BatchLayout``).
@@ -405,7 +472,11 @@ class DetectionPipeline:
         images.  Returns a ticket for ``collect``, which returns the n images' records (world > 1: the gathered blocks of every
         rank, rank r's images from row r * batch), or raises ``K2YError`` naming the JPEGs whose entropy-coded data was corrupt
         (their records would come from undefined pixels).  Same flow control as ``submit``.  Bad input raises ``ValueError``
-        before anything is enqueued."""
+        before anything is enqueued.
+
+        With ``enable_tracking`` `frames` is required: the stream positions of the global batch's frames in gathered-row order
+        (global image q is rank q // images_per_batch's image q % images_per_batch; images past len(frames) are not frames),
+        increasing along the stream.  Every rank gives the same list."""
         viewed = self._tiling is not None or self._flip
         if viewed and isinstance(images, (list, tuple)) and len(images) > self.images_per_batch:
             raise ValueError(f"{len(images)} images of {self._views} views do not fit a batch of {self.batch}")
@@ -414,6 +485,12 @@ class DetectionPipeline:
         n = len(layout)
         if n > self.batch:
             raise ValueError(f"{n} images do not fit a batch of {self.batch}")
+        if (frames is None) != (self._track is None):
+            raise ValueError("submit_images takes frames= exactly when tracking is on (enable_tracking)")
+        if frames is not None:
+            frames = self._track["tracker"].check_positions(frames)
+            if len(frames) > self.world * self._ipb or (self.world == 1 and len(frames) > n):
+                raise ValueError(f"{len(frames)} frame positions for {n} images per rank of {self.world} ranks")
         if self._render is not None:
             from .render import JPEG_MAX_DIMENSION
             for i, (h, w) in enumerate(layout.hw.tolist()):
@@ -454,7 +531,7 @@ class DetectionPipeline:
             at = self._staging[slot].dev.data_ptr() + layout.merge_table_at
             table = (at, at + 4 * (n + 1), at + 4 * (n + 1 + nv) if self._flip else None, n)
         t = self._run_slot(slot, buf, nv, self._slot_hw[slot][:nv], n if self.world == 1 else None,
-                           self._slot_yx[slot][:nv] if viewed else None, table)
+                           self._slot_yx[slot][:nv] if viewed else None, table, frames)
         self._rendered_slot[t] = self._render is not None
         if self._render is not None:
             with torch.cuda.device(dev):
@@ -462,8 +539,9 @@ class DetectionPipeline:
         return t
 
     def _run_slot(self, slot: int, buf: torch.Tensor, n: int, image_hw: Optional[torch.Tensor], rows: Optional[int],
-                  view_yx: Optional[torch.Tensor] = None, table=None) -> int:
-        """Network + decode (+ all-gather) of input slot `slot` once its H2D is done, then the D2H of the records."""
+                  view_yx: Optional[torch.Tensor] = None, table=None, frames: Optional[list] = None) -> int:
+        """Network + decode (+ all-gather) of input slot `slot` once its H2D is done, then (with `frames`) the tracking, then
+        the D2H of the records."""
         compute = torch.cuda.current_stream(self.device_index)
         compute.wait_event(self._h2d_done[slot])
         self.engine.bind_input(buf)
@@ -474,6 +552,8 @@ class DetectionPipeline:
         # D2H of the gathered blocks: behind the all-gather on the side stream (world > 1), else behind the decode
         st = self._side if self.world > 1 else self._det_stream
         with torch.cuda.stream(st):
+            if frames is not None:
+                self._track_slot(s, st, frames)
             self._host[s].copy_(self.gather.bufs[s], non_blocking=True)
             self._d2h_done[s].record(st)
             self._slot_free[s].record(st)
@@ -628,6 +708,10 @@ class LanedPipeline:
         for ln in self.lanes:
             ln.enable_tiling(rows, cols, overlap, tile_size=tile_size, images_per_batch=images_per_batch, match=match, merge=merge,
                              match_thresh=match_thresh, border=border)
+
+    def enable_tracking(self, max_age: int = 1, min_hits: int = 3, iou_thresh: float = 0.3) -> None:
+        """Not available: the lanes would have to hand one stream's frames over in order."""
+        raise NotImplementedError("tracking runs on a DetectionPipeline; a LanedPipeline's lanes cannot order one stream's frames")
 
     def enable_flip(self, *, match: Optional[str] = None, merge: Optional[str] = None, match_thresh: Optional[float] = None,
                     border: Optional[float] = None) -> None:

@@ -1,0 +1,67 @@
+"""SORT tracking on the GPU (``k2y_track_update``, csrc/track.cu; oracle/sort_ref.py states the rules): ``Tracker`` owns one
+stream's device state and runs one launch per batch of frames over a gathered record block."""
+from __future__ import annotations
+
+import ctypes
+from typing import Optional, Sequence
+
+import torch
+
+from ._lib import check, lib
+
+MAX_TRACKS_PER_CLASS = 1024
+
+
+def check_setting(K: int, max_age, min_hits, iou_thresh) -> None:
+    """Raises ValueError for a setting the tracker does not take (oracle/sort_ref.py ``check_setting``)."""
+    if isinstance(max_age, bool) or int(max_age) != max_age or max_age < 0:
+        raise ValueError(f"max_age {max_age}: a whole number of frames >= 0")
+    if isinstance(min_hits, bool) or int(min_hits) != min_hits or min_hits < 0:
+        raise ValueError(f"min_hits {min_hits}: a whole number >= 0")
+    if not 0.0 <= float(iou_thresh) <= 1.0:
+        raise ValueError(f"iou_thresh {iou_thresh} is outside [0, 1]")
+    if K * (int(max_age) + 1) > MAX_TRACKS_PER_CLASS:
+        raise ValueError(f"max_per_class {K} x (max_age {max_age} + 1) tracks per class exceed the {MAX_TRACKS_PER_CLASS} the "
+                         f"tracker holds: max_age <= {MAX_TRACKS_PER_CLASS // K - 1} at max_per_class {K}")
+
+
+class Tracker:
+    """One stream's tracks over `C` classes of at most `K` records per frame.  ``update`` enqueues one launch for a batch of
+    frames; ``reset`` starts a new stream.  Both are asynchronous on the stream given and must be ordered among themselves."""
+
+    def __init__(self, C: int, K: int, max_age: int = 1, min_hits: int = 3, iou_thresh: float = 0.3, device=None):
+        check_setting(K, max_age, min_hits, iou_thresh)
+        self.C, self.K = int(C), int(K)
+        self.max_age, self.min_hits, self.iou_thresh = int(max_age), int(min_hits), float(iou_thresh)
+        nbytes = ctypes.c_size_t()
+        check(lib.k2y_track_state_bytes(self.C, self.K, self.max_age, ctypes.byref(nbytes)))
+        dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        self.state = torch.zeros(nbytes.value, dtype=torch.uint8, device=dev)
+        self.last_position: Optional[int] = None      # host copy, to refuse positions that do not increase
+
+    def reset(self, stream: Optional[torch.cuda.Stream] = None) -> None:
+        with torch.cuda.stream(stream or torch.cuda.current_stream(self.state.device)):
+            self.state.zero_()
+        self.last_position = None
+
+    def check_positions(self, positions: Sequence[int]) -> list:
+        """The positions as ints; raises ValueError unless they increase, from the stream's last one on."""
+        pos = [int(p) for p in positions]
+        prev = self.last_position
+        for p in pos:
+            if p < 0 or (prev is not None and p <= prev):
+                raise ValueError(f"frame position {p} does not follow {prev}: positions increase along a stream, from 0")
+            prev = p
+        return pos
+
+    def update(self, dets: torch.Tensor, counts: torch.Tensor, rows: torch.Tensor, positions: torch.Tensor, n_frames: int,
+               ids_out: torch.Tensor, boxes_out: torch.Tensor, stream: torch.cuda.Stream, last_position: int) -> None:
+        """Frames rows[:n_frames] of the block (dets [N, C, K, 6] int32 and counts [N, C] of one buffer, same row stride), at
+        positions[:n_frames] (device int64, checked with ``check_positions``); writes ids_out [>= n_frames, C, K] int32 and
+        boxes_out [>= n_frames, C, K, 4] float32."""
+        if dets.stride(0) != counts.stride(0):
+            raise ValueError("dets and counts must share their row stride (a gather block)")
+        check(lib.k2y_track_update(self.state.data_ptr(), dets.data_ptr(), counts.data_ptr(), dets.stride(0), rows.data_ptr(),
+                                   positions.data_ptr(), int(n_frames), self.C, self.K, self.max_age, self.min_hits,
+                                   self.iou_thresh, ids_out.data_ptr(), boxes_out.data_ptr(), ctypes.c_void_p(stream.cuda_stream)))
+        self.last_position = int(last_position)

@@ -8,13 +8,26 @@ serve.py runs a video (detect_files, two batches in flight), for
   draw:         the GPU route with --draw: the drawn frames rendered and encoded on the GPU and written as a Motion-JPEG AVI;
   ffmpeg_mp4v:  the same frames as an mp4v video, decoded in order by OpenCV's FFmpeg backend on the host threads.
 
+With --track, also SORT tracking of the same records (DetectionPipeline.enable_tracking, default setting):
+  gpu_plain /    the GPU route on two fresh pipelines, one tracking on the GPU (one k2y_track_update launch per batch, behind
+  gpu_track:     the NMS) and one not, their windows alternating (which goes first alternates too);
+  track_kernel:  that kernel's time per batch of frames, from CUDA events around its launches, on the route's records and on
+                 two dense synthetic streams: "dense_voc" (20 classes, each with about 27 of its 30 records in every frame,
+                 moving objects) and "coco_bound" (80 classes of 100, max_age 9, one class with 100 new records in every frame,
+                 so that it holds its bound of 1000 tracks);
+  sort_ref /     the route's records and the dense_voc stream tracked on the host by oracle/sort_ref.py (scalar filter,
+  sort_matrix:   plain-Python assignment) and by a literal matrix-form SORT (numpy filter, iou_batch, scipy's
+                 linear_sum_assignment), frames/s of the tracker alone: scipy imported and one pass run before the timed
+                 windows (median).
+The GPU's ids and boxes must equal sort_ref's; the run fails otherwise.
+
 The video: the bench_ingest photos resized to 1280x720 with the golden dog photo pasted in (so that there are records to
 compare), written as a Motion-JPEG AVI at 4:2:2, quality 90, without DHT segments, as cameras write them.  Every route runs
 once to warm up and then `--windows` timed passes (median).  All Motion-JPEG routes must give the same records, and the mp4v
 route the records of its own decoded pixels; the run fails otherwise.  The card's name, power limit and SM clock are read in
 the same run.  Prints one JSON line.
 
-    python scripts/bench_video.py [--frames 256 --batch 32 --windows 3]
+    python scripts/bench_video.py [--frames 256 --batch 32 --windows 3 --track]
 """
 import argparse
 import io
@@ -64,11 +77,15 @@ def frames_720p(n):
     return out
 
 
-def run(pipe, n, load, threads, writer_path=None, fps=30.0):
-    """Records of frames 0 .. n-1 through detect_files; with `writer_path` the drawn frames go to a Motion-JPEG AVI."""
+def run(pipe, n, load, threads, writer_path=None, fps=30.0, tracks=None):
+    """Records of frames 0 .. n-1 through detect_files; with `writer_path` the drawn frames go to a Motion-JPEG AVI; with
+    `tracks` (a list; the pipeline's tracking enabled) the frames are tracked and each batch's (ids, boxes) copies go there."""
     recs, writer = [], None
-    for item in serve.detect_files(pipe, list(range(n)), threads, load, rendered=writer_path is not None):
+    positions = list(range(n)) if tracks is not None else None
+    for item in serve.detect_files(pipe, list(range(n)), threads, load, rendered=writer_path is not None, positions=positions):
         recs += DetectionPipeline.records(item[1], item[2])[:len(item[0])]
+        if tracks is not None:
+            tracks.append((item[-1][0].clone(), item[-1][1].clone()))
         if writer_path is not None:
             for data in item[3]:
                 writer = writer or AviWriter(writer_path, fps, jpeg_hw(data))
@@ -78,19 +95,25 @@ def run(pipe, n, load, threads, writer_path=None, fps=30.0):
     return recs
 
 
+def new_pipeline(anchors, batch):
+    pipe = DetectionPipeline("yolo_mobilev1", (224, 320), anchors, 20, 0.75, batch, obj_thresh=0.3, iou_thresh=0.5)
+    pipe.engine.set_weights(load_npz_weights(os.path.join(GOLDEN, "yolo_mobilev1_075_voc_weights.npz")))
+    return pipe
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=256)
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--windows", type=int, default=3)
+    ap.add_argument("--track", action="store_true", help="also measure SORT tracking on the GPU and on the host")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_video measures on a GPU"
     import cv2
     from PIL import Image
     torch.cuda.set_device(0)
     anchors = np.load(os.path.join(GOLDEN, "voc_anchor.npy"))
-    pipe = DetectionPipeline("yolo_mobilev1", (224, 320), anchors, 20, 0.75, args.batch, obj_thresh=0.3, iou_thresh=0.5)
-    pipe.engine.set_weights(load_npz_weights(os.path.join(GOLDEN, "yolo_mobilev1_075_voc_weights.npz")))
+    pipe = new_pipeline(anchors, args.batch)
     n = args.frames
     with tempfile.TemporaryDirectory() as tmp:
         avi, mp4 = os.path.join(tmp, "cam.avi"), os.path.join(tmp, "cam.mp4")
@@ -142,6 +165,8 @@ def main():
             times["draw"].append(time.perf_counter() - t0)
             recs["draw"] = recs["draw"] if out == recs["draw"] else None
         drawn_frames = open_video(drawn).n_frames
+        make_pipe = lambda: new_pipeline(anchors, args.batch)     # noqa: E731
+        track = bench_track(make_pipe, n, gpu_load, recs["gpu"], args.batch, args.windows) if args.track else None
         gpu = gpu_info()
     mjpeg = [recs[k] for k in ("gpu", "pil_1", "pil_4", "pil_16", "pixels", "draw")]
     same = all(r is not None and r == mjpeg[0] for r in mjpeg) and recs["ffmpeg_mp4v"] == mp4_ref and drawn_frames == n
@@ -150,9 +175,142 @@ def main():
         "metric": "video_frames_per_s", "cfg": f"yolo_mobilev1 alpha 0.75, 224x320, batch {args.batch}", "frames": n,
         "video": f"MJPEG AVI {W720}x{H720} 4:2:2 q90 without DHT", "avi_bytes": avi_bytes, "mp4v_bytes": mp4_bytes,
         "gpu_decoded_frames": int(gpu_frames), "records": int(sum(len(r) for r in mjpeg[0] or [])), "frames_per_s": rate,
-        "windows_s": {k: [round(t, 4) for t in v] for k, v in times.items()}, "records_equal": same, "gpu": gpu}))
+        "windows_s": {k: [round(t, 4) for t in v] for k, v in times.items()}, "records_equal": same,
+        **({"track": track} if track else {}), "gpu": gpu}))
     if not same:
         sys.exit("the routes' records differ")
+    if track and not track["ids_equal"]:
+        sys.exit("the GPU tracker's ids and boxes differ from oracle/sort_ref.py's")
+
+
+def frame_blocks(recs, C, K):
+    """Each frame's records as (boxes float32 [C, K, 4], counts [C]), in record order per class."""
+    out = []
+    for frame in recs:
+        boxes, counts = np.zeros((C, K, 4), np.float32), np.zeros(C, np.int32)
+        for c, _, _, t, l, b, r in frame:
+            boxes[c, counts[c]] = (t, l, b, r)
+            counts[c] += 1
+        out.append((boxes, counts))
+    return out
+
+
+def dense_voc_blocks(C, K, n, seed=0):
+    """Every class full: K objects of 40 x 40 px on a 60 px lattice (none overlaps another) moving 2 px per frame with noise,
+    each record left out of a frame with probability 0.1."""
+    rng = np.random.default_rng(seed)
+    out = []
+    for f in range(n):
+        boxes, counts = np.zeros((C, K, 4), np.float32), np.zeros(C, np.int32)
+        for c in range(C):
+            keep = [i for i in range(K) if rng.random() >= 0.1]
+            for k, i in enumerate(keep):
+                y, x = 60.0 * i + rng.normal(), 60.0 * c + 2.0 * f + rng.normal()
+                boxes[c, k] = (y, x, y + 40, x + 40)
+            counts[c] = len(keep)
+        out.append((boxes, counts))
+    return out
+
+
+def bound_blocks(C, K, n):
+    """Class 0 holds its track bound: K new 10 x 10 boxes in every frame that overlap nothing, so every record is born."""
+    out = []
+    for f in range(n):
+        boxes, counts = np.zeros((C, K, 4), np.float32), np.zeros(C, np.int32)
+        for i in range(K):
+            y, x = 20.0 * i, 100.0 + 20.0 * f
+            boxes[0, i] = (y, x, y + 10, x + 10)
+        counts[0] = K
+        out.append((boxes, counts))
+    return out
+
+
+def time_kernel(blocks, C, K, max_age, batch, windows, dev):
+    """(median, max) ms per launch of k2y_track_update over the frames in batches of `batch`, from CUDA events; the frames'
+    records staged on the device as gather blocks first, one untimed pass to warm up."""
+    from k210_yolo_framework_b200.dist import DetectionGather
+    from k210_yolo_framework_b200.track import Tracker
+    staged = []
+    for a in range(0, len(blocks), batch):
+        buf = torch.zeros((batch, C * (K * 6 + 1)), dtype=torch.int32)
+        d, c = DetectionGather.split(buf, C, K)
+        for i, (b, cnt) in enumerate(blocks[a:a + batch]):
+            d[i, :, :, :4] = torch.from_numpy(b.view(np.int32))
+            c[i] = torch.from_numpy(cnt)
+        m = len(blocks[a:a + batch])
+        staged.append((DetectionGather.split(buf.to(dev), C, K), m, torch.arange(a, a + m, dtype=torch.int64, device=dev), a + m - 1))
+    rows = torch.arange(batch, dtype=torch.int32, device=dev)
+    ids_d = torch.empty((batch, C, K), dtype=torch.int32, device=dev)
+    boxes_d = torch.empty((batch, C, K, 4), dtype=torch.float32, device=dev)
+    tracker = Tracker(C, K, max_age=max_age, device=dev.index)
+    st = torch.cuda.current_stream()
+    per_batch = []
+    for w in range(windows + 1):
+        tracker.reset()
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2 * len(staged))]
+        for i, ((d, c), m, pos, last) in enumerate(staged):
+            ev[2 * i].record(st)
+            tracker.update(d, c, rows, pos, m, ids_d, boxes_d, st, last)
+            ev[2 * i + 1].record(st)
+        torch.cuda.synchronize()
+        if w:
+            per_batch += [ev[2 * i].elapsed_time(ev[2 * i + 1]) for i in range(len(staged))]
+    return round(statistics.median(per_batch), 4), round(max(per_batch), 4)
+
+
+def bench_track(make_pipe, n, load, recs, batch, windows):
+    """The --track arms (see the module docstring)."""
+    import scipy.optimize  # noqa: F401  (imported before the host trackers' timing)
+    from oracle import sort_ref
+    plain, tracked = make_pipe(), make_pipe()
+    C, K = plain.gather.C, plain.gather.K
+    blocks = frame_blocks(recs, C, K)
+    tracked.enable_tracking()
+    got = []
+    assert run(plain, n, load, 4) == recs                           # warm-up of both
+    assert run(tracked, n, load, 4, tracks=got) == recs             # tracking leaves the records as they were
+    times = {"gpu_plain": [], "gpu_track": []}
+    for w in range(windows):
+        arms = ["gpu_plain", "gpu_track"] if w % 2 == 0 else ["gpu_track", "gpu_plain"]
+        for arm in arms:
+            if arm == "gpu_track":
+                tracked.reset_tracks()
+                got = []
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out = run(tracked, n, load, 4, tracks=got) if arm == "gpu_track" else run(plain, n, load, 4)
+            torch.cuda.synchronize()
+            times[arm].append(time.perf_counter() - t0)
+            assert out == recs
+    ids = torch.cat([g[0] for g in got]).numpy()
+    boxes = torch.cat([g[1] for g in got]).numpy()
+    dense = dense_voc_blocks(C, K, n)
+    host = {}
+    for stream, frames in (("route", blocks), ("dense_voc", dense)):
+        for name, cls in (("sort_ref", sort_ref.Sort), ("sort_matrix", sort_ref.MatrixSort)):
+            key = f"{name}_{stream}"
+            host[key] = []
+            for w in range(windows + 1):        # the first pass warms up
+                tracker = cls(C, K)
+                t0 = time.perf_counter()
+                out = [tracker.update(p, b, c) for p, (b, c) in enumerate(frames)]
+                if w:
+                    host[key].append(time.perf_counter() - t0)
+            if key == "sort_ref_route":
+                ref_ids, ref_boxes = np.stack([o[0] for o in out]), np.stack([o[1] for o in out])
+    nan = np.isnan(ref_boxes)
+    equal = bool(np.array_equal(ids, ref_ids) and np.array_equal(np.isnan(boxes), nan) and
+                 np.array_equal(np.where(nan, 0, boxes), np.where(nan, 0, ref_boxes)))
+    dev = torch.device("cuda", plain.device_index)
+    kernel = {"route": time_kernel(blocks, C, K, 1, batch, windows, dev),
+              "dense_voc": time_kernel(dense, C, K, 1, batch, windows, dev),
+              "coco_bound": time_kernel(bound_blocks(80, 100, n), 80, 100, 9, batch, windows, dev)}
+    return {"frames_per_s": {k: round(n / statistics.median(v), 1) for k, v in times.items()},
+            "windows_s": {k: [round(t, 4) for t in v] for k, v in times.items()},
+            "track_kernel_ms_per_batch_median_max": kernel,
+            "host_frames_per_s": {k: round(n / statistics.median(v), 1) for k, v in host.items()},
+            "host_windows_s": {k: [round(t, 4) for t in v] for k, v in host.items()},
+            "reported_records": int((ids >= 0).sum()), "tracks": int(ids.max(initial=0)), "ids_equal": equal}
 
 
 if __name__ == "__main__":

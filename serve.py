@@ -39,6 +39,10 @@ directory are not picked up).  Its frames go through the same loop, one JSON lin
 are read by index (k210_yolo_framework_b200.video) and routed as JPEG files are; every other video is decoded in order by
 OpenCV's FFmpeg backend on the decode threads of every rank, each rank keeping its own frames.  --draw DIR then writes
 DIR/<stem>.avi, a Motion-JPEG AVI of the drawn frames at the source frame rate, on rank 0.
+
+With --track (a video only) the objects are tracked across the frames on the GPU, SORT-style (DetectionPipeline.enable_tracking,
+--track_max_age, --track_min_hits, --track_iou): every detection of a line gains "track", its track id or null, and
+"track_box_tlbr", the track's box, when it has an id.  Dropped frames count as frames without detections.
 """
 import argparse
 import io
@@ -133,7 +137,7 @@ def draw_paths(files, out_dir):
     return [os.path.join(out_dir, os.path.splitext(os.path.basename(p))[0] + ".jpg") for p in files]
 
 
-def detect_files(pipe, files, decode_threads=4, load=None, rendered=False):
+def detect_files(pipe, files, decode_threads=4, load=None, rendered=False, positions=None):
     """Yields ``(paths, dets, counts)`` per global batch of world * images_per_batch files, in file order: the batch's gathered
     record blocks as ``collect`` returns them (pinned host views, valid until the generator resumes twice; with tiling on
     several ranks, copies of the rows that hold images, so that row j is file j here too).  Every rank reads ITS
@@ -142,7 +146,9 @@ def detect_files(pipe, files, decode_threads=4, load=None, rendered=False):
     final batch match a full one's bit for bit) and takes part in every all-gather: its share of a short batch is padded
     with a grey network-size image, whose records nobody reads.  `load` maps a path to what submit_images takes
     (default: load_image).  With `rendered` (the pipeline's rendering enabled) each tuple also carries this rank's drawn
-    JPEG files of the batch, its padding images' files left out."""
+    JPEG files of the batch, its padding images' files left out.  With `positions` (the pipeline's tracking enabled; each
+    file's position in the stream) the batch's positions go to submit_images and each tuple ends with ``pipe.tracks``: the
+    (ids, boxes) of the batch's files, row j being file j."""
     load = load or load_image
     B, G, rank = pipe.images_per_batch, pipe.world * pipe.images_per_batch, pipe.rank
     rows = None
@@ -157,24 +163,36 @@ def detect_files(pipe, files, decode_threads=4, load=None, rendered=False):
         def result(chunk, ticket, mine):
             dets, counts = pipe.collect(ticket)
             out = (chunk, dets, counts) if rows is None else (chunk, dets[rows], counts[rows])
-            return out + (pipe.rendered(ticket)[:mine],) if rendered else out
+            out = out + (pipe.rendered(ticket)[:mine],) if rendered else out
+            return out + (pipe.tracks(ticket),) if positions is not None else out
 
         pending = deque()
         nxt = decode(chunks[0]) if chunks else []
         for g, chunk in enumerate(chunks):
             imgs = [f.result() for f in nxt]
             nxt = decode(chunks[g + 1]) if g + 1 < len(chunks) else []
-            pending.append((chunk, pipe.submit_images(imgs + [filler] * (B - len(imgs))), len(imgs)))
+            kw = {} if positions is None else {"frames": [positions[g * G + q] for q in range(len(chunk))]}
+            pending.append((chunk, pipe.submit_images(imgs + [filler] * (B - len(imgs)), **kw), len(imgs)))
             if len(pending) == 2:
                 yield result(*pending.popleft())
         while pending:
             yield result(*pending.popleft())
 
 
-def detections(recs):
-    """The "detections" field of a JSON line: one image's (or frame's) records."""
-    return [{"class": int(c), "score": round(float(s), 6), "box_tlbr": [float(t), float(l), float(b), float(r)], "index": int(i)}
-            for c, i, s, t, l, b, r in recs]
+def detections(recs, track=None):
+    """The "detections" field of a JSON line: one image's (or frame's) records.  With `track` = (ids, boxes, counts) of the
+    frame (``DetectionPipeline.tracks`` and the record counts) each detection also gets "track" (null without one) and, with
+    an id, "track_box_tlbr"."""
+    out = [{"class": int(c), "score": round(float(s), 6), "box_tlbr": [float(t), float(l), float(b), float(r)], "index": int(i)}
+           for c, i, s, t, l, b, r in recs]
+    if track is not None:
+        ids, boxes, counts = (np.asarray(a) for a in track)
+        mine = np.arange(ids.shape[1])[None, :] < counts[:, None]      # the records, class-major as `recs` lists them
+        for d, tid, box in zip(out, ids[mine].tolist(), boxes[mine].tolist()):
+            d["track"] = tid if tid >= 0 else None
+            if tid >= 0:
+                d["track_box_tlbr"] = box
+    return out
 
 
 def serve(args, out_fh=None):
@@ -225,13 +243,18 @@ def serve_video(args, out_fh=None):
     if draw_dir:
         os.makedirs(draw_dir, exist_ok=True)
         pipe.enable_rendering(quality=args.draw_quality)
+    track = getattr(args, "track", False)
+    if track:
+        pipe.enable_tracking(args.track_max_age, args.track_min_hits, args.track_iou)
     B, G = pipe.images_per_batch, pipe.world * pipe.images_per_batch
     gpu_png, gpu_progressive = getattr(args, "gpu_png", False), getattr(args, "gpu_progressive", False)
     load = src.loader(keep=lambda k: (k % G) // B == rank, route=lambda data: route_image(data, gpu_png, gpu_progressive))
     target = os.path.join(draw_dir, os.path.splitext(os.path.basename(args.images))[0] + ".avi") if draw_dir else None
     writer, n_out = None, 0
     try:
-        for item in detect_files(pipe, list(range(src.n_frames)), getattr(args, "decode_threads", 4), load, rendered=bool(draw_dir)):
+        positions = [src.position(k) for k in range(src.n_frames)] if track else None
+        for item in detect_files(pipe, list(range(src.n_frames)), getattr(args, "decode_threads", 4), load, rendered=bool(draw_dir),
+                                 positions=positions):
             chunk, dets, counts = item[:3]
             if draw_dir:
                 drawn = item[3]
@@ -247,7 +270,8 @@ def serve_video(args, out_fh=None):
                 continue
             recs = DetectionPipeline.records(dets, counts)
             for j, k in enumerate(chunk):
-                line = {"video": args.images, "frame": src.position(k), "time": src.time(k), "detections": detections(recs[j])}
+                tr = (item[-1][0][j], item[-1][1][j], counts[j]) if track else None
+                line = {"video": args.images, "frame": src.position(k), "time": src.time(k), "detections": detections(recs[j], tr)}
                 if out_fh is not None:
                     out_fh.write(json.dumps(line) + "\n")
                 n_out += 1
@@ -315,8 +339,18 @@ def quality_arg(v):
     return q
 
 
+class ServeArgParser(ModelArgParser):
+    """serve.py's parser: also refuses --track for anything but a video file."""
+
+    def parse_known_args(self, args=None, namespace=None):
+        ns, rest = super().parse_known_args(args, namespace)
+        if getattr(ns, "track", False) and not is_video(ns.images):
+            self.error(f"--track tracks the frames of a video; {ns.images} is not a video file")
+        return ns, rest
+
+
 def build_parser():
-    ap = ModelArgParser()
+    ap = ServeArgParser()
     add_model_args(ap)
     ap.add_argument("images", help="directory of images, a text file with one path per line, or a video file (recognised by its "
                                     "content: AVI, MP4 / MOV or Matroska / WebM)")
@@ -327,6 +361,11 @@ def build_parser():
                     help="also write every image with its detections drawn (as keras_inference.py draws them) to DIR/<stem>.jpg, "
                          "rendered and JPEG-encoded on the GPU; for a video, its drawn frames as the Motion-JPEG AVI DIR/<stem>.avi")
     ap.add_argument("--draw_quality", type=quality_arg, default=75, help="JPEG quality of the --draw files (1..100)")
+    ap.add_argument("--track", action="store_true",
+                    help="track objects across a video's frames on the GPU (SORT): each detection gains its track id and box")
+    ap.add_argument("--track_max_age", type=int, default=1, help="frames a track may miss before it is removed (--track)")
+    ap.add_argument("--track_min_hits", type=int, default=3, help="matched frames in a row before a track is reported (--track)")
+    ap.add_argument("--track_iou", type=float, default=0.3, help="least IoU of a detection with its track's prediction (--track)")
     return ap
 
 
