@@ -1,0 +1,158 @@
+#!/usr/bin/env python
+"""A checkpoint's tracking on MOTChallenge sequences: CLEAR MOT and the identity metrics per sequence and combined, with the
+tracking (SORT, DetectionPipeline.enable_tracking) and the matching and counting on the GPU (evaluate.MotEval).
+
+    python evaluate_mot.py CKPT SEQ [SEQ ...] --person_class N [--benchmark MOT17 --track_max_age 1 --track_min_hits 3
+                                                                --track_iou 0.3 --results DIR --out mot.json]
+    python -m torch.distributed.run --nproc-per-node 8 evaluate_mot.py ...   # one rank per GPU; rank 0 evaluates
+
+SEQ is a MOTChallenge sequence directory (seqinfo.ini, imDir/%06d<imExt>, gt/gt.txt); a directory without seqinfo.ini
+stands for its subdirectories that have one, sorted by name (such as MOT17/train).  Each sequence is one stream of frame
+positions 0..seqLength-1, tracked from a fresh start.  A missing frame file, or one whose size differs from seqinfo.ini's,
+raises ValueError.  --person_class is the network's class index that MOTChallenge calls pedestrian (14 for VOC, 0 for COCO);
+its records with a track id are the tracker's rows: frame = position + 1, the track id, and the track box as (left, top, w,
+h) with left = xmin + 1 and top = ymin + 1 (MOTChallenge pixels start at 1), in float64.
+
+The protocol is TrackEval's MotChallenge2DBox with its CLEAR and Identity metrics, as oracle/mot_ref.py restates it (not
+compared with TrackEval itself).  --results DIR writes DIR/<name>.txt in MOTChallenge tracker format, floats written with
+repr so that reading a file back gives the evaluated values.  Sequences without gt/gt.txt are tracked and written with
+--results but left out of the metrics.
+"""
+import json
+import os
+import sys
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, ROOT)
+from evaluate_map import load_checked  # noqa: E402
+from serve import ModelArgParser, add_model_args, add_track_args, detect_files, open_pipeline  # noqa: E402
+from k210_yolo_framework_b200.evaluate import MOT_BENCHMARKS, MotEval, load_mot_gt, read_seqinfo  # noqa: E402
+
+COLUMNS = ("MOTA", "MOTP", "IDF1", "IDP", "IDR", "Rcll", "Prcn", "TP", "FP", "FN", "IDSW", "Frag", "MT", "PT", "ML", "IDTP",
+           "IDFP", "IDFN")
+
+
+def find_sequences(paths):
+    """The sequence directories of the command line, in order; a directory without seqinfo.ini gives its subdirectories with
+    one, sorted by name."""
+    out = []
+    for p in paths:
+        if os.path.isfile(os.path.join(p, "seqinfo.ini")):
+            out.append(p)
+            continue
+        subs = sorted(os.path.join(p, d) for d in os.listdir(p) if os.path.isfile(os.path.join(p, d, "seqinfo.ini"))) \
+            if os.path.isdir(p) else []
+        if not subs:
+            raise ValueError(f"{p}: neither a sequence directory (seqinfo.ini) nor a directory of sequences")
+        out += subs
+    return out
+
+
+def tracker_rows(positions, ids, boxes, dets, counts, person_class):
+    """float64 [n, 7] (frame, id, left, top, w, h, conf) of a batch's tracked records of `person_class`, in record order."""
+    ids, boxes, counts = np.asarray(ids), np.asarray(boxes, np.float32), np.asarray(counts)
+    score = np.ascontiguousarray(np.asarray(dets)[:, person_class, :, 4]).view(np.float32)
+    K = ids.shape[2]
+    take = (np.arange(K)[None, :] < counts[:, person_class, None]) & (ids[:, person_class] >= 0)
+    n, k = np.nonzero(take)
+    b = boxes[n, person_class, k].astype(np.float64)
+    frame = np.asarray(positions, np.float64)[n] + 1
+    return np.stack([frame, ids[n, person_class, k].astype(np.float64), b[:, 1] + 1.0, b[:, 0] + 1.0, b[:, 3] - b[:, 1],
+                     b[:, 2] - b[:, 0], score[n, k].astype(np.float64)], 1).reshape(-1, 7)
+
+
+def write_results(path, rows):
+    with open(path, "w") as fh:
+        for r in rows.tolist():
+            fh.write(f"{int(r[0])},{int(r[1])},{r[2]!r},{r[3]!r},{r[4]!r},{r[5]!r},{r[6]!r},-1,-1,-1\n")
+
+
+def evaluate(args):
+    """MotEval's result dict on rank 0 (None without any gt), None on the other ranks."""
+    import torch.distributed as dist
+    seqs = []
+    for d in find_sequences(args.seqs):
+        info = read_seqinfo(d)
+        gt_path = os.path.join(d, "gt", "gt.txt")
+        files = [os.path.join(d, info["imDir"], f"{k + 1:06d}{info['imExt']}") for k in range(info["seqLength"])]
+        missing = [f for f in files if not os.path.isfile(f)]
+        if missing:
+            raise ValueError(f"{info['name']}: frame file {missing[0]} is missing")
+        seqs.append((info, files, gt_path if os.path.isfile(gt_path) else None))
+    if not any(s[2] for s in seqs) and not args.results:
+        raise ValueError("no sequence has gt/gt.txt and --results is not given: nothing to do")
+    pipe, world, rank = open_pipeline(args, args.max_per_class)
+    if not 0 <= args.person_class < args.class_num:
+        raise ValueError(f"--person_class {args.person_class} is outside [0, {args.class_num})")
+    pipe.enable_tracking(args.track_max_age, args.track_min_hits, args.track_iou)
+    ev = MotEval(args.benchmark, device=pipe.device_index) if rank == 0 and any(s[2] for s in seqs) else None
+    if args.results and rank == 0:
+        os.makedirs(args.results, exist_ok=True)
+    gpu_png, gpu_progressive = getattr(args, "gpu_png", False), getattr(args, "gpu_progressive", False)
+    for info, files, gt_path in seqs:
+        name, L, hw = info["name"], info["seqLength"], (info["imHeight"], info["imWidth"])
+        if ev is not None and gt_path:
+            ev.add_sequence(name, load_mot_gt(gt_path, args.benchmark), L)
+        pipe.reset_tracks()
+        rows = []
+        for chunk, dets, counts, (ids, boxes) in detect_files(
+                pipe, list(range(L)), args.decode_threads, lambda k: load_checked(files[k], hw, gpu_png, gpu_progressive),
+                positions=list(range(L))):
+            if rank != 0:
+                continue
+            n = len(chunk)
+            if ev is not None and gt_path:
+                ev.update(name, chunk, ids[:n], boxes[:n], dets[:n], counts[:n], args.person_class)
+            if args.results:
+                rows.append(tracker_rows(chunk, ids[:n], boxes[:n], dets[:n], counts[:n], args.person_class))
+        if args.results and rank == 0:
+            write_results(os.path.join(args.results, name + ".txt"), np.concatenate(rows + [np.zeros((0, 7))]))
+    if world > 1:
+        dist.barrier()
+    return ev.result() if ev is not None else None
+
+
+def report(res):
+    """One row per sequence and a COMBINED row."""
+    rows = [(n, d) for n, d in res["sequences"].items()] + [("COMBINED", res["combined"])]
+    fmt = (lambda k, v: f"{v:.4f}" if isinstance(v, float) else str(v))
+    table = [["sequence"] + list(COLUMNS)] + [[n] + [fmt(k, d[k]) for k in COLUMNS] for n, d in rows]
+    width = [max(len(r[i]) for r in table) for i in range(len(table[0]))]
+    return "\n".join("  ".join(v.rjust(w) for v, w in zip(r, width)) for r in table)
+
+
+def to_json(res):
+    return {"sequences": res["sequences"], "combined": res["combined"]}
+
+
+def build_parser():
+    ap = ModelArgParser()
+    add_model_args(ap)
+    ap.add_argument("seqs", nargs="+", metavar="SEQ", help="MOTChallenge sequence directory, or a directory of them")
+    ap.add_argument("--person_class", type=int, required=True,
+                    help="the network's class index MOTChallenge calls pedestrian (14 for VOC, 0 for COCO)")
+    ap.add_argument("--benchmark", choices=sorted(MOT_BENCHMARKS), default="MOT17")
+    ap.add_argument("--obj_thresh", type=float, default=0.5)
+    ap.add_argument("--iou_thresh", type=float, default=0.5, help="NMS IoU threshold")
+    ap.add_argument("--max_per_class", type=int, default=100)
+    add_track_args(ap)
+    ap.add_argument("--results", default=None, metavar="DIR", help="write DIR/<name>.txt in MOTChallenge tracker format")
+    ap.add_argument("--out", default=None, help="write the table as JSON")
+    return ap
+
+
+def main():
+    args = build_parser().parse_args()
+    res = evaluate(args)
+    if res is None:
+        return
+    print(report(res))
+    if args.out:
+        with open(args.out, "w") as fh:
+            json.dump(to_json(res), fh)
+
+
+if __name__ == "__main__":
+    main()

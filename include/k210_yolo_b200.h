@@ -601,6 +601,46 @@ int k2y_coco_match(k2y_coco *coco, const int32_t *dets_dev, const int32_t *count
 int k2y_coco_result(k2y_coco *coco, double *precision_host, double *recall_host, unsigned *status_host, void *stream);
 int k2y_coco_reset(k2y_coco *coco, void *stream);
 
+/* ------------------------------------------------------------------------------------------
+ * MOTChallenge tracking evaluation on the device: CLEAR MOT and the identity metrics by the protocol of oracle/mot_ref.py
+ * (TrackEval's MotChallenge2DBox preprocessing and its CLEAR and Identity metrics), counts equal and float64 sums equal
+ * bit for bit.
+ *   k2y_mot_create        benchmark 15, 16, 17 or 20 (MOT15 has no distractor removal, MOT20 adds class 6 to the
+ *                         distractors).
+ *   k2y_mot_add_sequence  gt_host [n_gt][8] float64 (frame, id, left, top, w, h, conf, class; frames 1..seq_length, file
+ *                         order within a frame; class 1 for MOT15), uploaded once; *index the sequence's number.  At most
+ *                         K2Y_MOT_MAX_ROWS rows per frame.
+ *   k2y_mot_update        one batch of frames of sequence `seq`, asynchronous on `stream` (one kernel): counts_dev int32
+ *                         [n][C] and ids_dev int32 [n][C][K] / boxes_dev float32 [n][C][K][4] (ymin, xmin, ymax, xmax), the
+ *                         blocks of DetectionPipeline.collect / tracks on the device, strided per frame (in words);
+ *                         positions_dev int64 [n], each frame's position 0..seq_length-1, each given once (unchecked here).
+ *                         The records of person_class with a track id >= 0 become the frame's tracker rows.
+ *   k2y_mot_result        evaluates every sequence; synchronous.  counts_host [sequences][K2Y_MOT_FIELDS]: TP, FP, FN,
+ *                         IDSW, Frag, MT, PT, ML, IDTP, kept gt rows, kept tracker rows, tracker ids; motp_sum_host
+ *                         [sequences]; rounds_host [sequences] the CLEAR rounds, solved_host [sequences] the frame solves
+ *                         that needed an assignment.  status_host: K2Y_MOT_* bits of anything invalid (the results are
+ *                         then meaningless).
+ * Every call of one evaluator is ordered after the previous one, whatever streams they use.
+ * ---------------------------------------------------------------------------------------- */
+#define K2Y_MOT_MAX_ROWS 512              /* gt rows, and tracker rows, of one frame */
+#define K2Y_MOT_MAX_TRACK_ID (1 << 22)    /* tracker ids are below this */
+#define K2Y_MOT_FIELDS 12
+#define K2Y_MOT_TOO_MANY_ROWS 1           /* a frame has more than K2Y_MOT_MAX_ROWS tracker rows (the rest were dropped) */
+#define K2Y_MOT_BAD_ID 2                  /* a track id >= K2Y_MOT_MAX_TRACK_ID */
+#define K2Y_MOT_REPEATED_ID 4             /* a track id twice in one frame */
+#define K2Y_MOT_BAD_BOX 8                 /* a track box that is not finite */
+#define K2Y_MOT_BAD_COUNT 16              /* a count outside [0, max_per_class] (clamped) */
+#define K2Y_MOT_TOO_MANY_IDS 32           /* a sequence's gt ids x tracker ids exceed 2^28 (its identity metrics were skipped) */
+typedef struct k2y_mot k2y_mot;
+int k2y_mot_create(int benchmark, int device, k2y_mot **out);
+int k2y_mot_destroy(k2y_mot *mot);
+int k2y_mot_add_sequence(k2y_mot *mot, const double *gt_host, long long n_gt, int seq_length, int *index);
+int k2y_mot_update(k2y_mot *mot, int seq, const int32_t *counts_dev, const int32_t *ids_dev, const float *boxes_dev,
+                   long long count_stride_words, long long id_stride_words, long long box_stride_words, int n_frames,
+                   const long long *positions_dev, int class_num, int max_per_class, int person_class, void *stream);
+int k2y_mot_result(k2y_mot *mot, long long *counts_host, double *motp_sum_host, int *rounds_host, long long *solved_host,
+                   unsigned *status_host, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

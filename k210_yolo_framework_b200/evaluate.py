@@ -12,11 +12,17 @@ that of oracle/ap_ref.py: IoU without a "+1 pixel" term, and every object counts
 arrays and the 12 summary stats), matched, ranked and reduced by the k2y_coco_* kernels; the protocol is that of
 oracle/coco_ref.py.  ``load_coco_annotations`` reads a COCO instances JSON file, ``coco_results`` writes the records as
 a COCO results list and ``coco_summary`` prints the stats as COCOeval does.
+
+``MotEval``: CLEAR MOT and the identity metrics of tracks on MOTChallenge sequences (TrackEval's MotChallenge2DBox
+preprocessing, CLEAR and Identity, as oracle/mot_ref.py restates them), matched and counted by the k2y_mot_* kernels.
+``read_seqinfo`` and ``load_mot_gt`` read a sequence directory's seqinfo.ini and gt/gt.txt.
 """
 from __future__ import annotations
 
+import configparser
 import ctypes
 import json
+import os
 from typing import List, NamedTuple, Sequence, Tuple
 
 import numpy as np
@@ -352,4 +358,199 @@ class CocoEval:
         h = getattr(self, "_h", None)
         if h:
             lib.k2y_coco_destroy(h)
+            self._h = None
+
+
+MOT_BENCHMARKS = {"MOT15": 15, "MOT16": 16, "MOT17": 17, "MOT20": 20}
+MOT_STATUS = {1: "a frame has more than 512 tracker rows", 2: "a track id is >= 2^22",
+              4: "a track id appears twice in one frame", 8: "a track box is not finite",
+              16: "a record count is outside [0, max_per_class]",
+              32: "a sequence's gt ids x tracker ids exceed 2^28"}
+MOT_MAX_ROWS = 512
+MOT_FIELDS = ("TP", "FP", "FN", "IDSW", "Frag", "MT", "PT", "ML", "IDTP", "gt_rows", "tracker_rows")
+
+
+def read_seqinfo(seq_dir: str) -> dict:
+    """The [Sequence] section of ``seq_dir/seqinfo.ini``: name, imDir, imExt (str), frameRate, seqLength, imWidth, imHeight
+    (int).  ValueError when the file or a key is missing."""
+    path = os.path.join(seq_dir, "seqinfo.ini")
+    cp = configparser.ConfigParser()
+    cp.optionxform = str
+    if not cp.read(path) or "Sequence" not in cp:
+        raise ValueError(f"{path}: no [Sequence] section")
+    sec = cp["Sequence"]
+    try:
+        info = {k: sec[k] for k in ("name", "imDir", "imExt")}
+        info.update({k: int(sec[k]) for k in ("frameRate", "seqLength", "imWidth", "imHeight")})
+    except (KeyError, ValueError) as e:
+        raise ValueError(f"{path}: {e!r}") from None
+    return info
+
+
+def load_mot_gt(path: str, benchmark: str = "MOT17") -> np.ndarray:
+    """float64 rows [n, 8] (frame, id, left, top, w, h, conf, class) of a gt.txt: MOT16/17/20 rows (frame, id, left, top, w,
+    h, conf, class, visibility), MOT15 rows (frame, id, left, top, w, h, conf, x, y, z) read as class 1."""
+    if benchmark not in MOT_BENCHMARKS:
+        raise ValueError(f"benchmark {benchmark!r} is not one of {tuple(MOT_BENCHMARKS)}")
+    rows = np.loadtxt(path, delimiter=",", dtype=np.float64, ndmin=2)
+    if rows.size == 0:
+        return np.zeros((0, 8))
+    want = 10 if benchmark == "MOT15" else 9
+    if rows.shape[1] != want:
+        raise ValueError(f"{path}: {benchmark} gt rows have {want} values, not {rows.shape[1]}")
+    if benchmark == "MOT15":
+        return np.concatenate([rows[:, :7], np.ones((len(rows), 1))], 1)
+    return np.ascontiguousarray(rows[:, :8])
+
+
+def check_mot_gt(name: str, gt: np.ndarray, seq_length: int, benchmark: str) -> None:
+    """ValueError naming the sequence and frame for a frame outside 1..seq_length, an id twice in one frame, a class outside
+    1..13 (MOT16/17/20) or more than MOT_MAX_ROWS rows in one frame."""
+    if not np.all(np.isfinite(gt)):
+        raise ValueError(f"{name}: the gt has a value that is not finite")
+    f = gt[:, 0]
+    bad = np.flatnonzero((f != np.floor(f)) | (f < 1) | (f > seq_length))
+    if len(bad):
+        raise ValueError(f"{name}: gt frame {f[bad[0]]:g} is outside 1..{seq_length}")
+    if benchmark != "MOT15":
+        c = gt[:, 7]
+        bad = np.flatnonzero((c != np.floor(c)) | (c < 1) | (c > 13))
+        if len(bad):
+            raise ValueError(f"{name}: gt class {c[bad[0]]:g} in frame {int(f[bad[0]])} is outside 1..13")
+    pairs = gt[:, :2]
+    uniq, n = np.unique(pairs, axis=0, return_counts=True)
+    if np.any(n > 1):
+        fr, i = uniq[np.argmax(n > 1)]
+        raise ValueError(f"{name}: gt id {i:g} appears twice in frame {int(fr)}")
+    per = np.bincount(f.astype(np.int64), minlength=seq_length + 1)
+    if per.max(initial=0) > MOT_MAX_ROWS:
+        raise ValueError(f"{name}: frame {int(np.argmax(per))} has {per.max()} gt rows, more than {MOT_MAX_ROWS}")
+
+
+def mot_ratios(d: dict) -> dict:
+    """Adds MOTA, MOTP, Rcll, Prcn, IDR, IDP and IDF1 to a dict of the counts and MOTP_sum."""
+    TP, FP, FN, IDSW, IDTP, IDFP, IDFN = (d[k] for k in ("TP", "FP", "FN", "IDSW", "IDTP", "IDFP", "IDFN"))
+    d = dict(d)
+    d["MOTA"] = (TP - FP - IDSW) / max(1, TP + FN)
+    d["MOTP"] = d["MOTP_sum"] / max(1, TP)
+    d["Rcll"] = TP / max(1, TP + FN)
+    d["Prcn"] = TP / max(1, TP + FP)
+    d["IDR"] = IDTP / max(1, IDTP + IDFN)
+    d["IDP"] = IDTP / max(1, IDTP + IDFP)
+    d["IDF1"] = IDTP / max(1, IDTP + 0.5 * IDFP + 0.5 * IDFN)
+    return d
+
+
+class MotEval:
+    """MOTChallenge CLEAR MOT and identity metrics on the GPU.  ``add_sequence`` uploads a sequence's gt once; ``update``
+    takes the tracked record blocks of a batch of its frames; ``result`` evaluates every sequence.  Every call runs on the
+    current CUDA stream, and is ordered after the evaluator's previous call whatever stream that used.
+
+    Caps: 512 gt rows and 512 tracker rows per frame, track ids below 2^22, and gt ids x tracker ids of a sequence up to
+    2^28; past them ``add_sequence`` or ``result`` raises ValueError."""
+
+    def __init__(self, benchmark: str = "MOT17", device=None):
+        require_cuda()
+        if benchmark not in MOT_BENCHMARKS:
+            raise ValueError(f"benchmark {benchmark!r} is not one of {tuple(MOT_BENCHMARKS)}")
+        self.benchmark = benchmark
+        dev = torch.device("cuda", device) if isinstance(device, int) else torch.device(device or "cuda")
+        self.device = torch.device("cuda", torch.cuda.current_device() if dev.index is None else dev.index)
+        self._seqs = {}         # name -> (index, seq_length, positions given)
+        h = ctypes.c_void_p()
+        check(lib.k2y_mot_create(MOT_BENCHMARKS[benchmark], self.device.index, ctypes.byref(h)))
+        self._h = h
+
+    def _stream(self):
+        return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def add_sequence(self, name: str, gt_rows, seq_length: int) -> None:
+        """gt_rows float64 [n, 8] (frame, id, left, top, w, h, conf, class) as ``load_mot_gt`` reads them."""
+        if name in self._seqs:
+            raise ValueError(f"sequence {name!r} was added already")
+        gt = np.ascontiguousarray(np.asarray(gt_rows, np.float64).reshape(-1, 8))
+        seq_length = int(seq_length)
+        if seq_length < 1:
+            raise ValueError(f"{name}: seqLength {seq_length} < 1")
+        check_mot_gt(name, gt, seq_length, self.benchmark)
+        order = np.argsort(gt[:, 0], kind="stable")
+        gt = np.ascontiguousarray(gt[order])
+        idx = ctypes.c_int()
+        with torch.cuda.device(self.device):
+            check(lib.k2y_mot_add_sequence(self._h, gt.ctypes.data, len(gt), seq_length, ctypes.byref(idx)))
+        self._seqs[name] = (idx.value, seq_length, set())
+
+    def update(self, name: str, positions, ids: torch.Tensor, boxes: torch.Tensor, dets: torch.Tensor, counts: torch.Tensor,
+               person_class: int) -> None:
+        """One batch of frames of sequence `name`: positions (host ints, 0..seqLength-1, each once), ids int32 [N, C, K] and
+        boxes float32 [N, C, K, 4] as ``DetectionPipeline.tracks`` returns them, dets int32 [N, C, K, 6] and counts int32
+        [N, C] as ``collect`` does: pinned host views or device tensors, all on one side of the bus.  The records of
+        `person_class` with a track id >= 0 are the frame's tracker rows."""
+        if name not in self._seqs:
+            raise ValueError(f"unknown sequence {name!r}: add_sequence first")
+        idx, L, given = self._seqs[name]
+        pos = [int(p) for p in positions]
+        n = len(pos)
+        if ids.dim() != 3 or n != ids.shape[0]:
+            raise ValueError(f"expected ids [{n}, C, K], got {tuple(ids.shape)}")
+        C, K = int(ids.shape[1]), int(ids.shape[2])
+        if (ids.dtype != torch.int32 or boxes.dtype != torch.float32 or dets.dtype != torch.int32 or counts.dtype != torch.int32
+                or tuple(boxes.shape) != (n, C, K, 4) or tuple(dets.shape) != (n, C, K, 6) or tuple(counts.shape) != (n, C)
+                or tuple(ids.stride()[1:]) != (K, 1) or tuple(boxes.stride()[1:]) != (K * 4, 4, 1) or counts.stride(1) != 1
+                or len({t.is_cuda for t in (ids, boxes, dets, counts)}) != 1):
+            raise ValueError(f"expected int32 ids [{n}, {C}, {K}], float32 boxes [{n}, {C}, {K}, 4], int32 dets [{n}, {C}, {K}, 6] "
+                             f"and counts [{n}, {C}], dense per frame, on one side of the bus")
+        if not 0 <= int(person_class) < C:
+            raise ValueError(f"person_class {person_class} is outside [0, {C})")
+        for p in pos:
+            if not 0 <= p < L:
+                raise ValueError(f"{name}: frame position {p} is outside 0..{L - 1} (frame {p + 1} outside 1..{L})")
+            if p in given:
+                raise ValueError(f"{name}: frame {p + 1} was given twice")
+            given.add(p)
+        if n == 0:
+            return
+        with torch.cuda.device(self.device):
+            if ids.is_cuda:
+                if any(t.device != self.device for t in (ids, boxes, counts)):
+                    raise ValueError(f"blocks on {ids.device}, evaluator on {self.device}")
+            else:   # a blocking copy: the host views may be overwritten as soon as this returns
+                ids, boxes, counts = ids.to(self.device), boxes.to(self.device), counts.to(self.device)
+            p = torch.tensor(pos, dtype=torch.int64).to(self.device)
+            check(lib.k2y_mot_update(self._h, idx, counts.data_ptr(), ids.data_ptr(), boxes.data_ptr(), counts.stride(0),
+                                     ids.stride(0), boxes.stride(0), n, p.data_ptr(), C, K, int(person_class), self._stream()))
+
+    def result(self) -> dict:
+        """``{"sequences": {name: fields}, "combined": fields, "rounds": {name: CLEAR rounds}, "solved": {name: frame solves
+        that needed an assignment}}``; fields: TP, FP, FN, IDSW, Frag, MT, PT, ML, IDTP, IDFP, IDFN, gt_rows, tracker_rows
+        (int), MOTP_sum, MOTA, MOTP, Rcll, Prcn, IDR, IDP, IDF1 (float).  Integer fields and MOTP_sum (in sequence order)
+        are summed over the sequences and the ratios recomputed.  ``ValueError`` if an update held invalid input."""
+        S = len(self._seqs)
+        counts = np.zeros((max(S, 1), 12), np.int64)
+        motp = np.zeros(max(S, 1))
+        rounds = np.zeros(max(S, 1), np.int32)
+        solved = np.zeros(max(S, 1), np.int64)
+        status = ctypes.c_uint()
+        with torch.cuda.device(self.device):
+            check(lib.k2y_mot_result(self._h, counts.ctypes.data, motp.ctypes.data, rounds.ctypes.data, solved.ctypes.data,
+                                     ctypes.byref(status), self._stream()))
+        if status.value:
+            raise ValueError("MotEval: " + "; ".join(m for bit, m in MOT_STATUS.items() if status.value & bit))
+        seqs, out_rounds, out_solved = {}, {}, {}
+        for name, (i, _, _) in self._seqs.items():
+            d = {k: int(v) for k, v in zip(MOT_FIELDS, counts[i, :11])}
+            d.update(IDFN=d["gt_rows"] - d["IDTP"], IDFP=d["tracker_rows"] - d["IDTP"], MOTP_sum=float(motp[i]))
+            seqs[name] = mot_ratios(d)
+            out_rounds[name], out_solved[name] = int(rounds[i]), int(solved[i])
+        comb = {k: sum(d[k] for d in seqs.values()) for k in MOT_FIELDS + ("IDFN", "IDFP")}
+        s = 0.0
+        for d in seqs.values():
+            s += d["MOTP_sum"]
+        comb["MOTP_sum"] = s
+        return {"sequences": seqs, "combined": mot_ratios(comb), "rounds": out_rounds, "solved": out_solved}
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            lib.k2y_mot_destroy(h)
             self._h = None

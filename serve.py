@@ -363,10 +363,15 @@ def build_parser():
     ap.add_argument("--draw_quality", type=quality_arg, default=75, help="JPEG quality of the --draw files (1..100)")
     ap.add_argument("--track", action="store_true",
                     help="track objects across a video's frames on the GPU (SORT): each detection gains its track id and box")
-    ap.add_argument("--track_max_age", type=int, default=1, help="frames a track may miss before it is removed (--track)")
-    ap.add_argument("--track_min_hits", type=int, default=3, help="matched frames in a row before a track is reported (--track)")
-    ap.add_argument("--track_iou", type=float, default=0.3, help="least IoU of a detection with its track's prediction (--track)")
+    add_track_args(ap, " (--track)")
     return ap
+
+
+def add_track_args(ap, note=""):
+    """The SORT setting flags serve.py and evaluate_mot.py share (DetectionPipeline.enable_tracking)."""
+    ap.add_argument("--track_max_age", type=int, default=1, help="frames a track may miss before it is removed" + note)
+    ap.add_argument("--track_min_hits", type=int, default=3, help="matched frames in a row before a track is reported" + note)
+    ap.add_argument("--track_iou", type=float, default=0.3, help="least IoU of a detection with its track's prediction" + note)
 
 
 def main():
