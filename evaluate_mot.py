@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""A checkpoint's tracking on MOTChallenge sequences: CLEAR MOT and the identity metrics per sequence and combined, with the
-tracking (SORT, DetectionPipeline.enable_tracking) and the matching and counting on the GPU (evaluate.MotEval).
+"""A checkpoint's tracking on MOTChallenge sequences: CLEAR MOT, the identity metrics and HOTA per sequence and combined,
+with the tracking (SORT, DetectionPipeline.enable_tracking) and the matching and counting on the GPU (evaluate.MotEval).
 
     python evaluate_mot.py CKPT SEQ [SEQ ...] --person_class N [--benchmark MOT17 --track_max_age 1 --track_min_hits 3
                                                                 --track_iou 0.3 --results DIR --out mot.json]
@@ -13,8 +13,10 @@ raises ValueError.  --person_class is the network's class index that MOTChalleng
 its records with a track id are the tracker's rows: frame = position + 1, the track id, and the track box as (left, top, w,
 h) with left = xmin + 1 and top = ymin + 1 (MOTChallenge pixels start at 1), in float64.
 
-The protocol is TrackEval's MotChallenge2DBox with its CLEAR and Identity metrics, as oracle/mot_ref.py restates it (not
-compared with TrackEval itself).  --results DIR writes DIR/<name>.txt in MOTChallenge tracker format, floats written with
+The protocol is TrackEval's MotChallenge2DBox with its CLEAR, Identity and HOTA metrics, as oracle/mot_ref.py and
+oracle/mot_hota_ref.py restate them (not compared with TrackEval itself).  The first table holds CLEAR and Identity; the
+second HOTA, DetA, AssA, DetRe, DetPr, AssRe, AssPr, LocA and OWTA, each the mean over the 19 alphas 0.05 .. 0.95 as
+TrackEval's summary shows it, and HOTA(0), LocA(0) and HOTALocA(0).  --out writes both, the HOTA fields per alpha.  --results DIR writes DIR/<name>.txt in MOTChallenge tracker format, floats written with
 repr so that reading a file back gives the evaluated values.  Sequences without gt/gt.txt are tracked and written with
 --results but left out of the metrics.
 """
@@ -30,6 +32,8 @@ from evaluate_map import load_checked  # noqa: E402
 from serve import ModelArgParser, add_model_args, add_track_args, detect_files, open_pipeline  # noqa: E402
 from k210_yolo_framework_b200.evaluate import MOT_BENCHMARKS, MotEval, load_mot_gt, read_seqinfo  # noqa: E402
 
+HOTA_COLUMNS = ("HOTA", "DetA", "AssA", "DetRe", "DetPr", "AssRe", "AssPr", "LocA", "OWTA", "HOTA(0)", "LocA(0)",
+                "HOTALocA(0)")
 COLUMNS = ("MOTA", "MOTP", "IDF1", "IDP", "IDR", "Rcll", "Prcn", "TP", "FP", "FN", "IDSW", "Frag", "MT", "PT", "ML", "IDTP",
            "IDFP", "IDFN")
 
@@ -114,17 +118,33 @@ def evaluate(args):
     return ev.result() if ev is not None else None
 
 
-def report(res):
-    """One row per sequence and a COMBINED row."""
-    rows = [(n, d) for n, d in res["sequences"].items()] + [("COMBINED", res["combined"])]
-    fmt = (lambda k, v: f"{v:.4f}" if isinstance(v, float) else str(v))
-    table = [["sequence"] + list(COLUMNS)] + [[n] + [fmt(k, d[k]) for k in COLUMNS] for n, d in rows]
+def _table(rows, columns):
+    fmt = (lambda v: f"{v:.4f}" if isinstance(v, float) else str(v))
+    table = [["sequence"] + list(columns)] + [[n] + [fmt(d[k]) for k in columns] for n, d in rows]
     width = [max(len(r[i]) for r in table) for i in range(len(table[0]))]
     return "\n".join("  ".join(v.rjust(w) for v, w in zip(r, width)) for r in table)
 
 
+def hota_summary(d):
+    """TrackEval's summary of one HOTA dict: each per-alpha field's mean over the 19 alphas, and the (0) scalars."""
+    out = {k: float(np.mean(d[k])) for k in HOTA_COLUMNS[:9]}
+    out.update({k: d[k] for k in HOTA_COLUMNS[9:]})
+    return out
+
+
+def report(res):
+    """One row per sequence and a COMBINED row of CLEAR and Identity; then the same rows of HOTA (means over alphas)."""
+    rows = [(n, d) for n, d in res["sequences"].items()] + [("COMBINED", res["combined"])]
+    text = _table(rows, COLUMNS)
+    if "hota" in res:
+        h = res["hota"]
+        rows = [(n, hota_summary(d)) for n, d in h["sequences"].items()] + [("COMBINED", hota_summary(h["combined"]))]
+        text += "\n\n" + _table(rows, HOTA_COLUMNS)
+    return text
+
+
 def to_json(res):
-    return {"sequences": res["sequences"], "combined": res["combined"]}
+    return {"sequences": res["sequences"], "combined": res["combined"], "hota": res["hota"]}
 
 
 def build_parser():

@@ -620,6 +620,11 @@ int k2y_coco_reset(k2y_coco *coco, void *stream);
  *                         [sequences]; rounds_host [sequences] the CLEAR rounds, solved_host [sequences] the frame solves
  *                         that needed an assignment.  status_host: K2Y_MOT_* bits of anything invalid (the results are
  *                         then meaningless).
+ *   k2y_mot_result_ex     k2y_mot_result, and HOTA (oracle/mot_hota_ref.py) of every sequence when hota_counts_host and
+ *                         hota_sums_host are given (both or neither): hota_counts_host [sequences][3][K2Y_MOT_HOTA_ALPHAS]
+ *                         TP, FN, FP and hota_sums_host [sequences][4][K2Y_MOT_HOTA_ALPHAS] the float64 sums LocA, AssA,
+ *                         AssRe, AssPr per alpha (0.05, 0.10, ..., 0.95 as np.arange gives them), before their divisions.
+ *                         A sequence past the id cap keeps zeros there.  k2y_mot_result is k2y_mot_result_ex without HOTA.
  * Every call of one evaluator is ordered after the previous one, whatever streams they use.
  * ---------------------------------------------------------------------------------------- */
 #define K2Y_MOT_MAX_ROWS 512              /* gt rows, and tracker rows, of one frame */
@@ -631,6 +636,7 @@ int k2y_coco_reset(k2y_coco *coco, void *stream);
 #define K2Y_MOT_BAD_BOX 8                 /* a track box that is not finite */
 #define K2Y_MOT_BAD_COUNT 16              /* a count outside [0, max_per_class] (clamped) */
 #define K2Y_MOT_TOO_MANY_IDS 32           /* a sequence's gt ids x tracker ids exceed 2^28 (its identity metrics were skipped) */
+#define K2Y_MOT_HOTA_ALPHAS 19            /* HOTA's localisation thresholds */
 typedef struct k2y_mot k2y_mot;
 int k2y_mot_create(int benchmark, int device, k2y_mot **out);
 int k2y_mot_destroy(k2y_mot *mot);
@@ -640,6 +646,8 @@ int k2y_mot_update(k2y_mot *mot, int seq, const int32_t *counts_dev, const int32
                    const long long *positions_dev, int class_num, int max_per_class, int person_class, void *stream);
 int k2y_mot_result(k2y_mot *mot, long long *counts_host, double *motp_sum_host, int *rounds_host, long long *solved_host,
                    unsigned *status_host, void *stream);
+int k2y_mot_result_ex(k2y_mot *mot, long long *counts_host, double *motp_sum_host, int *rounds_host, long long *solved_host,
+                      long long *hota_counts_host, double *hota_sums_host, unsigned *status_host, void *stream);
 
 #ifdef __cplusplus
 }

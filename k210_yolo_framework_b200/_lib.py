@@ -177,6 +177,8 @@ _SIGNATURES = {
     "k2y_mot_update": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong,
                                c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     "k2y_mot_result": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(ctypes.c_uint), c_void_p]),
+    "k2y_mot_result_ex": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(ctypes.c_uint),
+                                  c_void_p]),
 }
 # include/region_layer.h (ABI-compatible firmware API)
 _REGION_ABI = ["region_layer_init", "region_layer_deinit", "region_layer_run", "region_layer_draw_boxes"]

@@ -14,6 +14,9 @@
 //             then MOTP_sum over the frames in order, serially;
 //   stage D   IDTP: one warp solves the maximum-weight matching of the potential-match counts (an exact assignment on
 //             the dense gt id x tracker id matrix; the value is unique).
+// With k2y_mot_result_ex, HOTA (oracle/mot_hota_ref.py) follows on stage A's kept rows: tracker ids ranked by sorted id,
+// per-frame row / column sums, potential-match sums per gt id in frame order, one assignment per frame of its score matrix,
+// per-pair match counts, and the association sums in numpy's pairwise order over the non-zero pairs.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -58,6 +61,8 @@ struct Dev {
     int *n = nullptr;           // [0] tracker ids seen, [1] frames changed in a round, [2] frames solved in a round
     unsigned *status = nullptr;
     int *tmap = nullptr;        // [MAX_ID]: dense index of a tracker id, -1 elsewhere
+    unsigned *hbits = nullptr;  // [MAX_ID / 32]: HOTA's kept tracker ids as bits, cleared after each sequence
+    long long *hwpre = nullptr; // [MAX_ID / 32 + 1]: kept ids in the words before each word (the sorted rank's base)
 };
 
 __device__ __forceinline__ double box_iou(const double *a, const double *b) {
@@ -446,6 +451,428 @@ __global__ void __launch_bounds__(32) mot_idtp_kernel(Seq q, const int *pairs, L
     if (threadIdx.x == 0) q.ctr[IDTP] = (unsigned long long)s;
 }
 
+// ---- HOTA (oracle/mot_hota_ref.py), on stage A's kept rows -------------------------------------------------------------
+constexpr int NA = K2Y_MOT_HOTA_ALPHAS;
+constexpr int NW = MAX_ID / 32;                  // words of the kept-tracker-id bitmap
+// np.arange(0.05, 0.99, 0.05); a match counts at alpha a when IoU >= alpha - eps
+__constant__ double c_alpha[NA] = {0.05, 0.1, 0.15000000000000002, 0.2, 0.25, 0.3, 0.35000000000000003, 0.4, 0.45, 0.5,
+                                   0.55, 0.6000000000000001, 0.6500000000000001, 0.7000000000000001, 0.7500000000000001,
+                                   0.8, 0.8500000000000001, 0.9000000000000001, 0.9500000000000001};
+
+struct Hota {
+    // per frame slot [L][CAP]: row sums (pairwise) and column sums (sequential) of S, positive entries per row, the sorted
+    // rank of each kept tracker row, and each kept gt row's HOTA match (column or -1) and level (the alphas it counts at)
+    double *rsum, *csum;
+    int *rowcnt, *trank, *hm, *hl;
+    int *msize, *ftp, *tc, *gcnt, *gdist;      // [L] ng * nt, [L][NA] matches, [T] frames per tracker rank, [G] x 2
+    long long *moff, *gseg, *poff;             // exclusive prefixes of msize, gcnt, gdist (with the total at the end)
+    double *floc, *M;                          // [L][NA] IoU sums; score matrices gas * S, [moff[L]]
+    // entries: one per (frame, kept gt row, kept tracker row) with S > 0, by gt id and then frame
+    int *et, *ef, *eij;                        // tracker rank, frame, i * CAP + j
+    double *ev, *es;                           // sim_iou, S
+    unsigned char *efirst, *elvl;              // first entry of its (gt id, tracker rank) in the gt id's list; HOTA level
+    // pairs (gt id, tracker rank) with an entry, by position g * T + t
+    long long *ppos;
+    int *pgc, *ptc, *pmc;                      // gt id's and tracker's frame counts, [P][NA] match counts
+    long long *cnt;                            // [3][NA] TP, FN, FP
+    double *sum;                               // [4][NA] LocA, AssA, AssRe, AssPr sums
+    int Th;                                    // kept tracker ids
+};
+
+// Exclusive prefix of in(0..n-1) into out[0..n], out[n] the total; one block of 1024 threads.
+struct PopcIn {
+    const unsigned *w;
+    __device__ long long operator()(int k) const { return __popc(w[k]); }
+};
+struct IntIn {
+    const int *p;
+    __device__ long long operator()(int k) const { return p[k]; }
+};
+template <class In>
+__global__ void __launch_bounds__(1024) hota_scan_kernel(In in, int n, long long *out) {
+    __shared__ long long part[1024];
+    const int t = threadIdx.x, per = (n + 1023) / 1024, b = min(n, t * per), e = min(n, b + per);
+    long long s = 0;
+    for (int k = b; k < e; ++k) s += in(k);
+    part[t] = s;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) {
+        const long long v = t >= o ? part[t - o] : 0;
+        __syncthreads();
+        part[t] += v;
+        __syncthreads();
+    }
+    long long run = part[t] - s;
+    for (int k = b; k < e; ++k) {
+        out[k] = run;
+        run += in(k);
+    }
+    if (t == 1023) out[n] = part[1023];
+}
+
+// The kept tracker ids as bits, then each kept row's rank among them (np.unique's index) and its tracker's frame count.
+__global__ void hota_mark_kernel(Seq q, unsigned *bits) {
+    const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (e >= (long long)q.L * CAP) return;
+    const int f = (int)(e / CAP), j = (int)(e % CAP);
+    if (j >= q.tkn[f]) return;
+    const int id = q.tid[(size_t)f * CAP + q.tkeep[e]];
+    if (id >= 0 && id < MAX_ID) atomicOr(&bits[id >> 5], 1u << (id & 31));
+}
+
+__global__ void hota_rank_kernel(Seq q, const unsigned *bits, const long long *wpre, Hota h) {
+    const long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    if (e >= (long long)q.L * CAP) return;
+    const int f = (int)(e / CAP), j = (int)(e % CAP);
+    if (j >= q.tkn[f]) return;
+    const int id = q.tid[(size_t)f * CAP + q.tkeep[e]];
+    const int r = id >= 0 && id < MAX_ID ? (int)(wpre[id >> 5] + __popc(bits[id >> 5] & ((1u << (id & 31)) - 1u))) : 0;
+    h.trank[e] = r;
+    atomicAdd(&h.tc[r], 1);
+}
+
+// numpy's pairwise sum of v(lo .. lo + n - 1): 8 interleaved accumulators up to 128 elements, split at n / 2 rounded down
+// to a multiple of 8 above (D levels, enough for CAP).
+template <class V>
+__device__ double pw_leaf(const V &v, int lo, int n) {
+    if (n < 8) {
+        double r = 0.0;
+        for (int k = 0; k < n; ++k) r += v(lo + k);
+        return r;
+    }
+    double r0 = v(lo), r1 = v(lo + 1), r2 = v(lo + 2), r3 = v(lo + 3), r4 = v(lo + 4), r5 = v(lo + 5), r6 = v(lo + 6),
+           r7 = v(lo + 7);
+    int i = 8;
+    for (; i < n - n % 8; i += 8) {
+        r0 += v(lo + i), r1 += v(lo + i + 1), r2 += v(lo + i + 2), r3 += v(lo + i + 3);
+        r4 += v(lo + i + 4), r5 += v(lo + i + 5), r6 += v(lo + i + 6), r7 += v(lo + i + 7);
+    }
+    double res = ((r0 + r1) + (r2 + r3)) + ((r4 + r5) + (r6 + r7));
+    for (; i < n; ++i) res += v(lo + i);
+    return res;
+}
+
+template <int D, class V>
+__device__ double pw_dense(const V &v, int lo, int n) {
+    if constexpr (D == 0) {
+        return pw_leaf(v, lo, n);
+    } else {
+        if (n <= 128) return pw_leaf(v, lo, n);
+        int n2 = n / 2;
+        n2 -= n2 % 8;
+        return pw_dense<D - 1>(v, lo, n2) + pw_dense<D - 1>(v, lo + n2, n - n2);
+    }
+}
+static_assert(CAP <= 1024, "pw_dense<4> covers rows of up to 1024 elements");
+
+// One warp per frame: S.sum(1) (pairwise) and S.sum(0) (sequential) of the kept rows, positives per row, ng * nt.
+__global__ void __launch_bounds__(32) hota_frame_sums_kernel(Seq q, Hota h) {
+    const int f = blockIdx.x, lane = threadIdx.x;
+    const int ng = q.koff[f + 1] - q.koff[f], nt = q.tkn[f];
+    const int *kidx = q.kidx + q.koff[f], *tkeep = q.tkeep + (size_t)f * CAP;
+    const double *tbox = q.tbox + (size_t)f * CAP * 4;
+    for (int i = lane; i < ng; i += 32) {
+        const double *g = q.gbox + 4 * kidx[i];
+        auto S = [&](int j) { return box_iou(g, tbox + 4 * tkeep[j]); };
+        int c = 0;
+        for (int j = 0; j < nt; ++j) c += S(j) > 0.0;
+        h.rsum[(size_t)f * CAP + i] = 0.0 + pw_dense<4>(S, 0, nt);
+        h.rowcnt[(size_t)f * CAP + i] = c;
+    }
+    for (int j = lane; j < nt; j += 32) {
+        double s = 0.0;
+        for (int i = 0; i < ng; ++i) s += box_iou(q.gbox + 4 * kidx[i], tbox + 4 * tkeep[j]);
+        h.csum[(size_t)f * CAP + j] = s;
+    }
+    if (lane == 0) h.msize[f] = ng * nt;
+}
+
+// Entries per gt id: the positive S of its rows over its frames.
+__global__ void hota_gcount_kernel(Seq q, Hota h) {
+    const int g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= q.G) return;
+    int n = 0;
+    for (int k = q.idoff[g]; k < q.idoff[g + 1]; ++k) n += h.rowcnt[(size_t)q.idframe[k] * CAP + q.idpos[k]];
+    h.gcnt[g] = n;
+}
+
+// One warp per gt id: its entries in frame order, with sim_iou = S / ((colsum + rowsum) - S) where that is > eps.
+__global__ void __launch_bounds__(32) hota_gather_kernel(Seq q, Hota h) {
+    const int g = blockIdx.x, lane = threadIdx.x;
+    long long base = h.gseg[g];
+    for (int k = q.idoff[g]; k < q.idoff[g + 1]; ++k) {
+        const int f = q.idframe[k], i = q.idpos[k], nt = q.tkn[f];
+        const double *gb = q.gbox + 4 * q.kidx[q.koff[f] + i];
+        const double rs = h.rsum[(size_t)f * CAP + i];
+        for (int j0 = 0; j0 < nt; j0 += 32) {
+            const int j = j0 + lane;
+            const double s = j < nt ? box_iou(gb, q.tbox + ((size_t)f * CAP + q.tkeep[(size_t)f * CAP + j]) * 4) : 0.0;
+            const unsigned b = __ballot_sync(0xffffffffu, s > 0.0);
+            if (s > 0.0) {
+                const long long e = base + __popc(b & ((1u << lane) - 1u));
+                const double den = (h.csum[(size_t)f * CAP + j] + rs) - s;
+                h.et[e] = h.trank[(size_t)f * CAP + j];
+                h.ev[e] = den > EPS ? s / den : 0.0;
+                h.es[e] = s;
+                h.ef[e] = f;
+                h.eij[e] = i * CAP + j;
+            }
+            base += __popc(b);
+        }
+    }
+}
+
+// One warp per gt id: pmc[g, t] = the entries' sim_iou summed in frame order, gas = pmc / ((gc + tc) - pmc), and each
+// entry's score gas * S into its frame's matrix; which entries come first for their tracker, and how many pairs.
+__global__ void __launch_bounds__(32) hota_pmc_kernel(Seq q, Hota h) {
+    const int g = blockIdx.x, lane = threadIdx.x;
+    const long long b = h.gseg[g], end = h.gseg[g + 1];
+    const double gc = (double)(q.idoff[g + 1] - q.idoff[g]);
+    int firsts = 0;
+    for (long long e = b + lane; e < end; e += 32) {
+        const int t = h.et[e];
+        double pmc = 0.0;
+        bool first = true;
+        for (long long e2 = b; e2 < end; ++e2)
+            if (h.et[e2] == t) {
+                pmc += h.ev[e2];
+                first &= e2 >= e;
+            }
+        const double gas = pmc / ((gc + (double)h.tc[t]) - pmc);
+        const int f = h.ef[e], ij = h.eij[e];
+        h.M[h.moff[f] + (long long)(ij / CAP) * q.tkn[f] + ij % CAP] = __dmul_rn(gas, h.es[e]);
+        h.efirst[e] = first;
+        firsts += first;
+    }
+    firsts = __reduce_add_sync(0xffffffffu, firsts);
+    if (lane == 0) h.gdist[g] = firsts;
+}
+
+struct ScoreCost {
+    const double *m;
+    int nt;
+    __device__ double operator()(int i, int j) const { return -m[i * nt + j]; }
+};
+
+// One warp per frame with gt and tracker rows: lsap(-score) once (or the positives when they are isolated), each row's
+// match and level, then per alpha the matches and their IoU sum in row order.
+__global__ void __launch_bounds__(32) hota_frame_kernel(Seq q, Hota h) {
+    __shared__ WarpSmem s;
+    const int f = blockIdx.x, lane = threadIdx.x;
+    const int ng = q.koff[f + 1] - q.koff[f], nt = q.tkn[f];
+    if (ng == 0 || nt == 0) {
+        if (lane < NA) {
+            h.ftp[f * NA + lane] = 0;
+            h.floc[f * NA + lane] = 0.0;
+        }
+        return;
+    }
+    const double *M = h.M + h.moff[f];
+    ScoreCost cost{M, nt};
+    auto pos = [&](int i, int j) { return M[i * nt + j] > 0.0; };
+    if (positives_isolated(ng, nt, pos, s)) {
+        for (int i = lane; i < ng; i += 32) {
+            int m = -1;
+            for (int j = 0; j < nt; ++j)
+                if (pos(i, j)) m = j;
+            s.match[i] = m;
+        }
+        __syncwarp();
+    } else {
+        warp_lsap(ng, nt, cost, smem_work(s), s.match);
+    }
+    const int *kidx = q.kidx + q.koff[f], *tkeep = q.tkeep + (size_t)f * CAP;
+    for (int i = lane; i < ng; i += 32) {
+        const int j = s.match[i];
+        int lvl = 0;
+        double v = 0.0;
+        if (j >= 0 && pos(i, j)) {
+            v = box_iou(q.gbox + 4 * kidx[i], q.tbox + ((size_t)f * CAP + tkeep[j]) * 4);
+            for (int a = 0; a < NA; ++a) lvl += v >= c_alpha[a] - EPS;
+        }
+        h.hm[(size_t)f * CAP + i] = lvl > 0 ? j : -1;
+        h.hl[(size_t)f * CAP + i] = lvl;
+        s.u[i] = v;
+        s.cnt_r[i] = lvl;
+    }
+    __syncwarp();
+    if (lane < NA) {
+        int tp = 0;
+        double loc = 0.0;
+        for (int i = 0; i < ng; ++i)
+            if (s.cnt_r[i] > lane) {
+                ++tp;
+                loc += s.u[i];
+            }
+        h.ftp[f * NA + lane] = tp;
+        h.floc[f * NA + lane] = loc;
+    }
+}
+
+// TP / FN / FP per alpha, and LocA_sum over the frames in order (one lane per alpha).
+__global__ void hota_total_kernel(Seq q, Hota h) {
+    const int a = threadIdx.x;
+    if (a >= NA) return;
+    long long tp = 0, fn = 0, fp = 0;
+    double loc = 0.0;
+    for (int f = 0; f < q.L; ++f) {
+        const int ng = q.koff[f + 1] - q.koff[f], nt = q.tkn[f];
+        if (ng == 0) {
+            fp += nt;
+        } else if (nt == 0) {
+            fn += ng;
+        } else {
+            const int m = h.ftp[f * NA + a];
+            tp += m;
+            fn += ng - m;
+            fp += nt - m;
+            loc += h.floc[f * NA + a];
+        }
+    }
+    h.cnt[a] = tp;
+    h.cnt[NA + a] = fn;
+    h.cnt[2 * NA + a] = fp;
+    h.sum[a] = loc;
+}
+
+// One warp per gt id: each pair's position (its tracker's rank among the gt id's trackers) and its match count per alpha.
+__global__ void __launch_bounds__(32) hota_pairs_kernel(Seq q, Hota h) {
+    const int g = blockIdx.x, lane = threadIdx.x;
+    const long long b = h.gseg[g], end = h.gseg[g + 1];
+    for (long long e = b + lane; e < end; e += 32) {
+        const int f = h.ef[e], ij = h.eij[e];
+        const size_t r = (size_t)f * CAP + ij / CAP;
+        h.elvl[e] = h.hm[r] == ij % CAP ? (unsigned char)h.hl[r] : 0;
+    }
+    __syncwarp();
+    for (long long e = b + lane; e < end; e += 32) {
+        if (!h.efirst[e]) continue;
+        const int t = h.et[e];
+        int rank = 0, m[NA];
+#pragma unroll
+        for (int a = 0; a < NA; ++a) m[a] = 0;
+        for (long long e2 = b; e2 < end; ++e2) {
+            const int t2 = h.et[e2];
+            rank += h.efirst[e2] && t2 < t;
+            if (t2 == t) {
+                const int lv = h.elvl[e2];
+#pragma unroll
+                for (int a = 0; a < NA; ++a) m[a] += lv > a;
+            }
+        }
+        const long long p = h.poff[g] + rank;
+        h.ppos[p] = (long long)g * h.Th + t;
+        h.pgc[p] = q.idoff[g + 1] - q.idoff[g];
+        h.ptc[p] = h.tc[t];
+#pragma unroll
+        for (int a = 0; a < NA; ++a) h.pmc[p * NA + a] = m[a];
+    }
+}
+
+// mc * (mc / den) of pair p for sum `kind` (0 AssA, 1 AssRe, 2 AssPr) at alpha a.
+__device__ __forceinline__ double ass_value(const Hota &h, long long p, int kind, int a) {
+    const double m = (double)h.pmc[p * NA + a], gc = (double)h.pgc[p], tc = (double)h.ptc[p];
+    const double den = kind == 0 ? fmax(1.0, (gc + tc) - m) : fmax(1.0, kind == 1 ? gc : tc);
+    return __dmul_rn(m, m / den);
+}
+
+// The association sums: numpy's pairwise sum over the dense G x T array, walked over the sorted pairs (zeros are neutral,
+// so empty subtrees are skipped).  One warp; lane l computes sums l and l + 32 of the 3 x NA, all on one walk.
+__global__ void __launch_bounds__(32) hota_assoc_kernel(Hota h, int G, long long n) {
+    constexpr int DEPTH = 64;
+    __shared__ long long s_lo[DEPTH], s_n[DEPTH];
+    __shared__ int s_st[DEPTH];
+    __shared__ double s_left[DEPTH][2][32];
+    const int lane = threadIdx.x;
+    const long long P = h.poff[G];
+    const int c1 = lane + 32 < 3 * NA ? lane + 32 : lane;
+    const int k0 = lane / NA, a0 = lane % NA, k1 = c1 / NA, a1 = c1 % NA;
+    if (lane == 0) {
+        s_lo[0] = 0;
+        s_n[0] = n;
+        s_st[0] = 0;
+    }
+    __syncwarp();
+    int sp = 0;
+    long long k = 0;
+    double v0 = 0.0, v1 = 0.0;
+    while (true) {
+        const long long lo = s_lo[sp], len = s_n[sp];
+        const int st = s_st[sp];
+        long long n2 = len / 2;
+        n2 -= n2 % 8;
+        if (st == 0 && !(k >= P || h.ppos[k] >= lo + len) && len > 128) {
+            __syncwarp();
+            if (lane == 0) {
+                s_st[sp] = 1;
+                s_lo[sp + 1] = lo;
+                s_n[sp + 1] = n2;
+                s_st[sp + 1] = 0;
+            }
+            ++sp;
+            __syncwarp();
+            continue;
+        }
+        if (st == 1) {
+            s_left[sp][0][lane] = v0;
+            s_left[sp][1][lane] = v1;
+            __syncwarp();
+            if (lane == 0) {
+                s_st[sp] = 2;
+                s_lo[sp + 1] = lo + n2;
+                s_n[sp + 1] = len - n2;
+                s_st[sp + 1] = 0;
+            }
+            ++sp;
+            __syncwarp();
+            continue;
+        }
+        if (st == 2) {
+            v0 = s_left[sp][0][lane] + v0;
+            v1 = s_left[sp][1][lane] + v1;
+        } else if (k >= P || h.ppos[k] >= lo + len) {
+            v0 = v1 = 0.0;
+        } else {        // a leaf with pairs: numpy's 8 accumulators over the block, the remainder after them
+            const long long nb = len - len % 8;
+            double r0[8], r1[8], x0 = 0.0, x1 = 0.0;
+#pragma unroll
+            for (int c = 0; c < 8; ++c) r0[c] = r1[c] = 0.0;
+            bool tree = false;
+            for (; k < P && h.ppos[k] < lo + len; ++k) {
+                const long long d = h.ppos[k] - lo;
+                const double y0 = ass_value(h, k, k0, a0), y1 = ass_value(h, k, k1, a1);
+                if (d < nb) {
+                    const int c = (int)(d & 7);
+#pragma unroll
+                    for (int u = 0; u < 8; ++u)
+                        if (u == c) {
+                            r0[u] += y0;
+                            r1[u] += y1;
+                        }
+                    continue;
+                }
+                if (!tree) {
+                    x0 = ((r0[0] + r0[1]) + (r0[2] + r0[3])) + ((r0[4] + r0[5]) + (r0[6] + r0[7]));
+                    x1 = ((r1[0] + r1[1]) + (r1[2] + r1[3])) + ((r1[4] + r1[5]) + (r1[6] + r1[7]));
+                    tree = true;
+                }
+                x0 += y0;
+                x1 += y1;
+            }
+            if (!tree) {
+                x0 = ((r0[0] + r0[1]) + (r0[2] + r0[3])) + ((r0[4] + r0[5]) + (r0[6] + r0[7]));
+                x1 = ((r1[0] + r1[1]) + (r1[2] + r1[3])) + ((r1[4] + r1[5]) + (r1[6] + r1[7]));
+            }
+            v0 = x0;
+            v1 = x1;
+        }
+        if (sp == 0) break;
+        --sp;
+    }
+    h.sum[NA + lane] = 0.0 + v0;
+    if (lane + 32 < 3 * NA) h.sum[NA + lane + 32] = 0.0 + v1;
+}
+
 template <class T>
 cudaError_t dalloc(T **p, size_t n) {
     return cudaMalloc((void **)p, std::max<size_t>(n, 1) * sizeof(T));
@@ -505,6 +932,9 @@ extern "C" int k2y_mot_create(int benchmark, int device, k2y_mot **out) {
     if (e == cudaSuccess) e = dalloc(&h->d.status, 1);
     if (e == cudaSuccess) e = dalloc(&h->d.tmap, MAX_ID);
     if (e == cudaSuccess) e = cudaMemset(h->d.tmap, 0xff, sizeof(int) * (size_t)MAX_ID);
+    if (e == cudaSuccess) e = dalloc(&h->d.hbits, MAX_ID / 32);
+    if (e == cudaSuccess) e = dalloc(&h->d.hwpre, MAX_ID / 32 + 1);
+    if (e == cudaSuccess) e = cudaMemset(h->d.hbits, 0, sizeof(unsigned) * (MAX_ID / 32));
     if (e == cudaSuccess) e = cudaMemset(h->d.status, 0, sizeof(unsigned));
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&h->done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaDeviceSynchronize();
@@ -525,6 +955,8 @@ extern "C" int k2y_mot_destroy(k2y_mot *h) {
     cudaFree(h->d.n);
     cudaFree(h->d.status);
     cudaFree(h->d.tmap);
+    cudaFree(h->d.hbits);
+    cudaFree(h->d.hwpre);
     if (h->done) cudaEventDestroy(h->done);
     delete h;
     return K2Y_OK;
@@ -738,9 +1170,81 @@ static cudaError_t evaluate_seq(k2y_mot *h, Seq &q, cudaStream_t st, int *host_n
     return cudaGetLastError();
 }
 
-extern "C" int k2y_mot_result(k2y_mot *h, long long *counts_host, double *motp_sum_host, int *rounds_host,
-                              long long *solved_host, unsigned *status_host, void *stream) {
-    if (!h || (!h->seqs.empty() && (!counts_host || !motp_sum_host || !rounds_host || !solved_host)) || !status_host) {
+// HOTA of one sequence after its CLEAR stages, on stage A's kept slots: counts [3][NA] and sums [4][NA] to the host.
+struct HotaScratch {
+    cudaStream_t st;
+    std::vector<void *> ps;
+    explicit HotaScratch(cudaStream_t s) : st(s) {}
+    template <class T>
+    cudaError_t alloc(T **p, size_t n) {
+        cudaError_t e = dalloc(p, n);
+        if (e == cudaSuccess) ps.push_back(*p);
+        return e;
+    }
+    ~HotaScratch() {
+        cudaStreamSynchronize(st);
+        for (void *p : ps) cudaFree(p);
+    }
+};
+
+static cudaError_t hota_seq(k2y_mot *hd, const Seq &q, cudaStream_t st, long long *cnt_host, double *sum_host) {
+    const int L = q.L, G = q.G;
+    const size_t slots = (size_t)L * CAP;
+    const int blocks = (int)((slots + 255) / 256);
+    HotaScratch x(st);
+    Hota h{};
+    cudaError_t e = cudaSuccess;
+    auto ok = [&](cudaError_t r) { return (e = r) == cudaSuccess; };
+    if (!(ok(x.alloc(&h.rsum, slots)) && ok(x.alloc(&h.csum, slots)) && ok(x.alloc(&h.rowcnt, slots)) &&
+          ok(x.alloc(&h.trank, slots)) && ok(x.alloc(&h.hm, slots)) && ok(x.alloc(&h.hl, slots)) &&
+          ok(x.alloc(&h.msize, L)) && ok(x.alloc(&h.ftp, (size_t)L * NA)) && ok(x.alloc(&h.floc, (size_t)L * NA)) &&
+          ok(x.alloc(&h.tc, std::max(q.T, 1))) && ok(x.alloc(&h.gcnt, G)) && ok(x.alloc(&h.gdist, G)) &&
+          ok(x.alloc(&h.moff, (size_t)L + 1)) && ok(x.alloc(&h.gseg, (size_t)G + 1)) && ok(x.alloc(&h.poff, (size_t)G + 1)) &&
+          ok(x.alloc(&h.cnt, 3 * NA)) && ok(x.alloc(&h.sum, 4 * NA)) &&
+          ok(cudaMemsetAsync(h.tc, 0, sizeof(int) * std::max(q.T, 1), st))))
+        return e;
+    hota_mark_kernel<<<blocks, 256, 0, st>>>(q, hd->d.hbits);
+    hota_scan_kernel<<<1, 1024, 0, st>>>(PopcIn{hd->d.hbits}, NW, hd->d.hwpre);
+    hota_rank_kernel<<<blocks, 256, 0, st>>>(q, hd->d.hbits, hd->d.hwpre, h);
+    if (!ok(cudaMemsetAsync(hd->d.hbits, 0, sizeof(unsigned) * NW, st))) return e;
+    hota_frame_sums_kernel<<<L, 32, 0, st>>>(q, h);
+    if (G > 0) hota_gcount_kernel<<<(G + 127) / 128, 128, 0, st>>>(q, h);
+    hota_scan_kernel<<<1, 1024, 0, st>>>(IntIn{h.gcnt}, G, h.gseg);
+    hota_scan_kernel<<<1, 1024, 0, st>>>(IntIn{h.msize}, L, h.moff);
+    long long sizes[3];       // entries, score matrix elements, kept tracker ids
+    if (!(ok(cudaMemcpyAsync(sizes, h.gseg + G, sizeof(long long), cudaMemcpyDeviceToHost, st)) &&
+          ok(cudaMemcpyAsync(sizes + 1, h.moff + L, sizeof(long long), cudaMemcpyDeviceToHost, st)) &&
+          ok(cudaMemcpyAsync(sizes + 2, hd->d.hwpre + NW, sizeof(long long), cudaMemcpyDeviceToHost, st)) &&
+          ok(cudaStreamSynchronize(st))))
+        return e;
+    const size_t E = (size_t)sizes[0];
+    h.Th = (int)sizes[2];
+    if (!(ok(x.alloc(&h.et, E)) && ok(x.alloc(&h.ef, E)) && ok(x.alloc(&h.eij, E)) && ok(x.alloc(&h.ev, E)) &&
+          ok(x.alloc(&h.es, E)) && ok(x.alloc(&h.efirst, E)) && ok(x.alloc(&h.elvl, E)) && ok(x.alloc(&h.ppos, E)) &&
+          ok(x.alloc(&h.pgc, E)) && ok(x.alloc(&h.ptc, E)) && ok(x.alloc(&h.pmc, E * NA)) &&
+          ok(x.alloc(&h.M, (size_t)sizes[1])) && ok(cudaMemsetAsync(h.M, 0, sizeof(double) * (size_t)sizes[1], st))))
+        return e;
+    if (G > 0) {
+        hota_gather_kernel<<<G, 32, 0, st>>>(q, h);
+        hota_pmc_kernel<<<G, 32, 0, st>>>(q, h);
+    }
+    hota_scan_kernel<<<1, 1024, 0, st>>>(IntIn{h.gdist}, G, h.poff);
+    hota_frame_kernel<<<L, 32, 0, st>>>(q, h);
+    hota_total_kernel<<<1, 32, 0, st>>>(q, h);
+    if (G > 0) hota_pairs_kernel<<<G, 32, 0, st>>>(q, h);
+    hota_assoc_kernel<<<1, 32, 0, st>>>(h, G, (long long)G * h.Th);
+    if (!(ok(cudaGetLastError()) &&
+          ok(cudaMemcpyAsync(cnt_host, h.cnt, sizeof(long long) * 3 * NA, cudaMemcpyDeviceToHost, st)) &&
+          ok(cudaMemcpyAsync(sum_host, h.sum, sizeof(double) * 4 * NA, cudaMemcpyDeviceToHost, st))))
+        return e;
+    return cudaStreamSynchronize(st);
+}
+
+extern "C" int k2y_mot_result_ex(k2y_mot *h, long long *counts_host, double *motp_sum_host, int *rounds_host,
+                                 long long *solved_host, long long *hota_counts_host, double *hota_sums_host,
+                                 unsigned *status_host, void *stream) {
+    if (!h || (!h->seqs.empty() && (!counts_host || !motp_sum_host || !rounds_host || !solved_host)) || !status_host ||
+        (!hota_counts_host != !hota_sums_host)) {
         set_error("k2y_mot_result: null pointer");
         return K2Y_ERR_INVALID;
     }
@@ -763,6 +1267,9 @@ extern "C" int k2y_mot_result(k2y_mot *h, long long *counts_host, double *motp_s
         o[10] = c[TRK_ROWS];
         o[11] = q.T;
         if ((long long)q.G * q.T > MAX_PAIRS) *status_host |= K2Y_MOT_TOO_MANY_IDS;
+        else if (hota_counts_host)
+            e = hota_seq(h, q, st, hota_counts_host + 3 * NA * s, hota_sums_host + 4 * NA * s);
+        if (e != cudaSuccess) break;
     }
     unsigned st_dev = 0;
     if (e == cudaSuccess) e = cudaMemcpyAsync(&st_dev, h->d.status, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
@@ -774,4 +1281,9 @@ extern "C" int k2y_mot_result(k2y_mot *h, long long *counts_host, double *motp_s
     }
     *status_host = st_dev | (*status_host & K2Y_MOT_TOO_MANY_IDS);
     return K2Y_OK;
+}
+
+extern "C" int k2y_mot_result(k2y_mot *h, long long *counts_host, double *motp_sum_host, int *rounds_host,
+                              long long *solved_host, unsigned *status_host, void *stream) {
+    return k2y_mot_result_ex(h, counts_host, motp_sum_host, rounds_host, solved_host, nullptr, nullptr, status_host, stream);
 }

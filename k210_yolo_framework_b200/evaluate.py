@@ -427,6 +427,54 @@ def check_mot_gt(name: str, gt: np.ndarray, seq_length: int, benchmark: str) -> 
         raise ValueError(f"{name}: frame {int(np.argmax(per))} has {per.max()} gt rows, more than {MOT_MAX_ROWS}")
 
 
+HOTA_ALPHAS = 19
+HOTA_ARRAY_FIELDS = ("HOTA", "DetA", "AssA", "DetRe", "DetPr", "AssRe", "AssPr", "LocA", "OWTA", "HOTA_TP", "HOTA_FN",
+                     "HOTA_FP")
+HOTA_SCALAR_FIELDS = ("HOTA(0)", "LocA(0)", "HOTALocA(0)")
+
+
+def hota_final(TP, FN, FP, ass_a, ass_re, ass_pr, loc_a) -> dict:
+    """TrackEval's final HOTA fields from arrays of 19: lists per alpha (counts as ints) and the three (0) scalars."""
+    TP, FN, FP = (np.asarray(x, np.float64) for x in (TP, FN, FP))
+    d = dict(AssA=np.asarray(ass_a, np.float64), AssRe=np.asarray(ass_re, np.float64), AssPr=np.asarray(ass_pr, np.float64),
+             LocA=np.asarray(loc_a, np.float64))
+    d["DetRe"] = TP / np.maximum(1, TP + FN)
+    d["DetPr"] = TP / np.maximum(1, TP + FP)
+    d["DetA"] = TP / np.maximum(1, TP + FN + FP)
+    d["HOTA"] = np.sqrt(d["DetA"] * d["AssA"])
+    d["OWTA"] = np.sqrt(d["DetRe"] * d["AssA"])
+    out = {k: [float(v) for v in d[k]] for k in HOTA_ARRAY_FIELDS if k in d}
+    for k, x in (("HOTA_TP", TP), ("HOTA_FN", FN), ("HOTA_FP", FP)):
+        out[k] = [int(v) for v in x]
+    out["HOTA(0)"] = float(d["HOTA"][0])
+    out["LocA(0)"] = float(d["LocA"][0])
+    out["HOTALocA(0)"] = float(d["HOTA"][0] * d["LocA"][0])
+    return {k: out[k] for k in HOTA_ARRAY_FIELDS + HOTA_SCALAR_FIELDS}
+
+
+def hota_sequence(counts, sums) -> dict:
+    """One sequence's HOTA fields from the device's counts [3][19] (TP, FN, FP) and sums [4][19] (LocA, AssA, AssRe,
+    AssPr): AssX = AssX_sum / max(1, TP), LocA = max(1e-10, LocA_sum) / max(1e-10, TP)."""
+    TP = np.asarray(counts[0], np.float64)
+    ass = [np.asarray(sums[k], np.float64) / np.maximum(1, TP) for k in (1, 2, 3)]
+    loc_a = np.maximum(1e-10, np.asarray(sums[0], np.float64)) / np.maximum(1e-10, TP)
+    return hota_final(counts[0], counts[1], counts[2], ass[0], ass[1], ass[2], loc_a)
+
+
+def hota_combine(results) -> dict:
+    """TrackEval's combine_sequences: counts summed, AssA / AssRe / AssPr and LocA weighted by each sequence's TP, summed in
+    sequence order."""
+    if not results:
+        z = np.zeros(HOTA_ALPHAS)
+        return hota_final(z, z, z, z, z, z, np.ones(HOTA_ALPHAS))
+    TP, FN, FP = (sum(np.asarray(r[k], np.int64) for r in results) for k in ("HOTA_TP", "HOTA_FN", "HOTA_FP"))
+    w = {}
+    for k in ("AssRe", "AssPr", "AssA"):
+        w[k] = sum(np.asarray(r[k], np.float64) * np.asarray(r["HOTA_TP"], np.float64) for r in results) / np.maximum(1.0, TP)
+    loc = sum(np.asarray(r["LocA"], np.float64) * np.asarray(r["HOTA_TP"], np.float64) for r in results)
+    return hota_final(TP, FN, FP, w["AssA"], w["AssRe"], w["AssPr"], np.maximum(1e-10, loc) / np.maximum(1e-10, TP))
+
+
 def mot_ratios(d: dict) -> dict:
     """Adds MOTA, MOTP, Rcll, Prcn, IDR, IDP and IDF1 to a dict of the counts and MOTP_sum."""
     TP, FP, FN, IDSW, IDTP, IDFP, IDFN = (d[k] for k in ("TP", "FP", "FN", "IDSW", "IDTP", "IDFP", "IDFN"))
@@ -442,7 +490,7 @@ def mot_ratios(d: dict) -> dict:
 
 
 class MotEval:
-    """MOTChallenge CLEAR MOT and identity metrics on the GPU.  ``add_sequence`` uploads a sequence's gt once; ``update``
+    """MOTChallenge CLEAR MOT, identity metrics and HOTA on the GPU.  ``add_sequence`` uploads a sequence's gt once; ``update``
     takes the tracked record blocks of a batch of its frames; ``result`` evaluates every sequence.  Every call runs on the
     current CUDA stream, and is ordered after the evaluator's previous call whatever stream that used.
 
@@ -524,20 +572,26 @@ class MotEval:
         """``{"sequences": {name: fields}, "combined": fields, "rounds": {name: CLEAR rounds}, "solved": {name: frame solves
         that needed an assignment}}``; fields: TP, FP, FN, IDSW, Frag, MT, PT, ML, IDTP, IDFP, IDFN, gt_rows, tracker_rows
         (int), MOTP_sum, MOTA, MOTP, Rcll, Prcn, IDR, IDP, IDF1 (float).  Integer fields and MOTP_sum (in sequence order)
-        are summed over the sequences and the ratios recomputed.  ``ValueError`` if an update held invalid input."""
+        are summed over the sequences and the ratios recomputed.  ``"hota"``: ``{"sequences": {name: fields}, "combined":
+        fields}`` with HOTA, DetA, AssA, DetRe, DetPr, AssRe, AssPr, LocA, OWTA (lists of 19 floats, one per alpha 0.05 ..
+        0.95), HOTA_TP, HOTA_FN, HOTA_FP (lists of 19 ints) and HOTA(0), LocA(0), HOTALocA(0), as TrackEval's HOTA gives
+        them (oracle/mot_hota_ref.py).  ``ValueError`` if an update held invalid input."""
         S = len(self._seqs)
         counts = np.zeros((max(S, 1), 12), np.int64)
         motp = np.zeros(max(S, 1))
         rounds = np.zeros(max(S, 1), np.int32)
         solved = np.zeros(max(S, 1), np.int64)
+        hcounts = np.zeros((max(S, 1), 3, HOTA_ALPHAS), np.int64)
+        hsums = np.zeros((max(S, 1), 4, HOTA_ALPHAS))
         status = ctypes.c_uint()
         with torch.cuda.device(self.device):
-            check(lib.k2y_mot_result(self._h, counts.ctypes.data, motp.ctypes.data, rounds.ctypes.data, solved.ctypes.data,
-                                     ctypes.byref(status), self._stream()))
+            check(lib.k2y_mot_result_ex(self._h, counts.ctypes.data, motp.ctypes.data, rounds.ctypes.data, solved.ctypes.data,
+                                        hcounts.ctypes.data, hsums.ctypes.data, ctypes.byref(status), self._stream()))
         if status.value:
             raise ValueError("MotEval: " + "; ".join(m for bit, m in MOT_STATUS.items() if status.value & bit))
-        seqs, out_rounds, out_solved = {}, {}, {}
+        seqs, out_rounds, out_solved, hota = {}, {}, {}, {}
         for name, (i, _, _) in self._seqs.items():
+            hota[name] = hota_sequence(hcounts[i], hsums[i])
             d = {k: int(v) for k, v in zip(MOT_FIELDS, counts[i, :11])}
             d.update(IDFN=d["gt_rows"] - d["IDTP"], IDFP=d["tracker_rows"] - d["IDTP"], MOTP_sum=float(motp[i]))
             seqs[name] = mot_ratios(d)
@@ -547,7 +601,8 @@ class MotEval:
         for d in seqs.values():
             s += d["MOTP_sum"]
         comb["MOTP_sum"] = s
-        return {"sequences": seqs, "combined": mot_ratios(comb), "rounds": out_rounds, "solved": out_solved}
+        return {"sequences": seqs, "combined": mot_ratios(comb), "rounds": out_rounds, "solved": out_solved,
+                "hota": {"sequences": hota, "combined": hota_combine(list(hota.values()))}}
 
     def __del__(self):
         h = getattr(self, "_h", None)

@@ -1,5 +1,6 @@
 #!/usr/bin/env python
-"""Tracking evaluation on the GPU (evaluate.MotEval) against the host (oracle/mot_ref.py and its literal numpy / scipy form)
+"""Tracking evaluation on the GPU (evaluate.MotEval: CLEAR, Identity and HOTA) against the host (oracle/mot_ref.py,
+oracle/mot_hota_ref.py and their literal numpy / scipy forms)
 on seeded synthetic data shaped like MOT17 train: 7 sequences of 600, 1050, 837, 525, 654, 900 and 750 frames, about 21
 pedestrian gt rows per frame plus zero-marked and distractor rows, and tracker records made from the gt with jitter, misses,
 false positives, ghost boxes, id switches and crossing pairs (tests/mot_sequences.py).
@@ -13,8 +14,9 @@ is largest; the host forms are not run there (the literal form's square matrix a
 Prints the GPU evaluation time (create, every update from device blocks and result(), on a host clock around a device
 synchronise, median of --repeat), the CLEAR rounds, the assignments solved over all rounds and the share of frames whose positives are not isolated
 (the frames that need an assignment), the host times of
-mot_ref and of the literal form (the results asserted identical to the GPU's), and the card name, power limit and SM clock
-read in the same run.
+mot_ref and of the literal form, and of the HOTA restatement and its literal form (the results asserted identical to the
+GPU's), the kernel time of the HOTA kernels and of the CLEAR and Identity kernels in a separate torch.profiler run of each
+data set, and the card name, power limit and SM clock read in the same run.
 """
 import argparse
 import json
@@ -58,6 +60,27 @@ def gpu_eval(data, dev_blocks, benchmark="MOT17"):
     return time.perf_counter() - t, res
 
 
+def kernel_shares(data, dev_blocks, benchmark="MOT17"):
+    """One evaluation under torch.profiler: kernel time (ms) of the HOTA kernels, of the other evaluation kernels (CLEAR and
+    Identity) and of all kernels."""
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        gpu_eval(data, dev_blocks, benchmark)
+    hota = other = 0.0
+    per = {}
+    for e in prof.key_averages():
+        t = getattr(e, "device_time_total", None)
+        t = e.cuda_time_total if t is None else t
+        if "hota_" in e.key:
+            hota += t
+            name = e.key[e.key.index("hota_"):].split("(")[0].split("<")[0].split("ENS")[0]
+            per[name] = per.get(name, 0.0) + t / 1e3
+        elif "mot_" in e.key:
+            other += t
+    return {"hota_kernels_ms": hota / 1e3, "clear_identity_kernels_ms": other / 1e3,
+            "hota_by_kernel_ms": dict(sorted(per.items(), key=lambda kv: -kv[1]))}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--repeat", type=int, default=3)
@@ -98,7 +121,19 @@ def main():
         for name in ref:
             assert ref[name] == lit[name] == res["sequences"][name], name
         assert mot_ref.combine(list(ref.values())) == res["combined"]
+        from oracle import mot_hota_ref
+        t = time.perf_counter()
+        href = {name: mot_hota_ref.evaluate_hota(name, gt, rows[name], L) for name, gt, L, _ in data}
+        out["hota_ref_s"] = time.perf_counter() - t
+        t = time.perf_counter()
+        hlit = {name: mot_hota_ref.evaluate_hota_literal(gt, rows[name], L) for name, gt, L, _ in data}
+        out["hota_literal_s"] = time.perf_counter() - t
+        for name in href:
+            assert href[name] == hlit[name] == res["hota"]["sequences"][name], name
+        assert mot_hota_ref.combine_hota(list(href.values())) == res["hota"]["combined"]
         out["identical"] = True
+    out["HOTA"] = float(np.mean(res["hota"]["combined"]["HOTA"]))
+    out["profile"] = kernel_shares(data, dev_blocks)
     gt, frames = sequence(np.random.default_rng(2020), 600, n_ped=1000, n_other=60, ambiguous=0.3, benchmark="MOT20",
                           life=(60, 180))
     blk = blocks(frames, K=320, rng=rng)
@@ -113,7 +148,9 @@ def main():
     out["mot20_shaped"] = {"frames": 600, "gt_rows": int(len(gt)), "max_gt_rows_per_frame": int(np.bincount(gt[:, 0].astype(int)).max()),
                            "tracker_rows": c["tracker_rows"], "gt_ids": len(np.unique(gt[(gt[:, 6] != 0) & (gt[:, 7] == 1), 1])),
                            "tracker_ids": len({t for f in frames for t, _, _ in f}), "gpu_s_median": float(np.median(times)),
-                           "gpu_s_all": times, "rounds": r20["rounds"]["SYN20-00"], "MOTA": c["MOTA"], "IDF1": c["IDF1"]}
+                           "gpu_s_all": times, "rounds": r20["rounds"]["SYN20-00"], "MOTA": c["MOTA"], "IDF1": c["IDF1"],
+                           "HOTA": float(np.mean(r20["hota"]["combined"]["HOTA"])),
+                           "profile": kernel_shares(dense, dense_dev, "MOT20")}
     print(json.dumps(out))
 
 
