@@ -1,9 +1,11 @@
 #!/usr/bin/env python
 """A checkpoint's tracking on MOTChallenge sequences: CLEAR MOT, the identity metrics and HOTA per sequence and combined,
-with the tracking (SORT, DetectionPipeline.enable_tracking) and the matching and counting on the GPU (evaluate.MotEval).
+with the tracking (SORT, or ByteTrack with --tracker bytetrack: DetectionPipeline.enable_tracking) and the matching and counting on the GPU (evaluate.MotEval).
 
     python evaluate_mot.py CKPT SEQ [SEQ ...] --person_class N [--benchmark MOT17 --track_max_age 1 --track_min_hits 3
                                                                 --track_iou 0.3 --results DIR --out mot.json]
+    python evaluate_mot.py CKPT SEQ [SEQ ...] --person_class N --tracker bytetrack --obj_thresh 0.1 [--track_thresh 0.5
+                                      --track_match 0.8 --track_buffer 30 --track_no_fuse_score ...]
     python -m torch.distributed.run --nproc-per-node 8 evaluate_mot.py ...   # one rank per GPU; rank 0 evaluates
 
 SEQ is a MOTChallenge sequence directory (seqinfo.ini, imDir/%06d<imExt>, gt/gt.txt); a directory without seqinfo.ini
@@ -29,7 +31,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 from evaluate_map import load_checked  # noqa: E402
-from serve import ModelArgParser, add_model_args, add_track_args, detect_files, open_pipeline  # noqa: E402
+from serve import ModelArgParser, add_model_args, add_track_args, detect_files, enable_tracking, open_pipeline  # noqa: E402
 from k210_yolo_framework_b200.evaluate import MOT_BENCHMARKS, MotEval, load_mot_gt, read_seqinfo  # noqa: E402
 
 HOTA_COLUMNS = ("HOTA", "DetA", "AssA", "DetRe", "DetPr", "AssRe", "AssPr", "LocA", "OWTA", "HOTA(0)", "LocA(0)",
@@ -90,7 +92,7 @@ def evaluate(args):
     pipe, world, rank = open_pipeline(args, args.max_per_class)
     if not 0 <= args.person_class < args.class_num:
         raise ValueError(f"--person_class {args.person_class} is outside [0, {args.class_num})")
-    pipe.enable_tracking(args.track_max_age, args.track_min_hits, args.track_iou)
+    enable_tracking(pipe, args)
     ev = MotEval(args.benchmark, device=pipe.device_index) if rank == 0 and any(s[2] for s in seqs) else None
     if args.results and rank == 0:
         os.makedirs(args.results, exist_ok=True)

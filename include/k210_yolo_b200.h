@@ -252,6 +252,22 @@ int k2y_track_update(void *state_dev, const k2y_det *dets_dev, const int32_t *co
                      const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num, int max_per_class,
                      int max_age, int min_hits, double iou_thresh, int32_t *ids_out_dev, float *boxes_out_dev, void *stream);
 
+/* ByteTrack tracking (oracle/bytetrack_ref.py states every rule, and this call follows it bit for bit): per class, a Kalman
+ * filter per track, a first association of the tracks with the high-score records (score > track_thresh), a second of the
+ * tracks left with the low-score records (0.1 < score < track_thresh, the score in word 4 of each record), births from the
+ * high-score records left with score >= track_thresh + 0.1, tracks kept lost for track_buffer frames, ids from one counter
+ * per stream.  state_dev (k2y_bytetrack_state_bytes() bytes, zeroed to start a stream), the gathered block, rows_dev,
+ * positions_dev, ids_out_dev and boxes_out_dev are as for k2y_track_update; a record gets an id when its track ends the
+ * frame tracked and activated.  fuse_score nonzero multiplies the IoU by the record's score in the high-score associations.
+ * One launch of one CTA per call, whatever n_frames, asynchronous on `stream`.  K2Y_ERR_INVALID (nothing launched) for
+ * class_num outside 1..1024, track_buffer < 0, track_thresh or match_thresh outside [0, 1], or max_per_class *
+ * (max(track_buffer, 1) + 2) over the 4096 tracks one class holds. */
+int k2y_bytetrack_state_bytes(int class_num, int max_per_class, int track_buffer, size_t *bytes);
+int k2y_bytetrack_update(void *state_dev, const k2y_det *dets_dev, const int32_t *counts_dev, long long row_stride_words,
+                         const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num, int max_per_class,
+                         double track_thresh, double match_thresh, int track_buffer, int fuse_score, int32_t *ids_out_dev,
+                         float *boxes_out_dev, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Multi-GPU collation: images shard across ranks (one process per GPU), and the one exchange on the path
  * is ONE ncclAllGather of the fixed-size record blocks.  The reference is single-process (keras_inference.py:12-17), so

@@ -1,5 +1,6 @@
-"""SORT tracking on the GPU (``k2y_track_update``, csrc/track.cu; oracle/sort_ref.py states the rules): ``Tracker`` owns one
-stream's device state and runs one launch per batch of frames over a gathered record block."""
+"""Tracking on the GPU: SORT (``k2y_track_update``, csrc/track.cu; oracle/sort_ref.py states the rules) and ByteTrack
+(``k2y_bytetrack_update``, csrc/bytetrack.cu; oracle/bytetrack_ref.py).  ``Tracker`` and ``ByteTracker`` each own one stream's
+device state and run one launch per batch of frames over a gathered record block."""
 from __future__ import annotations
 
 import ctypes
@@ -10,6 +11,7 @@ import torch
 from ._lib import check, lib
 
 MAX_TRACKS_PER_CLASS = 1024
+BYTETRACK_MAX_TRACKS_PER_CLASS = 4096
 
 
 def check_setting(K: int, max_age, min_hits, iou_thresh) -> None:
@@ -64,4 +66,47 @@ class Tracker:
         check(lib.k2y_track_update(self.state.data_ptr(), dets.data_ptr(), counts.data_ptr(), dets.stride(0), rows.data_ptr(),
                                    positions.data_ptr(), int(n_frames), self.C, self.K, self.max_age, self.min_hits,
                                    self.iou_thresh, ids_out.data_ptr(), boxes_out.data_ptr(), ctypes.c_void_p(stream.cuda_stream)))
+        self.last_position = int(last_position)
+
+
+def check_bytetrack_setting(K: int, track_thresh, match_thresh, track_buffer) -> None:
+    """Raises ValueError for a ByteTrack setting the tracker does not take: a class holds K (max(track_buffer, 1) + 2)
+    tracks within a frame (oracle/bytetrack_ref.py ``max_tracks``), at most 4096."""
+    if not 0.0 <= float(track_thresh) <= 1.0:
+        raise ValueError(f"track_thresh {track_thresh} is outside [0, 1]")
+    if not 0.0 <= float(match_thresh) <= 1.0:
+        raise ValueError(f"match_thresh {match_thresh} is outside [0, 1]")
+    if isinstance(track_buffer, bool) or int(track_buffer) != track_buffer or track_buffer < 0:
+        raise ValueError(f"track_buffer {track_buffer}: a whole number of frames >= 0")
+    cap = BYTETRACK_MAX_TRACKS_PER_CLASS
+    if K * (max(int(track_buffer), 1) + 2) > cap:
+        raise ValueError(f"max_per_class {K} x (max(track_buffer {track_buffer}, 1) + 2) tracks per class exceed the {cap} the "
+                         f"tracker holds: track_buffer <= {cap // K - 2} at max_per_class {K}")
+
+
+class ByteTracker(Tracker):
+    """``Tracker``'s interface over ByteTrack: one stream's tracks over `C` classes of at most `K` records per frame, the
+    score in word 4 of each record."""
+
+    def __init__(self, C: int, K: int, track_thresh: float = 0.5, match_thresh: float = 0.8, track_buffer: int = 30,
+                 fuse_score: bool = True, device=None):
+        check_bytetrack_setting(K, track_thresh, match_thresh, track_buffer)
+        self.C, self.K = int(C), int(K)
+        self.track_thresh, self.match_thresh = float(track_thresh), float(match_thresh)
+        self.track_buffer, self.fuse_score = int(track_buffer), bool(fuse_score)
+        nbytes = ctypes.c_size_t()
+        check(lib.k2y_bytetrack_state_bytes(self.C, self.K, self.track_buffer, ctypes.byref(nbytes)))
+        dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        self.state = torch.zeros(nbytes.value, dtype=torch.uint8, device=dev)
+        self.last_position: Optional[int] = None
+
+    def update(self, dets: torch.Tensor, counts: torch.Tensor, rows: torch.Tensor, positions: torch.Tensor, n_frames: int,
+               ids_out: torch.Tensor, boxes_out: torch.Tensor, stream: torch.cuda.Stream, last_position: int) -> None:
+        """As ``Tracker.update``."""
+        if dets.stride(0) != counts.stride(0):
+            raise ValueError("dets and counts must share their row stride (a gather block)")
+        check(lib.k2y_bytetrack_update(self.state.data_ptr(), dets.data_ptr(), counts.data_ptr(), dets.stride(0),
+                                       rows.data_ptr(), positions.data_ptr(), int(n_frames), self.C, self.K, self.track_thresh,
+                                       self.match_thresh, self.track_buffer, int(self.fuse_score), ids_out.data_ptr(),
+                                       boxes_out.data_ptr(), ctypes.c_void_p(stream.cuda_stream)))
         self.last_position = int(last_position)

@@ -21,13 +21,26 @@ With --track, also SORT tracking of the same records (DetectionPipeline.enable_t
                  windows (median).
 The GPU's ids and boxes must equal sort_ref's; the run fails otherwise.
 
+With --track bytetrack, also ByteTrack (DetectionPipeline.enable_tracking(method="bytetrack"), default setting) beside the SORT
+arms, on pipelines at obj_thresh 0.1 so that the low-score association has records:
+  gpu_plain /    the GPU route on two fresh pipelines, one tracking with k2y_bytetrack_update and one not, windows alternating;
+  gpu_track:
+  bytetrack_kernel:  the kernel's time per batch of frames, from CUDA events around its launches, on the route's records, on
+                 the "dense_voc" stream of the SORT arms with scores (0.9, or 0.3 for a record with probability 0.15) and at
+                 "coco_bound" (80 classes of 100, track_buffer 30, class 0 given 100 new boxes every second frame, which it
+                 confirms the frame after and then loses, so that its lost tracks pile up to about 1,600);
+  bytetrack_ref: the route's records and the first batch of dense_voc tracked on the host by oracle/bytetrack_ref.py,
+                 frames/s of the tracker alone (one pass run first, median).
+The GPU's ids and boxes on the route's records and on the first batch of dense_voc must equal bytetrack_ref's; the run fails
+otherwise.
+
 The video: the bench_ingest photos resized to 1280x720 with the golden dog photo pasted in (so that there are records to
 compare), written as a Motion-JPEG AVI at 4:2:2, quality 90, without DHT segments, as cameras write them.  Every route runs
 once to warm up and then `--windows` timed passes (median).  All Motion-JPEG routes must give the same records, and the mp4v
 route the records of its own decoded pixels; the run fails otherwise.  The card's name, power limit and SM clock are read in
 the same run.  Prints one JSON line.
 
-    python scripts/bench_video.py [--frames 256 --batch 32 --windows 3 --track]
+    python scripts/bench_video.py [--frames 256 --batch 32 --windows 3 --track [bytetrack]]
 """
 import argparse
 import io
@@ -95,8 +108,8 @@ def run(pipe, n, load, threads, writer_path=None, fps=30.0, tracks=None):
     return recs
 
 
-def new_pipeline(anchors, batch):
-    pipe = DetectionPipeline("yolo_mobilev1", (224, 320), anchors, 20, 0.75, batch, obj_thresh=0.3, iou_thresh=0.5)
+def new_pipeline(anchors, batch, obj_thresh=0.3):
+    pipe = DetectionPipeline("yolo_mobilev1", (224, 320), anchors, 20, 0.75, batch, obj_thresh=obj_thresh, iou_thresh=0.5)
     pipe.engine.set_weights(load_npz_weights(os.path.join(GOLDEN, "yolo_mobilev1_075_voc_weights.npz")))
     return pipe
 
@@ -106,7 +119,8 @@ def main():
     ap.add_argument("--frames", type=int, default=256)
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--windows", type=int, default=3)
-    ap.add_argument("--track", action="store_true", help="also measure SORT tracking on the GPU and on the host")
+    ap.add_argument("--track", nargs="?", const="sort", default=None, choices=["sort", "bytetrack"],
+                    help="also measure SORT tracking on the GPU and on the host; `--track bytetrack` measures ByteTrack too")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_video measures on a GPU"
     import cv2
@@ -165,8 +179,9 @@ def main():
             times["draw"].append(time.perf_counter() - t0)
             recs["draw"] = recs["draw"] if out == recs["draw"] else None
         drawn_frames = open_video(drawn).n_frames
-        make_pipe = lambda: new_pipeline(anchors, args.batch)     # noqa: E731
+        make_pipe = lambda obj_thresh=0.3: new_pipeline(anchors, args.batch, obj_thresh)     # noqa: E731
         track = bench_track(make_pipe, n, gpu_load, recs["gpu"], args.batch, args.windows) if args.track else None
+        byte = bench_bytetrack(make_pipe, n, gpu_load, args.batch, args.windows) if args.track == "bytetrack" else None
         gpu = gpu_info()
     mjpeg = [recs[k] for k in ("gpu", "pil_1", "pil_4", "pil_16", "pixels", "draw")]
     same = all(r is not None and r == mjpeg[0] for r in mjpeg) and recs["ffmpeg_mp4v"] == mp4_ref and drawn_frames == n
@@ -176,22 +191,47 @@ def main():
         "video": f"MJPEG AVI {W720}x{H720} 4:2:2 q90 without DHT", "avi_bytes": avi_bytes, "mp4v_bytes": mp4_bytes,
         "gpu_decoded_frames": int(gpu_frames), "records": int(sum(len(r) for r in mjpeg[0] or [])), "frames_per_s": rate,
         "windows_s": {k: [round(t, 4) for t in v] for k, v in times.items()}, "records_equal": same,
-        **({"track": track} if track else {}), "gpu": gpu}))
+        **({"track": track} if track else {}), **({"bytetrack": byte} if byte else {}), "gpu": gpu}))
     if not same:
         sys.exit("the routes' records differ")
     if track and not track["ids_equal"]:
         sys.exit("the GPU tracker's ids and boxes differ from oracle/sort_ref.py's")
+    if byte and not byte["ids_equal"]:
+        sys.exit("the GPU ByteTrack's ids and boxes differ from oracle/bytetrack_ref.py's")
 
 
-def frame_blocks(recs, C, K):
-    """Each frame's records as (boxes float32 [C, K, 4], counts [C]), in record order per class."""
+def frame_blocks(recs, C, K, scores=False):
+    """Each frame's records as (boxes float32 [C, K, 4], counts [C]), in record order per class; with `scores` also their
+    scores float32 [C, K]."""
     out = []
     for frame in recs:
-        boxes, counts = np.zeros((C, K, 4), np.float32), np.zeros(C, np.int32)
-        for c, _, _, t, l, b, r in frame:
+        boxes, counts, sc = np.zeros((C, K, 4), np.float32), np.zeros(C, np.int32), np.zeros((C, K), np.float32)
+        for c, _, s, t, l, b, r in frame:
             boxes[c, counts[c]] = (t, l, b, r)
+            sc[c, counts[c]] = s
             counts[c] += 1
-        out.append((boxes, counts))
+        out.append((boxes, counts, sc) if scores else (boxes, counts))
+    return out
+
+
+def with_scores(blocks, seed=1):
+    """The blocks with a score for each record: 0.9, or 0.3 (an occluded object, ByteTrack's low band) with probability 0.15."""
+    rng = np.random.default_rng(seed)
+    return [(b, c, np.where(rng.random(b.shape[:2]) < 0.15, 0.3, 0.9).astype(np.float32)) for b, c in blocks]
+
+
+def bytetrack_bound_blocks(C, K, n):
+    """Class 0 piles up lost tracks: K new 10 x 10 high-score boxes every second frame, repeated in the frame after (which
+    confirms them) and then left, so that each pair of frames adds K lost tracks until track_buffer removes them."""
+    out = []
+    for f in range(n):
+        boxes, counts, sc = np.zeros((C, K, 4), np.float32), np.zeros(C, np.int32), np.zeros((C, K), np.float32)
+        for i in range(K):
+            y, x = 40.0 * i, 100.0 + 40.0 * (f // 2)
+            boxes[0, i] = (y, x, y + 10, x + 10)
+        counts[0] = K
+        sc[0, :K] = 0.9
+        out.append((boxes, counts, sc))
     return out
 
 
@@ -225,24 +265,27 @@ def bound_blocks(C, K, n):
     return out
 
 
-def time_kernel(blocks, C, K, max_age, batch, windows, dev):
-    """(median, max) ms per launch of k2y_track_update over the frames in batches of `batch`, from CUDA events; the frames'
-    records staged on the device as gather blocks first, one untimed pass to warm up."""
+def time_kernel(blocks, C, K, max_age, batch, windows, dev, make_tracker=None, first=None):
+    """(median, max) ms per launch of k2y_track_update (or of the tracker `make_tracker` makes) over the frames in batches
+    of `batch`, from CUDA events; the frames' records (and scores, with a third item) staged on the device as gather blocks
+    first, one untimed pass to warm up.  With `first` (a list) the first batch's (ids, boxes) of the last pass go there."""
     from k210_yolo_framework_b200.dist import DetectionGather
     from k210_yolo_framework_b200.track import Tracker
     staged = []
     for a in range(0, len(blocks), batch):
         buf = torch.zeros((batch, C * (K * 6 + 1)), dtype=torch.int32)
         d, c = DetectionGather.split(buf, C, K)
-        for i, (b, cnt) in enumerate(blocks[a:a + batch]):
-            d[i, :, :, :4] = torch.from_numpy(b.view(np.int32))
-            c[i] = torch.from_numpy(cnt)
+        for i, blk in enumerate(blocks[a:a + batch]):
+            d[i, :, :, :4] = torch.from_numpy(blk[0].view(np.int32))
+            if len(blk) > 2:
+                d[i, :, :, 4] = torch.from_numpy(blk[2].view(np.int32))
+            c[i] = torch.from_numpy(blk[1])
         m = len(blocks[a:a + batch])
         staged.append((DetectionGather.split(buf.to(dev), C, K), m, torch.arange(a, a + m, dtype=torch.int64, device=dev), a + m - 1))
     rows = torch.arange(batch, dtype=torch.int32, device=dev)
     ids_d = torch.empty((batch, C, K), dtype=torch.int32, device=dev)
     boxes_d = torch.empty((batch, C, K, 4), dtype=torch.float32, device=dev)
-    tracker = Tracker(C, K, max_age=max_age, device=dev.index)
+    tracker = make_tracker() if make_tracker else Tracker(C, K, max_age=max_age, device=dev.index)
     st = torch.cuda.current_stream()
     per_batch = []
     for w in range(windows + 1):
@@ -252,6 +295,8 @@ def time_kernel(blocks, C, K, max_age, batch, windows, dev):
             ev[2 * i].record(st)
             tracker.update(d, c, rows, pos, m, ids_d, boxes_d, st, last)
             ev[2 * i + 1].record(st)
+            if i == 0 and w == windows and first is not None:
+                first += [ids_d[:m].cpu().numpy(), boxes_d[:m].cpu().numpy()]
         torch.cuda.synchronize()
         if w:
             per_batch += [ev[2 * i].elapsed_time(ev[2 * i + 1]) for i in range(len(staged))]
@@ -311,6 +356,66 @@ def bench_track(make_pipe, n, load, recs, batch, windows):
             "host_frames_per_s": {k: round(n / statistics.median(v), 1) for k, v in host.items()},
             "host_windows_s": {k: [round(t, 4) for t in v] for k, v in host.items()},
             "reported_records": int((ids >= 0).sum()), "tracks": int(ids.max(initial=0)), "ids_equal": equal}
+
+
+def _same(ids, boxes, ref_ids, ref_boxes):
+    nan = np.isnan(ref_boxes)
+    return bool(np.array_equal(ids, ref_ids) and np.array_equal(np.isnan(boxes), nan) and
+                np.array_equal(np.where(nan, 0, boxes).view(np.int32), np.where(nan, 0, ref_boxes).view(np.int32)))
+
+
+def bench_bytetrack(make_pipe, n, load, batch, windows):
+    """The --track bytetrack arms (see the module docstring)."""
+    from k210_yolo_framework_b200.track import ByteTracker
+    from oracle import bytetrack_ref
+    plain, tracked = make_pipe(0.1), make_pipe(0.1)
+    C, K = plain.gather.C, plain.gather.K
+    recs = run(plain, n, load, 4)                                   # warm-up of both
+    tracked.enable_tracking(method="bytetrack")
+    got = []
+    assert run(tracked, n, load, 4, tracks=got) == recs             # tracking leaves the records as they were
+    times = {"gpu_plain": [], "gpu_track": []}
+    for w in range(windows):
+        arms = ["gpu_plain", "gpu_track"] if w % 2 == 0 else ["gpu_track", "gpu_plain"]
+        for arm in arms:
+            if arm == "gpu_track":
+                tracked.reset_tracks()
+                got = []
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out = run(tracked, n, load, 4, tracks=got) if arm == "gpu_track" else run(plain, n, load, 4)
+            torch.cuda.synchronize()
+            times[arm].append(time.perf_counter() - t0)
+            assert out == recs
+    ids = torch.cat([g[0] for g in got]).numpy()
+    boxes = torch.cat([g[1] for g in got]).numpy()
+    blocks = frame_blocks(recs, C, K, scores=True)
+    dense = with_scores(dense_voc_blocks(C, K, n))
+    host, ref = {}, {}
+    for stream, frames in (("route", blocks), ("dense_voc_first_batch", dense[:batch])):
+        host[stream] = []
+        for w in range(windows + 1):            # the first pass warms up
+            tracker = bytetrack_ref.ByteTrack(C, K)
+            t0 = time.perf_counter()
+            out = [tracker.update(p, *f) for p, f in enumerate(frames)]
+            if w:
+                host[stream].append(time.perf_counter() - t0)
+        ref[stream] = np.stack([o[0] for o in out]), np.stack([o[1] for o in out])
+    dev = torch.device("cuda", plain.device_index)
+    first = []
+    kernel = {"route": time_kernel(blocks, C, K, 0, batch, windows, dev, lambda: ByteTracker(C, K, device=dev.index)),
+              "dense_voc": time_kernel(dense, C, K, 0, batch, windows, dev, lambda: ByteTracker(C, K, device=dev.index), first),
+              "coco_bound": time_kernel(bytetrack_bound_blocks(80, 100, n), 80, 100, 0, batch, windows, dev,
+                                        lambda: ByteTracker(80, 100, device=dev.index))}
+    equal = {"route": _same(ids, boxes, *ref["route"]), "dense_voc_first_batch": _same(*first, *ref["dense_voc_first_batch"])}
+    return {"obj_thresh": 0.1, "records": int(sum(len(r) for r in recs)),
+            "frames_per_s": {k: round(n / statistics.median(v), 1) for k, v in times.items()},
+            "windows_s": {k: [round(t, 4) for t in v] for k, v in times.items()},
+            "bytetrack_kernel_ms_per_batch_median_max": kernel,
+            "bytetrack_ref_frames_per_s": {k: round(len(blocks if k == "route" else dense[:batch]) / statistics.median(v), 1)
+                                           for k, v in host.items()},
+            "reported_records": int((ids >= 0).sum()), "tracks": int(ids.max(initial=0)), "ids_equal_by_stream": equal,
+            "ids_equal": all(equal.values())}
 
 
 if __name__ == "__main__":

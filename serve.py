@@ -41,7 +41,9 @@ OpenCV's FFmpeg backend on the decode threads of every rank, each rank keeping i
 DIR/<stem>.avi, a Motion-JPEG AVI of the drawn frames at the source frame rate, on rank 0.
 
 With --track (a video only) the objects are tracked across the frames on the GPU, SORT-style (DetectionPipeline.enable_tracking,
---track_max_age, --track_min_hits, --track_iou): every detection of a line gains "track", its track id or null, and
+--track_max_age, --track_min_hits, --track_iou), or with --tracker bytetrack by ByteTrack (--track_thresh, --track_match,
+--track_buffer, --track_no_fuse_score; its low-score association sees only the records above --obj_thresh, so it wants
+--obj_thresh 0.1): every detection of a line gains "track", its track id or null, and
 "track_box_tlbr", the track's box, when it has an id.  Dropped frames count as frames without detections.
 """
 import argparse
@@ -245,7 +247,7 @@ def serve_video(args, out_fh=None):
         pipe.enable_rendering(quality=args.draw_quality)
     track = getattr(args, "track", False)
     if track:
-        pipe.enable_tracking(args.track_max_age, args.track_min_hits, args.track_iou)
+        enable_tracking(pipe, args)
     B, G = pipe.images_per_batch, pipe.world * pipe.images_per_batch
     gpu_png, gpu_progressive = getattr(args, "gpu_png", False), getattr(args, "gpu_progressive", False)
     load = src.loader(keep=lambda k: (k % G) // B == rank, route=lambda data: route_image(data, gpu_png, gpu_progressive))
@@ -320,7 +322,8 @@ def add_model_args(ap):
 
 class ModelArgParser(argparse.ArgumentParser):
     """An ArgumentParser that also refuses the add_model_args flags that need one another alone: --tile_size without
-    --tile_images, and --tile_images without --tile_size."""
+    --tile_images, and --tile_images without --tile_size; and, with add_track_args, the flags of the tracker --tracker does
+    not select."""
 
     def parse_known_args(self, args=None, namespace=None):
         ns, rest = super().parse_known_args(args, namespace)
@@ -329,6 +332,8 @@ class ModelArgParser(argparse.ArgumentParser):
             self.error("--tile_size needs --tile_images N: the images one batch holds")
         if n is not None and size is None:
             self.error("--tile_images goes with --tile_size")
+        if hasattr(ns, "tracker") and track_args_error(ns):
+            self.error(track_args_error(ns))
         return ns, rest
 
 
@@ -362,16 +367,47 @@ def build_parser():
                          "rendered and JPEG-encoded on the GPU; for a video, its drawn frames as the Motion-JPEG AVI DIR/<stem>.avi")
     ap.add_argument("--draw_quality", type=quality_arg, default=75, help="JPEG quality of the --draw files (1..100)")
     ap.add_argument("--track", action="store_true",
-                    help="track objects across a video's frames on the GPU (SORT): each detection gains its track id and box")
+                    help="track objects across a video's frames on the GPU (SORT, or --tracker bytetrack): each detection gains "
+                         "its track id and box")
     add_track_args(ap, " (--track)")
     return ap
 
 
 def add_track_args(ap, note=""):
-    """The SORT setting flags serve.py and evaluate_mot.py share (DetectionPipeline.enable_tracking)."""
-    ap.add_argument("--track_max_age", type=int, default=1, help="frames a track may miss before it is removed" + note)
-    ap.add_argument("--track_min_hits", type=int, default=3, help="matched frames in a row before a track is reported" + note)
-    ap.add_argument("--track_iou", type=float, default=0.3, help="least IoU of a detection with its track's prediction" + note)
+    """The tracker flags serve.py and evaluate_mot.py share (DetectionPipeline.enable_tracking)."""
+    ap.add_argument("--tracker", choices=["sort", "bytetrack"], default="sort",
+                    help="SORT, or ByteTrack, which also associates the tracks left with the low-score records; it sees only "
+                         "the records above --obj_thresh, so its second association needs --obj_thresh 0.1" + note)
+    ap.add_argument("--track_max_age", type=int, default=1, help="frames a track may miss before it is removed (SORT)" + note)
+    ap.add_argument("--track_min_hits", type=int, default=3, help="matched frames in a row before a track is reported (SORT)" + note)
+    ap.add_argument("--track_iou", type=float, default=0.3, help="least IoU of a detection with its track's prediction (SORT)" + note)
+    ap.add_argument("--track_thresh", type=float, default=0.5,
+                    help="score above which a record is high (ByteTrack; low records score in (0.1, track_thresh))" + note)
+    ap.add_argument("--track_match", type=float, default=0.8, help="largest cost of the first association (ByteTrack)" + note)
+    ap.add_argument("--track_buffer", type=int, default=30, help="frames a lost track is kept (ByteTrack)" + note)
+    ap.add_argument("--track_no_fuse_score", action="store_true",
+                    help="associate by IoU alone, not IoU times score (ByteTrack; its --mot20)" + note)
+
+
+SORT_FLAGS = {"track_max_age": 1, "track_min_hits": 3, "track_iou": 0.3}
+BYTETRACK_FLAGS = {"track_thresh": 0.5, "track_match": 0.8, "track_buffer": 30, "track_no_fuse_score": False}
+
+
+def track_args_error(ns):
+    """The message for add_track_args flags of the tracker --tracker does not select, set away from their defaults; None when
+    there are none."""
+    other = BYTETRACK_FLAGS if ns.tracker == "sort" else SORT_FLAGS
+    wrong = [f"--{k}" for k, v in other.items() if getattr(ns, k) != v]
+    if wrong:
+        return f"{', '.join(wrong)} set the other tracker than --tracker {ns.tracker}"
+    return None
+
+
+def enable_tracking(pipe, args):
+    """DetectionPipeline.enable_tracking with the add_track_args flags."""
+    pipe.enable_tracking(args.track_max_age, args.track_min_hits, args.track_iou, method=args.tracker,
+                         track_thresh=args.track_thresh, match_thresh=args.track_match, track_buffer=args.track_buffer,
+                         fuse_score=not args.track_no_fuse_score)
 
 
 def main():
