@@ -1,11 +1,14 @@
 #!/usr/bin/env python
 """A checkpoint's tracking on MOTChallenge sequences: CLEAR MOT, the identity metrics and HOTA per sequence and combined,
-with the tracking (SORT, or ByteTrack with --tracker bytetrack: DetectionPipeline.enable_tracking) and the matching and counting on the GPU (evaluate.MotEval).
+with the tracking (SORT, ByteTrack with --tracker bytetrack or OC-SORT with --tracker ocsort: DetectionPipeline.enable_tracking) and the matching and counting on the GPU (evaluate.MotEval).
 
     python evaluate_mot.py CKPT SEQ [SEQ ...] --person_class N [--benchmark MOT17 --track_max_age 1 --track_min_hits 3
                                                                 --track_iou 0.3 --results DIR --out mot.json]
     python evaluate_mot.py CKPT SEQ [SEQ ...] --person_class N --tracker bytetrack --obj_thresh 0.1 [--track_thresh 0.5
                                       --track_match 0.8 --track_buffer 30 --track_no_fuse_score ...]
+    python evaluate_mot.py CKPT SEQ [SEQ ...] --person_class N --tracker ocsort [--track_max_age 30 --track_min_hits 3
+                                      --track_iou 0.3 --track_det_thresh 0.6 --track_delta_t 3 --track_inertia 0.2
+                                      --track_use_byte --obj_thresh 0.1 ...]
     python -m torch.distributed.run --nproc-per-node 8 evaluate_mot.py ...   # one rank per GPU; rank 0 evaluates
 
 SEQ is a MOTChallenge sequence directory (seqinfo.ini, imDir/%06d<imExt>, gt/gt.txt); a directory without seqinfo.ini

@@ -268,6 +268,24 @@ int k2y_bytetrack_update(void *state_dev, const k2y_det *dets_dev, const int32_t
                          double track_thresh, double match_thresh, int track_buffer, int fuse_score, int32_t *ids_out_dev,
                          float *boxes_out_dev, void *stream);
 
+/* OC-SORT tracking (oracle/ocsort_ref.py states every rule, and this call follows it bit for bit): per class, SORT's Kalman
+ * filter per track with OC-SORT's re-update along a virtual path when a lost track is found again (ORU), a first association
+ * of the tracks with the records scored above det_thresh by IoU plus the direction term weighted by inertia (OCM, over the
+ * observation delta_t frames back), with use_byte a second of the tracks left with the records scored in (0.1, det_thresh),
+ * a third of the records and tracks left by the tracks' last observations (OCR), births from the high-score records left,
+ * tracks removed after max_age frames unmatched and reported after min_hits matched frames in a row (or in the stream's
+ * first min_hits frames), ids from one counter per stream.  state_dev (k2y_ocsort_state_bytes() bytes, zeroed to start a
+ * stream), the gathered block (score in word 4 of each record), rows_dev, positions_dev, ids_out_dev and boxes_out_dev are as
+ * for k2y_track_update; a record's box is its own when its track reports it.  One launch of one CTA per call, whatever
+ * n_frames, asynchronous on `stream`.  K2Y_ERR_INVALID (nothing launched) for class_num outside 1..1024, max_age or min_hits
+ * < 0, delta_t outside 1..8, det_thresh, iou_thresh or inertia outside [0, 1], or max_per_class * (max_age + 1) over the
+ * 4096 tracks one class holds. */
+int k2y_ocsort_state_bytes(int class_num, int max_per_class, int max_age, int delta_t, size_t *bytes);
+int k2y_ocsort_update(void *state_dev, const k2y_det *dets_dev, const int32_t *counts_dev, long long row_stride_words,
+                      const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num, int max_per_class,
+                      double det_thresh, int max_age, int min_hits, double iou_thresh, int delta_t, double inertia, int use_byte,
+                      int32_t *ids_out_dev, float *boxes_out_dev, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Multi-GPU collation: images shard across ranks (one process per GPU), and the one exchange on the path
  * is ONE ncclAllGather of the fixed-size record blocks.  The reference is single-process (keras_inference.py:12-17), so

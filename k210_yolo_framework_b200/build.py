@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libk210yolo_b200.so")
-SOURCES = ["conv_simt.cu", "gemm_tc.cu", "detect.cu", "net.cu", "region_layer_abi.cu", "preprocess.cu", "jpeg.cu", "jpeg_progressive.cu", "png.cu", "jpeg_encode.cu", "render.cu", "evaluate.cu", "evaluate_mot.cu", "track.cu", "bytetrack.cu", "comm.cu"]
+SOURCES = ["conv_simt.cu", "gemm_tc.cu", "detect.cu", "net.cu", "region_layer_abi.cu", "preprocess.cu", "jpeg.cu", "jpeg_progressive.cu", "png.cu", "jpeg_encode.cu", "render.cu", "evaluate.cu", "evaluate_mot.cu", "track.cu", "bytetrack.cu", "ocsort.cu", "comm.cu"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a",
               "-Xcompiler", "-fPIC", "-shared"]
 

@@ -18,6 +18,7 @@
 
 #include "common.h"
 #include "lsap_warp.cuh"
+#include "warp_util.cuh"
 
 namespace k2y {
 namespace {
@@ -26,7 +27,6 @@ constexpr int BT_MAX = 4096;                       // tracks per class (track.py
 constexpr double W_P = 1.0 / 20, W_V = 1.0 / 160;
 constexpr double LOW_THRESH = 0.1, SECOND_THRESH = 0.5, UNCONFIRMED_THRESH = 0.7, DUPLICATE_THRESH = 0.15;
 constexpr int TRACKED = 1, LOST = 2, REMOVED = 3;
-constexpr unsigned FULL = 0xffffffffu;
 constexpr int BT_WARPS = 8, BT_THREADS = BT_WARPS * 32;    // 148 registers a thread, no spills (at 16 warps, 128 spill)
 
 struct BTrk {
@@ -49,12 +49,6 @@ struct BtLayout {
     size_t lists, trk, born, high, low, pool, unc, rest, match, nlist, drop, left, hm, pbox, ubox, nbox, u, v, spc, path,
         col4row, row4col, remaining, sr, sc, total;
 };
-
-__host__ __device__ inline size_t take(size_t &o, size_t bytes) {
-    size_t at = o;
-    o = (o + bytes + 255) & ~(size_t)255;
-    return at;
-}
 
 __host__ __device__ inline int bt_cap(int K, int B) { return K * ((B > 1 ? B : 1) + 2); }
 
@@ -93,7 +87,6 @@ __host__ __device__ inline BtLayout bt_layout(int C, int K, int cap) {
     return L;
 }
 
-__device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
 // Cython's min / max: the second operand when it compares below / above the first
 __device__ __forceinline__ double cmin(double a, double b) { return b < a ? b : a; }
 __device__ __forceinline__ double cmax(double a, double b) { return b > a ? b : a; }
@@ -197,22 +190,6 @@ __device__ int load_det(const int32_t *rec, int k, double track_thresh, BDet &d)
     d.score = s;
     d.k = k;
     return kind;
-}
-
-// Calls emit(i, at) for the i in [0, n) with keep(i), at counting them in order from 0; returns their count.  Warp-wide.
-template <class Keep, class Emit>
-__device__ int compact(int n, const Keep &keep, const Emit &emit) {
-    const int lane = threadIdx.x & 31;
-    int base = 0;
-    for (int i0 = 0; i0 < n; i0 += 32) {
-        const int i = i0 + lane;
-        const bool k = i < n && keep(i);
-        const unsigned b = __ballot_sync(FULL, k);
-        if (k) emit(i, base + __popc(b & ((1u << lane) - 1u)));
-        base += __popc(b);
-    }
-    __syncwarp();
-    return base;
 }
 
 // oracle/bytetrack_ref.py ``assign``: match[i] = the column of row i whose cost is < thresh in the assignment of

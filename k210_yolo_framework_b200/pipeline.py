@@ -37,9 +37,10 @@ smaller box, fold the matched boxes into the kept one and drop records at the ti
 with): the letterbox fetches the mirrored columns, and ``k2y_merge_views_mirror`` maps the mirrored views' records back into
 the image while it loads them, then merges all views as above.  It combines with either grid, in either order.
 
-``enable_tracking`` tracks objects across the frames of a stream, SORT-style (``track.Tracker``, oracle/sort_ref.py) or with
-ByteTrack (``track.ByteTracker``, oracle/bytetrack_ref.py): ``submit_images(frames=...)`` gives each image's position in the
-stream, one ``k2y_track_update`` (``k2y_bytetrack_update``) launch per batch runs behind the
+``enable_tracking`` tracks objects across the frames of a stream, SORT-style (``track.Tracker``, oracle/sort_ref.py), with
+ByteTrack (``track.ByteTracker``, oracle/bytetrack_ref.py) or with OC-SORT (``track.OcSortTracker``, oracle/ocsort_ref.py):
+``submit_images(frames=...)`` gives each image's position in the stream, one ``k2y_track_update`` (``k2y_bytetrack_update``,
+``k2y_ocsort_update``) launch per batch runs behind the
 NMS / all-gather on the stream that holds the gathered block, before its D2H, and ``tracks(ticket)`` returns each record's track
 id and box.  The records are unchanged.
 
@@ -241,13 +242,15 @@ class DetectionPipeline:
             self._view_counts = torch.zeros((self.batch, self.gather.C), dtype=torch.int32, device=dev)
             self._slot_yx = [torch.zeros((self.batch, 2), dtype=torch.float32, device=dev) for _ in range(SLOTS)]
 
-    def enable_tracking(self, max_age: int = 1, min_hits: int = 3, iou_thresh: float = 0.3, *, method: str = "sort",
-                        track_thresh: float = 0.5, match_thresh: float = 0.8, track_buffer: int = 30,
-                        fuse_score: bool = True) -> None:
+    def enable_tracking(self, max_age: Optional[int] = None, min_hits: Optional[int] = None, iou_thresh: Optional[float] = None, *,
+                        method: str = "sort", track_thresh: float = 0.5, match_thresh: float = 0.8, track_buffer: int = 30,
+                        fuse_score: bool = True, det_thresh: float = 0.6, delta_t: int = 3, inertia: float = 0.2,
+                        use_byte: bool = False) -> None:
         """From now on ``submit_images`` takes `frames`, each image's position in a stream of frames, and tracks the objects of
         the stream as SORT does (oracle/sort_ref.py states every rule): per class, a Kalman filter per track, IoU association
         by optimal assignment, a track born for each unmatched detection and removed once it missed more than `max_age`
-        frames, and reported once it was matched in `min_hits` frames in a row (or in the stream's first `min_hits` frames).
+        frames (1 when left out), and reported once it was matched in `min_hits` frames in a row (3; or in the stream's first
+        `min_hits` frames), matching at IoU `iou_thresh` (0.3).
         ``tracks(ticket)`` returns each record's id and track box.  A new call starts a new stream, as ``reset_tracks`` does.
         Raises ``ValueError``, leaving the pipeline as it was, for a bad setting or when max_per_class * (max_age + 1)
         exceeds the 1024 tracks one class holds (max_age <= 33 at max_per_class 30, <= 9 at 100).
@@ -258,22 +261,45 @@ class DetectionPipeline:
         and lost tracks kept `track_buffer` frames.  It only sees the records the detector keeps, so its second association
         needs an obj_thresh below track_thresh (0.1 as ByteTrack).  Each method refuses the other's arguments away from their
         defaults, and ByteTrack a setting where max_per_class * (max(track_buffer, 1) + 2) exceeds the 4096 tracks one
-        class holds."""
-        from .track import ByteTracker, Tracker
-        sort_args = (max_age, min_hits, iou_thresh) != (1, 3, 0.3)
+        class holds.
+
+        ``method="ocsort"`` tracks with OC-SORT (oracle/ocsort_ref.py states every rule): SORT's filter, re-updated along a
+        virtual path when a lost track is found again; a first association of the records scored above `det_thresh` by IoU
+        plus `inertia` times the agreement of directions over `delta_t` frames; with `use_byte` a second of the tracks left
+        with the records scored in (0.1, det_thresh) (it needs an obj_thresh below det_thresh); a third by the tracks' last
+        observations.  It takes `max_age`, `min_hits` and `iou_thresh` too, with OC-SORT's defaults when left out (30, 3,
+        0.3), refuses ByteTrack's arguments (and SORT and ByteTrack refuse its own away from their defaults), and refuses a
+        setting where max_per_class * (max_age + 1) exceeds the 4096 tracks one class holds or delta_t is outside 1..8.  Its
+        track box is the record's own box."""
+        from .track import ByteTracker, OcSortTracker, Tracker
+        sort_setting = (1 if max_age is None else max_age, 3 if min_hits is None else min_hits,
+                        0.3 if iou_thresh is None else iou_thresh)
+        sort_args = sort_setting != (1, 3, 0.3)
         byte_args = (track_thresh, match_thresh, track_buffer, fuse_score) != (0.5, 0.8, 30, True)
+        oc_args = (det_thresh, delta_t, inertia, use_byte) != (0.6, 3, 0.2, False)
         if method == "sort":
             if byte_args:
                 raise ValueError("track_thresh, match_thresh, track_buffer and fuse_score set ByteTrack: use method='bytetrack'")
-            tracker = Tracker(self.gather.C, self.gather.K, max_age, min_hits, iou_thresh, self.device_index)
+            if oc_args:
+                raise ValueError("det_thresh, delta_t, inertia and use_byte set OC-SORT: use method='ocsort'")
+            tracker = Tracker(self.gather.C, self.gather.K, *sort_setting, self.device_index)
         elif method == "bytetrack":
             if sort_args:
                 raise ValueError("max_age, min_hits and iou_thresh set SORT: ByteTrack takes track_thresh, match_thresh, "
                                  "track_buffer and fuse_score")
+            if oc_args:
+                raise ValueError("det_thresh, delta_t, inertia and use_byte set OC-SORT: use method='ocsort'")
             tracker = ByteTracker(self.gather.C, self.gather.K, track_thresh, match_thresh, track_buffer, fuse_score,
                                   self.device_index)
+        elif method == "ocsort":
+            if byte_args:
+                raise ValueError("track_thresh, match_thresh, track_buffer and fuse_score set ByteTrack: OC-SORT takes max_age, "
+                                 "min_hits, iou_thresh, det_thresh, delta_t, inertia and use_byte")
+            tracker = OcSortTracker(self.gather.C, self.gather.K, det_thresh, 30 if max_age is None else max_age,
+                                    3 if min_hits is None else min_hits, 0.3 if iou_thresh is None else iou_thresh, delta_t,
+                                    inertia, use_byte, self.device_index)
         else:
-            raise ValueError(f"tracking method {method!r}: 'sort' or 'bytetrack'")
+            raise ValueError(f"tracking method {method!r}: 'sort', 'bytetrack' or 'ocsort'")
         dev = torch.device("cuda", self.device_index)
         n, C, K = self.world * self.batch, self.gather.C, self.gather.K
         self._track = dict(
@@ -306,7 +332,7 @@ class DetectionPipeline:
 
     def _track_slot(self, s: int, st: torch.cuda.Stream, frames: list) -> None:
         """Enqueues the tracking of gather slot s's frames on `st`, behind its gathered block: rows and positions H2D, one
-        launch of the tracker's kernel (k2y_track_update or k2y_bytetrack_update), ids and boxes D2H."""
+        launch of the tracker's kernel (k2y_track_update, k2y_bytetrack_update or k2y_ocsort_update), ids and boxes D2H."""
         tk, m, B = self._track, len(frames), self._ipb
         self._track_n[s] = m
         if m == 0:

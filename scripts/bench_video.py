@@ -34,13 +34,19 @@ arms, on pipelines at obj_thresh 0.1 so that the low-score association has recor
 The GPU's ids and boxes on the route's records and on the first batch of dense_voc must equal bytetrack_ref's; the run fails
 otherwise.
 
+With --track ocsort, the same arms for OC-SORT (DetectionPipeline.enable_tracking(method="ocsort"), default setting) on
+pipelines at the default obj_thresh 0.3: gpu_plain / gpu_track, ocsort_kernel (k2y_ocsort_update on the route's records, on the
+scored dense_voc stream and at "coco_bound", 80 classes of 100 with max_age 39, class 0 given 100 new boxes in every frame so
+that it holds its bound of 4,000 tracks) and ocsort_ref (oracle/ocsort_ref.py on the host).  The GPU's ids and boxes on the
+route's records and on the first batch of dense_voc must equal ocsort_ref's; the run fails otherwise.
+
 The video: the bench_ingest photos resized to 1280x720 with the golden dog photo pasted in (so that there are records to
 compare), written as a Motion-JPEG AVI at 4:2:2, quality 90, without DHT segments, as cameras write them.  Every route runs
 once to warm up and then `--windows` timed passes (median).  All Motion-JPEG routes must give the same records, and the mp4v
 route the records of its own decoded pixels; the run fails otherwise.  The card's name, power limit and SM clock are read in
 the same run.  Prints one JSON line.
 
-    python scripts/bench_video.py [--frames 256 --batch 32 --windows 3 --track [bytetrack]]
+    python scripts/bench_video.py [--frames 256 --batch 32 --windows 3 --track [bytetrack | ocsort]]
 """
 import argparse
 import io
@@ -114,13 +120,17 @@ def new_pipeline(anchors, batch, obj_thresh=0.3):
     return pipe
 
 
+SCORED = {"bytetrack": "ByteTrack", "ocsort": "OC-SORT"}     # the --track arms beside SORT's
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--frames", type=int, default=256)
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--windows", type=int, default=3)
-    ap.add_argument("--track", nargs="?", const="sort", default=None, choices=["sort", "bytetrack"],
-                    help="also measure SORT tracking on the GPU and on the host; `--track bytetrack` measures ByteTrack too")
+    ap.add_argument("--track", nargs="?", const="sort", default=None, choices=["sort", "bytetrack", "ocsort"],
+                    help="also measure SORT tracking on the GPU and on the host; `--track bytetrack` measures ByteTrack too, "
+                         "`--track ocsort` OC-SORT")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_video measures on a GPU"
     import cv2
@@ -181,7 +191,7 @@ def main():
         drawn_frames = open_video(drawn).n_frames
         make_pipe = lambda obj_thresh=0.3: new_pipeline(anchors, args.batch, obj_thresh)     # noqa: E731
         track = bench_track(make_pipe, n, gpu_load, recs["gpu"], args.batch, args.windows) if args.track else None
-        byte = bench_bytetrack(make_pipe, n, gpu_load, args.batch, args.windows) if args.track == "bytetrack" else None
+        scored = bench_scored(make_pipe, n, gpu_load, args.batch, args.windows, args.track) if args.track in SCORED else None
         gpu = gpu_info()
     mjpeg = [recs[k] for k in ("gpu", "pil_1", "pil_4", "pil_16", "pixels", "draw")]
     same = all(r is not None and r == mjpeg[0] for r in mjpeg) and recs["ffmpeg_mp4v"] == mp4_ref and drawn_frames == n
@@ -191,13 +201,13 @@ def main():
         "video": f"MJPEG AVI {W720}x{H720} 4:2:2 q90 without DHT", "avi_bytes": avi_bytes, "mp4v_bytes": mp4_bytes,
         "gpu_decoded_frames": int(gpu_frames), "records": int(sum(len(r) for r in mjpeg[0] or [])), "frames_per_s": rate,
         "windows_s": {k: [round(t, 4) for t in v] for k, v in times.items()}, "records_equal": same,
-        **({"track": track} if track else {}), **({"bytetrack": byte} if byte else {}), "gpu": gpu}))
+        **({"track": track} if track else {}), **({args.track: scored} if scored else {}), "gpu": gpu}))
     if not same:
         sys.exit("the routes' records differ")
     if track and not track["ids_equal"]:
         sys.exit("the GPU tracker's ids and boxes differ from oracle/sort_ref.py's")
-    if byte and not byte["ids_equal"]:
-        sys.exit("the GPU ByteTrack's ids and boxes differ from oracle/bytetrack_ref.py's")
+    if scored and not scored["ids_equal"]:
+        sys.exit(f"the GPU {SCORED[args.track]}'s ids and boxes differ from oracle/{args.track}_ref.py's")
 
 
 def frame_blocks(recs, C, K, scores=False):
@@ -364,14 +374,31 @@ def _same(ids, boxes, ref_ids, ref_boxes):
                 np.array_equal(np.where(nan, 0, boxes).view(np.int32), np.where(nan, 0, ref_boxes).view(np.int32)))
 
 
-def bench_bytetrack(make_pipe, n, load, batch, windows):
-    """The --track bytetrack arms (see the module docstring)."""
-    from k210_yolo_framework_b200.track import ByteTracker
-    from oracle import bytetrack_ref
-    plain, tracked = make_pipe(0.1), make_pipe(0.1)
+def ocsort_bound_blocks(C, K, n):
+    """``bound_blocks`` with a high score (0.9) on every record: class 0 is given K new boxes in every frame that overlap
+    nothing, so that it holds K (max_age + 1) tracks."""
+    return [(b, c, np.full((C, K), 0.9, np.float32)) for b, c in bound_blocks(C, K, n)]
+
+
+def scored_trackers(method):
+    """(obj_thresh of its pipelines, GPU tracker(C, K, device), host tracker(C, K), the bound stream's (C, K, blocks(n),
+    tracker(device))) of the --track bytetrack / ocsort arms."""
+    from k210_yolo_framework_b200.track import ByteTracker, OcSortTracker
+    from oracle import bytetrack_ref, ocsort_ref
+    if method == "bytetrack":
+        return (0.1, lambda C, K, d: ByteTracker(C, K, device=d), bytetrack_ref.ByteTrack,
+                (80, 100, lambda n: bytetrack_bound_blocks(80, 100, n), lambda d: ByteTracker(80, 100, device=d)))
+    return (0.3, lambda C, K, d: OcSortTracker(C, K, device=d), ocsort_ref.OcSort,
+            (80, 100, lambda n: ocsort_bound_blocks(80, 100, n), lambda d: OcSortTracker(80, 100, max_age=39, device=d)))
+
+
+def bench_scored(make_pipe, n, load, batch, windows, method):
+    """The --track bytetrack and --track ocsort arms (see the module docstring)."""
+    obj_thresh, gpu_tracker, host_tracker, (bC, bK, bound, bound_tracker) = scored_trackers(method)
+    plain, tracked = make_pipe(obj_thresh), make_pipe(obj_thresh)
     C, K = plain.gather.C, plain.gather.K
     recs = run(plain, n, load, 4)                                   # warm-up of both
-    tracked.enable_tracking(method="bytetrack")
+    tracked.enable_tracking(method=method)
     got = []
     assert run(tracked, n, load, 4, tracks=got) == recs             # tracking leaves the records as they were
     times = {"gpu_plain": [], "gpu_track": []}
@@ -395,7 +422,7 @@ def bench_bytetrack(make_pipe, n, load, batch, windows):
     for stream, frames in (("route", blocks), ("dense_voc_first_batch", dense[:batch])):
         host[stream] = []
         for w in range(windows + 1):            # the first pass warms up
-            tracker = bytetrack_ref.ByteTrack(C, K)
+            tracker = host_tracker(C, K)
             t0 = time.perf_counter()
             out = [tracker.update(p, *f) for p, f in enumerate(frames)]
             if w:
@@ -403,16 +430,15 @@ def bench_bytetrack(make_pipe, n, load, batch, windows):
         ref[stream] = np.stack([o[0] for o in out]), np.stack([o[1] for o in out])
     dev = torch.device("cuda", plain.device_index)
     first = []
-    kernel = {"route": time_kernel(blocks, C, K, 0, batch, windows, dev, lambda: ByteTracker(C, K, device=dev.index)),
-              "dense_voc": time_kernel(dense, C, K, 0, batch, windows, dev, lambda: ByteTracker(C, K, device=dev.index), first),
-              "coco_bound": time_kernel(bytetrack_bound_blocks(80, 100, n), 80, 100, 0, batch, windows, dev,
-                                        lambda: ByteTracker(80, 100, device=dev.index))}
+    kernel = {"route": time_kernel(blocks, C, K, 0, batch, windows, dev, lambda: gpu_tracker(C, K, dev.index)),
+              "dense_voc": time_kernel(dense, C, K, 0, batch, windows, dev, lambda: gpu_tracker(C, K, dev.index), first),
+              "coco_bound": time_kernel(bound(n), bC, bK, 0, batch, windows, dev, lambda: bound_tracker(dev.index))}
     equal = {"route": _same(ids, boxes, *ref["route"]), "dense_voc_first_batch": _same(*first, *ref["dense_voc_first_batch"])}
-    return {"obj_thresh": 0.1, "records": int(sum(len(r) for r in recs)),
+    return {"obj_thresh": obj_thresh, "records": int(sum(len(r) for r in recs)),
             "frames_per_s": {k: round(n / statistics.median(v), 1) for k, v in times.items()},
             "windows_s": {k: [round(t, 4) for t in v] for k, v in times.items()},
-            "bytetrack_kernel_ms_per_batch_median_max": kernel,
-            "bytetrack_ref_frames_per_s": {k: round(len(blocks if k == "route" else dense[:batch]) / statistics.median(v), 1)
+            f"{method}_kernel_ms_per_batch_median_max": kernel,
+            f"{method}_ref_frames_per_s": {k: round(len(blocks if k == "route" else dense[:batch]) / statistics.median(v), 1)
                                            for k, v in host.items()},
             "reported_records": int((ids >= 0).sum()), "tracks": int(ids.max(initial=0)), "ids_equal_by_stream": equal,
             "ids_equal": all(equal.values())}

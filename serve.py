@@ -43,8 +43,10 @@ DIR/<stem>.avi, a Motion-JPEG AVI of the drawn frames at the source frame rate, 
 With --track (a video only) the objects are tracked across the frames on the GPU, SORT-style (DetectionPipeline.enable_tracking,
 --track_max_age, --track_min_hits, --track_iou), or with --tracker bytetrack by ByteTrack (--track_thresh, --track_match,
 --track_buffer, --track_no_fuse_score; its low-score association sees only the records above --obj_thresh, so it wants
---obj_thresh 0.1): every detection of a line gains "track", its track id or null, and
-"track_box_tlbr", the track's box, when it has an id.  Dropped frames count as frames without detections.
+--obj_thresh 0.1), or with --tracker ocsort by OC-SORT (--track_max_age, default 30, --track_min_hits, --track_iou,
+--track_det_thresh, --track_delta_t, --track_inertia, --track_use_byte): every detection of a line gains "track", its track id
+or null, and "track_box_tlbr", the track's box, when it has an id (under OC-SORT the record's own box).  Dropped frames count
+as frames without detections.
 """
 import argparse
 import io
@@ -332,8 +334,10 @@ class ModelArgParser(argparse.ArgumentParser):
             self.error("--tile_size needs --tile_images N: the images one batch holds")
         if n is not None and size is None:
             self.error("--tile_images goes with --tile_size")
-        if hasattr(ns, "tracker") and track_args_error(ns):
-            self.error(track_args_error(ns))
+        if hasattr(ns, "tracker"):
+            fill_track_defaults(ns)
+            if track_args_error(ns):
+                self.error(track_args_error(ns))
         return ns, rest
 
 
@@ -367,39 +371,63 @@ def build_parser():
                          "rendered and JPEG-encoded on the GPU; for a video, its drawn frames as the Motion-JPEG AVI DIR/<stem>.avi")
     ap.add_argument("--draw_quality", type=quality_arg, default=75, help="JPEG quality of the --draw files (1..100)")
     ap.add_argument("--track", action="store_true",
-                    help="track objects across a video's frames on the GPU (SORT, or --tracker bytetrack): each detection gains "
-                         "its track id and box")
+                    help="track objects across a video's frames on the GPU (SORT, or --tracker bytetrack or ocsort): each "
+                         "detection gains its track id and box")
     add_track_args(ap, " (--track)")
     return ap
 
 
 def add_track_args(ap, note=""):
-    """The tracker flags serve.py and evaluate_mot.py share (DetectionPipeline.enable_tracking)."""
-    ap.add_argument("--tracker", choices=["sort", "bytetrack"], default="sort",
-                    help="SORT, or ByteTrack, which also associates the tracks left with the low-score records; it sees only "
-                         "the records above --obj_thresh, so its second association needs --obj_thresh 0.1" + note)
-    ap.add_argument("--track_max_age", type=int, default=1, help="frames a track may miss before it is removed (SORT)" + note)
-    ap.add_argument("--track_min_hits", type=int, default=3, help="matched frames in a row before a track is reported (SORT)" + note)
-    ap.add_argument("--track_iou", type=float, default=0.3, help="least IoU of a detection with its track's prediction (SORT)" + note)
+    """The tracker flags serve.py and evaluate_mot.py share (DetectionPipeline.enable_tracking).  --track_max_age,
+    --track_min_hits and --track_iou default to the selected tracker's values (ModelArgParser fills them in)."""
+    ap.add_argument("--tracker", choices=["sort", "bytetrack", "ocsort"], default="sort",
+                    help="SORT; ByteTrack, which also associates the tracks left with the low-score records (it sees only "
+                         "the records above --obj_thresh, so its second association needs --obj_thresh 0.1); or OC-SORT, which "
+                         "re-updates a re-found track along a virtual path, adds a direction term to the association and "
+                         "re-matches by the tracks' last observations" + note)
+    ap.add_argument("--track_max_age", type=int, default=None,
+                    help="frames a track may miss before it is removed (SORT, default 1; OC-SORT, default 30)" + note)
+    ap.add_argument("--track_min_hits", type=int, default=None,
+                    help="matched frames in a row before a track is reported (SORT and OC-SORT, default 3)" + note)
+    ap.add_argument("--track_iou", type=float, default=None,
+                    help="least IoU of a detection with its track's prediction (SORT and OC-SORT, default 0.3)" + note)
     ap.add_argument("--track_thresh", type=float, default=0.5,
                     help="score above which a record is high (ByteTrack; low records score in (0.1, track_thresh))" + note)
     ap.add_argument("--track_match", type=float, default=0.8, help="largest cost of the first association (ByteTrack)" + note)
     ap.add_argument("--track_buffer", type=int, default=30, help="frames a lost track is kept (ByteTrack)" + note)
     ap.add_argument("--track_no_fuse_score", action="store_true",
                     help="associate by IoU alone, not IoU times score (ByteTrack; its --mot20)" + note)
+    ap.add_argument("--track_det_thresh", type=float, default=0.6,
+                    help="score above which a record is associated first and may start a track (OC-SORT)" + note)
+    ap.add_argument("--track_delta_t", type=int, default=3,
+                    help="frames back to the observation a track's direction is taken from, 1..8 (OC-SORT)" + note)
+    ap.add_argument("--track_inertia", type=float, default=0.2, help="weight of the direction term (OC-SORT)" + note)
+    ap.add_argument("--track_use_byte", action="store_true",
+                    help="also associate the tracks left with the records scored in (0.1, track_det_thresh), as ByteTrack "
+                         "does; it needs --obj_thresh 0.1 (OC-SORT)" + note)
 
 
 SORT_FLAGS = {"track_max_age": 1, "track_min_hits": 3, "track_iou": 0.3}
 BYTETRACK_FLAGS = {"track_thresh": 0.5, "track_match": 0.8, "track_buffer": 30, "track_no_fuse_score": False}
+OCSORT_FLAGS = {"track_det_thresh": 0.6, "track_delta_t": 3, "track_inertia": 0.2, "track_use_byte": False}
+OCSORT_SHARED = {"track_max_age": 30, "track_min_hits": 3, "track_iou": 0.3}
+
+
+def fill_track_defaults(ns):
+    """Gives --track_max_age, --track_min_hits and --track_iou, where left out, the value of the tracker --tracker selects."""
+    for k, v in (OCSORT_SHARED if ns.tracker == "ocsort" else SORT_FLAGS).items():
+        if getattr(ns, k) is None:
+            setattr(ns, k, v)
 
 
 def track_args_error(ns):
-    """The message for add_track_args flags of the tracker --tracker does not select, set away from their defaults; None when
-    there are none."""
-    other = BYTETRACK_FLAGS if ns.tracker == "sort" else SORT_FLAGS
+    """The message for add_track_args flags of the trackers --tracker does not select, set away from their defaults; None
+    when there are none."""
+    other = {"sort": {**BYTETRACK_FLAGS, **OCSORT_FLAGS}, "bytetrack": {**SORT_FLAGS, **OCSORT_FLAGS},
+             "ocsort": BYTETRACK_FLAGS}[ns.tracker]
     wrong = [f"--{k}" for k, v in other.items() if getattr(ns, k) != v]
     if wrong:
-        return f"{', '.join(wrong)} set the other tracker than --tracker {ns.tracker}"
+        return f"{', '.join(wrong)} set another tracker than --tracker {ns.tracker}"
     return None
 
 
@@ -407,7 +435,8 @@ def enable_tracking(pipe, args):
     """DetectionPipeline.enable_tracking with the add_track_args flags."""
     pipe.enable_tracking(args.track_max_age, args.track_min_hits, args.track_iou, method=args.tracker,
                          track_thresh=args.track_thresh, match_thresh=args.track_match, track_buffer=args.track_buffer,
-                         fuse_score=not args.track_no_fuse_score)
+                         fuse_score=not args.track_no_fuse_score, det_thresh=args.track_det_thresh,
+                         delta_t=args.track_delta_t, inertia=args.track_inertia, use_byte=args.track_use_byte)
 
 
 def main():
