@@ -4,21 +4,20 @@
 // One CTA per stream, one warp per class (the warps stride over the classes when there are more): a class's track lists,
 // associations and Kalman filters are its warp's alone.  The lanes predict and update the tracks, compact the ordered lists
 // with ballots, and solve each association with warp_lsap (lsap_warp.cuh, scipy's assignment, ties included), whose cost
-// functor computes the IoU costs on the fly.  The classes meet once per frame, where the frame's births take their ids from
-// one counter in (class, birth) order through a prefix over the CTA.  The launch walks the batch's frames in order.
+// functor computes the IoU costs on the fly.  The classes meet once per frame in frame_loop (tracker.cuh), where the
+// frame's births take their ids from one counter in (class, birth) order.  The launch walks the batch's frames in order.
 //
-// The state lives in global memory between launches (bt_layout): the stream's frame count, last position and ids taken, and
-// per class its two lists, tracked then lost, in one of two track buffers (each frame's rebuild writes the other), plus
-// per-class scratch.  Each buffer holds cap = K (max(B, 1) + 2) tracks, the bound oracle/bytetrack_ref.py derives for the
-// tracks of a class within a frame; the host refuses a setting where it passes BT_MAX.
+// The state lives in global memory between launches (BT_ARRAYS): the stream's header, and per class its two lists, tracked
+// then lost, in one of two track buffers (each frame's rebuild writes the other), plus per-class scratch.  Each buffer
+// holds cap = K (max(B, 1) + 2) tracks, the bound oracle/bytetrack_ref.py derives for the tracks of a class within a frame;
+// the host refuses a setting where it passes BT_MAX.
 //
 // Float64 throughout, in the oracle's operation order: every product is __dmul_rn (so nothing contracts into an FMA),
 // division and sqrt are IEEE round-to-nearest.
 #include <cmath>
 
 #include "common.h"
-#include "lsap_warp.cuh"
-#include "warp_util.cuh"
+#include "tracker.cuh"
 
 namespace k2y {
 namespace {
@@ -40,51 +39,37 @@ struct BDet {
     int k, pad;
 };
 
-struct BtHeader {
-    long long frame_count, last_pos;
-    int ids_taken, started;
-};
-
-struct BtLayout {
-    size_t lists, trk, born, high, low, pool, unc, rest, match, nlist, drop, left, hm, pbox, ubox, nbox, u, v, spc, path,
-        col4row, row4col, remaining, sr, sc, total;
-};
-
 __host__ __device__ inline int bt_cap(int K, int B) { return K * ((B > 1 ? B : 1) + 2); }
 
-// Every per-class array is C consecutive slices of its per-class size.
-__host__ __device__ inline BtLayout bt_layout(int C, int K, int cap) {
-    BtLayout L;
-    size_t o = 0;
-    const size_t c = (size_t)C, n = (size_t)cap, k = (size_t)K;
-    take(o, sizeof(BtHeader));
-    L.lists = take(o, sizeof(int) * 4 * c);                    // n_tracked, n_lost, buffer
-    L.trk = take(o, sizeof(BTrk) * c * 2 * n);
-    L.born = take(o, sizeof(BTrk) * c * k);
-    L.high = take(o, sizeof(BDet) * c * k);
-    L.low = take(o, sizeof(BDet) * c * k);
-    L.pool = take(o, sizeof(int) * c * n);
-    L.unc = take(o, sizeof(int) * c * n);
-    L.rest = take(o, sizeof(int) * c * n);
-    L.match = take(o, sizeof(int) * c * n);
-    L.nlist = take(o, sizeof(int) * c * n);
-    L.drop = take(o, sizeof(int) * c * n);
-    L.left = take(o, sizeof(int) * c * k);
-    L.hm = take(o, sizeof(int) * c * k);
-    L.pbox = take(o, sizeof(double) * 4 * c * n);
-    L.ubox = take(o, sizeof(double) * 4 * c * n);
-    L.nbox = take(o, sizeof(double) * 4 * c * n);
-    L.u = take(o, sizeof(double) * c * n);
-    L.v = take(o, sizeof(double) * c * n);
-    L.spc = take(o, sizeof(double) * c * n);
-    L.path = take(o, sizeof(int) * c * n);
-    L.col4row = take(o, sizeof(int) * c * n);
-    L.row4col = take(o, sizeof(int) * c * n);
-    L.remaining = take(o, sizeof(int) * c * n);
-    L.sr = take(o, c * n);
-    L.sc = take(o, c * n);
-    L.total = o;
-    return L;
+// Every per-class array: type, name, entries per class (k = K records, n = cap tracks).
+#define BT_ARRAYS(X)                                                                                                        \
+    X(int, lists, 4)                /* n_tracked, n_lost, buffer */                                                         \
+    X(BTrk, trk, 2 * n)             /* the two track buffers */                                                             \
+    X(BTrk, born, k)                                                                                                        \
+    X(BDet, high, k)                                                                                                        \
+    X(BDet, low, k)                                                                                                         \
+    X(int, pool, n) X(int, unc, n) X(int, rest, n) X(int, match, n) X(int, nlist, n) X(int, drop, n)                        \
+    X(int, left, k) X(int, hm, k)                                                                                           \
+    X(double, pbox, 4 * n) X(double, ubox, 4 * n) X(double, nbox, 4 * n)
+
+struct ClassView {
+    BT_ARRAYS(K2Y_STATE_FIELD)
+    LsapWork w;
+};
+
+__device__ ClassView class_view(unsigned char *state, size_t C, int c, size_t k, size_t n) {
+    ClassView v;
+    size_t o = state_start();
+    BT_ARRAYS(K2Y_STATE_SLICE)
+    K2Y_LSAP_ARRAYS(K2Y_STATE_SLICE, n, n)
+    return v;
+}
+
+size_t state_bytes(size_t C, size_t k, size_t n) {
+    size_t o = state_start();
+    BT_ARRAYS(K2Y_STATE_BYTES)
+    K2Y_LSAP_ARRAYS(K2Y_STATE_BYTES, n, n)
+    return o;
 }
 
 // Cython's min / max: the second operand when it compares below / above the first
@@ -215,47 +200,6 @@ __device__ void assign(int nr, int nc, const Cost &c, double thresh, const LsapW
     __syncwarp();
 }
 
-// One class's view of the state.
-struct ClassView {
-    int *lists;
-    BTrk *trk, *born;
-    BDet *high, *low;
-    int *pool, *unc, *rest, *match, *nlist, *drop, *left, *hm;
-    double *pbox, *ubox, *nbox;
-    LsapWork w;
-};
-
-__device__ ClassView class_view(unsigned char *state, const BtLayout &L, int c, int K, int cap) {
-    ClassView s;
-    const size_t n = cap, k = K;
-    s.lists = reinterpret_cast<int *>(state + L.lists) + 4 * (size_t)c;
-    s.trk = reinterpret_cast<BTrk *>(state + L.trk) + c * 2 * n;
-    s.born = reinterpret_cast<BTrk *>(state + L.born) + c * k;
-    s.high = reinterpret_cast<BDet *>(state + L.high) + c * k;
-    s.low = reinterpret_cast<BDet *>(state + L.low) + c * k;
-    s.pool = reinterpret_cast<int *>(state + L.pool) + c * n;
-    s.unc = reinterpret_cast<int *>(state + L.unc) + c * n;
-    s.rest = reinterpret_cast<int *>(state + L.rest) + c * n;
-    s.match = reinterpret_cast<int *>(state + L.match) + c * n;
-    s.nlist = reinterpret_cast<int *>(state + L.nlist) + c * n;
-    s.drop = reinterpret_cast<int *>(state + L.drop) + c * n;
-    s.left = reinterpret_cast<int *>(state + L.left) + c * k;
-    s.hm = reinterpret_cast<int *>(state + L.hm) + c * k;
-    s.pbox = reinterpret_cast<double *>(state + L.pbox) + c * 4 * n;
-    s.ubox = reinterpret_cast<double *>(state + L.ubox) + c * 4 * n;
-    s.nbox = reinterpret_cast<double *>(state + L.nbox) + c * 4 * n;
-    s.w.u = reinterpret_cast<double *>(state + L.u) + c * n;
-    s.w.v = reinterpret_cast<double *>(state + L.v) + c * n;
-    s.w.spc = reinterpret_cast<double *>(state + L.spc) + c * n;
-    s.w.path = reinterpret_cast<int *>(state + L.path) + c * n;
-    s.w.col4row = reinterpret_cast<int *>(state + L.col4row) + c * n;
-    s.w.row4col = reinterpret_cast<int *>(state + L.row4col) + c * n;
-    s.w.remaining = reinterpret_cast<int *>(state + L.remaining) + c * n;
-    s.w.SR = state + L.sr + c * n;
-    s.w.SC = state + L.sc + c * n;
-    return s;
-}
-
 struct Setting {
     double track_thresh, match_thresh, det_thresh;
     int buffer, cap;
@@ -367,93 +311,48 @@ __device__ int class_step(const ClassView &s, int f, const int32_t *rec, int cnt
     return nb;
 }
 
-__global__ void __launch_bounds__(BT_THREADS, 1) bytetrack_update_kernel(
-    unsigned char *state, const int32_t *dets, const int32_t *counts, long long row_stride, const int32_t *rows,
-    const long long *positions, int n_frames, int C, int K, Setting st, int32_t *ids_out, float *boxes_out) {
-    __shared__ int s_births[1024];
-    __shared__ int s_base[1024];
-    __shared__ int s_total;
+// The batch and the setting are read in place from the parameters (__grid_constant__), as the callbacks take them by
+// reference.
+__global__ void __launch_bounds__(BT_THREADS, 1) bytetrack_update_kernel(unsigned char *state, const __grid_constant__ Batch bt,
+                                                                         const __grid_constant__ Setting st) {
     __shared__ ClassView s_view[BT_WARPS];      // the warp's class, in shared memory to keep its pointers out of registers
-    const int warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5, lane = threadIdx.x & 31;
-    const BtLayout L = bt_layout(C, K, st.cap);
-    BtHeader *hdr = reinterpret_cast<BtHeader *>(state);
-    long long fc = hdr->frame_count, last = hdr->last_pos;
-    int taken = hdr->ids_taken, started = hdr->started;
-    for (int f = 0; f < n_frames; ++f) {
-        const long long pos = positions[f];
-        // a jump of g positions is g - 1 updates without detections; after track_buffer + 2 of them no track is left
-        const long long gap = started && pos > last + 1 ? pos - last - 1 : 0;
-        const long long empty = gap < (long long)st.buffer + 2 ? gap : (long long)st.buffer + 2;
-        for (int c = warp; c < C; c += n_warps) {
-            ClassView &s = s_view[warp];
-            __syncwarp();
-            if (lane == 0) s = class_view(state, L, c, K, st.cap);
-            __syncwarp();
-            for (long long e = 0; e < empty; ++e) class_step(s, (int)(fc + 1 + e), nullptr, 0, st);
-        }
-        fc += gap + 1;
-        last = pos;
-        started = 1;
-        for (int c = warp; c < C; c += n_warps) {
-            ClassView &s = s_view[warp];
-            __syncwarp();
-            if (lane == 0) s = class_view(state, L, c, K, st.cap);
-            __syncwarp();
-            const int32_t *rec = dets + rows[f] * row_stride + (long long)c * K * 6;
-            int cnt = counts[rows[f] * row_stride + c];
-            cnt = cnt < 0 ? 0 : (cnt > K ? K : cnt);
+    const int lane = threadIdx.x & 31;
+    ClassView &s = s_view[threadIdx.x >> 5];
+    auto view = [&](int c) { return class_view(state, bt.C, c, bt.K, st.cap); };
+    auto empty = [&](long long n, long long fc) {
+        for_each_class(bt.C, s, view, [&](int) {
+            for (long long e = 0; e < n; ++e) class_step(s, (int)(fc + 1 + e), nullptr, 0, st);
+        });
+    };
+    auto frame = [&](int f, long long fc, int *births) {
+        for_each_class(bt.C, s, view, [&](int c) {
+            const int32_t *rec;
+            const int cnt = bt.records(f, c, rec);
             const int nb = class_step(s, (int)fc, rec, cnt, st);
-            if (lane == 0) s_births[c] = nb;
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            int acc = 0;
-            for (int q = 0; q < C; ++q) {
-                s_base[q] = acc;
-                acc += s_births[q];
-            }
-            s_total = acc;
-        }
-        __syncthreads();
-        for (int c = warp; c < C; c += n_warps) {
-            ClassView &s = s_view[warp];
+            if (lane == 0) births[c] = nb;
+        });
+    };
+    auto emit = [&](int f, long long, const int *, const int *base) {
+        for_each_class(bt.C, s, view, [&](int c) {
+            bt.clear(f, c, lane, 32);
             __syncwarp();
-            if (lane == 0) s = class_view(state, L, c, K, st.cap);
-            __syncwarp();
-            int32_t *ids = ids_out + ((long long)f * C + c) * K;
-            float *obox = boxes_out + (((long long)f * C + c) * K) * 4;
-            for (int k = lane; k < K; k += 32) {
-                ids[k] = -1;
-                for (int q = 0; q < 4; ++q) obox[4 * k + q] = 0.f;
-            }
-            __syncwarp();
+            int32_t *ids = bt.ids(f, c);
+            float *obox = bt.boxes(f, c);
             BTrk *trk = s.trk + (size_t)s.lists[2] * st.cap;
-            const int base = taken + s_base[c];
             for (int i = lane; i < s.lists[0]; i += 32) {
                 BTrk &t = trk[i];
-                if (t.id < 0) t.id = base - t.id;
+                if (t.id < 0) t.id = base[c] - t.id;
                 if (t.activated) {
                     double b[4];
                     tlbr(t, b);
                     ids[t.rec] = t.id;
-                    float *o = obox + 4 * t.rec;
-                    o[0] = (float)b[1];
-                    o[1] = (float)b[0];
-                    o[2] = (float)b[3];
-                    o[3] = (float)b[2];
+                    write_box(obox + 4 * t.rec, b);
                 }
             }
             __syncwarp();
-        }
-        taken += s_total;
-        __syncthreads();        // s_births / s_base / s_total are rewritten by the next frame
-    }
-    if (threadIdx.x == 0) {
-        hdr->frame_count = fc;
-        hdr->last_pos = last;
-        hdr->ids_taken = taken;
-        hdr->started = started;
-    }
+        });
+    };
+    frame_loop(state, bt, (long long)st.buffer + 2, empty, frame, emit);
 }
 
 bool bt_args_ok(const char *fn, int C, int K, int B) {
@@ -476,7 +375,7 @@ extern "C" int k2y_bytetrack_state_bytes(int class_num, int max_per_class, int t
         return K2Y_ERR_INVALID;
     }
     if (!bt_args_ok("k2y_bytetrack_state_bytes", class_num, max_per_class, track_buffer)) return K2Y_ERR_INVALID;
-    *bytes = bt_layout(class_num, max_per_class, bt_cap(max_per_class, track_buffer)).total;
+    *bytes = state_bytes(class_num, max_per_class, bt_cap(max_per_class, track_buffer));
     return K2Y_OK;
 }
 
@@ -485,14 +384,11 @@ extern "C" int k2y_bytetrack_update(void *state_dev, const k2y_det *dets_dev, co
                                     int max_per_class, double track_thresh, double match_thresh, int track_buffer, int fuse_score,
                                     int32_t *ids_out_dev, float *boxes_out_dev, void *stream) {
     const char *fn = "k2y_bytetrack_update";
-    if (!bt_args_ok(fn, class_num, max_per_class, track_buffer)) return K2Y_ERR_INVALID;
-    if (!state_dev || !dets_dev || !counts_dev || !rows_dev || !positions_dev || !ids_out_dev || !boxes_out_dev || n_frames < 0 ||
-        !(track_thresh >= 0.0 && track_thresh <= 1.0) || !(match_thresh >= 0.0 && match_thresh <= 1.0)) {
-        set_error("%s: null pointer, n_frames < 0, or track_thresh or match_thresh outside [0, 1]", fn);
-        return K2Y_ERR_INVALID;
-    }
-    if (row_stride_words < (long long)class_num * max_per_class * 6) {
-        set_error("%s: row stride %lld words is smaller than one row's records", fn, row_stride_words);
+    const Batch bt{(const int32_t *)dets_dev, counts_dev, rows_dev, positions_dev, row_stride_words, n_frames, class_num,
+                   max_per_class, ids_out_dev, boxes_out_dev};
+    if (!bt_args_ok(fn, class_num, max_per_class, track_buffer) || !batch_ok(fn, state_dev, bt)) return K2Y_ERR_INVALID;
+    if (!(track_thresh >= 0.0 && track_thresh <= 1.0) || !(match_thresh >= 0.0 && match_thresh <= 1.0)) {
+        set_error("%s: track_thresh or match_thresh outside [0, 1]", fn);
         return K2Y_ERR_INVALID;
     }
     if (n_frames == 0) return K2Y_OK;
@@ -504,9 +400,7 @@ extern "C" int k2y_bytetrack_update(void *state_dev, const k2y_det *dets_dev, co
     st.cap = bt_cap(max_per_class, track_buffer);
     st.fuse = fuse_score != 0;
     const int threads = (class_num < BT_WARPS ? class_num : BT_WARPS) * 32;
-    bytetrack_update_kernel<<<1, threads, 0, (cudaStream_t)stream>>>(
-        (unsigned char *)state_dev, (const int32_t *)dets_dev, counts_dev, row_stride_words, rows_dev, positions_dev, n_frames,
-        class_num, max_per_class, st, ids_out_dev, boxes_out_dev);
+    bytetrack_update_kernel<<<1, threads, 0, (cudaStream_t)stream>>>((unsigned char *)state_dev, bt, st);
     K2Y_CUDA_CHECK(cudaGetLastError());
     return K2Y_OK;
 }

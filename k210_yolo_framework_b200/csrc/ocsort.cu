@@ -3,21 +3,21 @@
 //
 // One CTA per stream, one warp per class (the warps stride over the classes when there are more), as bytetrack.cu.  The
 // lanes predict the tracks, update the matched ones (a re-found track replays its ORU path, at most max_age + 1 steps, on its
-// lane) and keep the ordered lists with ballots.  Each association is one warp_lsap (lsap_warp.cuh): round 1's cost
-// -(iou + angle) is worked out once per pair into scratch, the IoU of rounds 2 and 3 in the cost functor.  The classes meet
-// once per frame, where the births take their ids from one counter in (class, birth) order through a prefix over the CTA.
+// lane) and keep the ordered lists with ballots.  The filter and the IoU are SORT's (tracker.cuh).  Each association is one
+// warp_lsap (lsap_warp.cuh): round 1's cost -(iou + angle) is worked out once per pair into scratch, the IoU of rounds 2 and
+// 3 in the cost functor.  The classes meet once per frame in frame_loop (tracker.cuh), where the births take their ids from
+// one counter in (class, birth) order.
 //
-// The state lives in global memory between launches (oc_layout): the stream's frame count, last position and ids taken, and
-// per class its track list (slot numbers in list order), cap = K (max_age + 1) track slots, the bound oracle/ocsort_ref.py
-// derives, and scratch, round 1's K x cap cost matrix among it.  The host refuses a setting where cap passes OC_MAX.
+// The state lives in global memory between launches (OC_ARRAYS): the stream's header, and per class its track list (slot
+// numbers in list order), cap = K (max_age + 1) track slots, the bound oracle/ocsort_ref.py derives, and scratch, round 1's
+// K x cap cost matrix among it.  The host refuses a setting where cap passes OC_MAX.
 //
 // Float64 throughout, in the oracle's operation order: every product is __dmul_rn (so nothing contracts into an FMA),
 // division and sqrt are IEEE round-to-nearest, and acos is fdlibm's, as the oracle restates it.
 #include <cmath>
 
 #include "common.h"
-#include "lsap_warp.cuh"
-#include "warp_util.cuh"
+#include "tracker.cuh"
 
 namespace k2y {
 namespace {
@@ -25,14 +25,7 @@ namespace {
 constexpr int OC_MAX = 4096;                      // tracks per class (track.py OCSORT_MAX_TRACKS_PER_CLASS)
 constexpr int DT_MAX = 8;                         // delta_t, the ring of observations each track keeps
 constexpr double LOW_THRESH = 0.1;
-constexpr double P0 = 10.0, V0 = 10000.0;
 constexpr int OC_WARPS = 8, OC_THREADS = OC_WARPS * 32;
-
-// SORT's filter in block form (oracle/sort_ref.py): (p, v, P_pp, P_pv, P_vv) of cx, cy, s, and (r, P_rr)
-struct Filt {
-    double b[3][5];
-    double r[2];
-};
 
 struct OTrk {
     Filt kf, frozen;
@@ -50,54 +43,38 @@ struct ODet {
     int k, pad;
 };
 
-struct OcHeader {
-    long long frame_count, last_pos;
-    int ids_taken, started;
-};
-
-struct OcLayout {
-    size_t n, ord, ord2, trk, high, low, pbox, prev, cost, colc, rowp, match, dflag, tflag, ud, ut, owner, born, freel, u, v,
-        spc, path, col4row, row4col, remaining, sr, sc, total;
-};
-
 __host__ __device__ inline int oc_cap(int K, int max_age) { return K * (max_age + 1); }
 
-// Every per-class array is C consecutive slices of its per-class size.
-__host__ __device__ inline OcLayout oc_layout(int C, int K, int cap) {
-    OcLayout L;
-    size_t o = 0;
-    const size_t c = (size_t)C, n = (size_t)cap, k = (size_t)K;
-    take(o, sizeof(OcHeader));
-    L.n = take(o, sizeof(int) * c);
-    L.ord = take(o, sizeof(int) * c * n);
-    L.ord2 = take(o, sizeof(int) * c * n);
-    L.trk = take(o, sizeof(OTrk) * c * n);
-    L.high = take(o, sizeof(ODet) * c * k);
-    L.low = take(o, sizeof(ODet) * c * k);
-    L.pbox = take(o, sizeof(double) * 4 * c * n);
-    L.prev = take(o, sizeof(double) * 5 * c * n);         // k-previous centre (cx, cy), valid, velocity (dy, dx)
-    L.cost = take(o, sizeof(double) * c * k * n);
-    L.colc = take(o, sizeof(int) * c * n);
-    L.rowp = take(o, sizeof(int) * c * k);
-    L.match = take(o, sizeof(int) * c * n);
-    L.dflag = take(o, sizeof(int) * c * k);
-    L.tflag = take(o, sizeof(int) * c * n);
-    L.ud = take(o, sizeof(int) * c * k);
-    L.ut = take(o, sizeof(int) * c * n);
-    L.owner = take(o, sizeof(int) * c * k);
-    L.born = take(o, sizeof(int) * c * k);
-    L.freel = take(o, sizeof(int) * c * n);
-    L.u = take(o, sizeof(double) * c * n);
-    L.v = take(o, sizeof(double) * c * n);
-    L.spc = take(o, sizeof(double) * c * n);
-    L.path = take(o, sizeof(int) * c * n);
-    L.col4row = take(o, sizeof(int) * c * n);
-    L.row4col = take(o, sizeof(int) * c * n);
-    L.remaining = take(o, sizeof(int) * c * n);
-    L.sr = take(o, c * n);
-    L.sc = take(o, c * n);
-    L.total = o;
-    return L;
+// Every per-class array: type, name, entries per class (k = K records, n = cap track slots).
+#define OC_ARRAYS(X)                                                                                                        \
+    X(int, n, 1)                    /* the list's length */                                                                 \
+    X(int, ord, n) X(int, ord2, n)  /* the list: slot numbers in list order */                                              \
+    X(OTrk, trk, n)                                                                                                         \
+    X(ODet, high, k) X(ODet, low, k)                                                                                        \
+    X(double, pbox, 4 * n)                                                                                                  \
+    X(double, prev, 5 * n)          /* k-previous centre (cx, cy), valid, velocity (dy, dx) */                              \
+    X(double, cost, k * n)          /* round 1's cost matrix */                                                             \
+    X(int, colc, n) X(int, rowp, k) X(int, match, n) X(int, dflag, k) X(int, tflag, n) X(int, ud, k) X(int, ut, n)          \
+    X(int, owner, k) X(int, born, k) X(int, freel, n)
+
+struct ClassView {
+    OC_ARRAYS(K2Y_STATE_FIELD)
+    LsapWork w;
+};
+
+__device__ ClassView class_view(unsigned char *state, size_t C, int c, size_t k, size_t n) {
+    ClassView v;
+    size_t o = state_start();
+    OC_ARRAYS(K2Y_STATE_SLICE)
+    K2Y_LSAP_ARRAYS(K2Y_STATE_SLICE, n, n)
+    return v;
+}
+
+size_t state_bytes(size_t C, size_t k, size_t n) {
+    size_t o = state_start();
+    OC_ARRAYS(K2Y_STATE_BYTES)
+    K2Y_LSAP_ARRAYS(K2Y_STATE_BYTES, n, n)
+    return o;
 }
 
 // -- fdlibm's __ieee754_acos (oracle/ocsort_ref.py ``acos``) ---------------------------------------------------------------
@@ -146,44 +123,7 @@ __device__ double fd_acos(double x) {
     return mul(2.0, df + w);
 }
 
-// -- the filter ------------------------------------------------------------------------------------------------------------
-__device__ void filt_predict(Filt &f) {
-    for (int q = 0; q < 3; ++q) {
-        double *b = f.b[q];
-        const double t = b[3] + b[4];
-        b[0] = b[0] + b[1];
-        b[2] = ((b[2] + b[3]) + t) + 1.0;
-        b[3] = t;
-        b[4] = b[4] + (q == 2 ? 1e-4 : 0.01);
-    }
-    f.r[1] = f.r[1] + 1.0;
-}
-
-__device__ void filt_update(Filt &f, const double *z) {
-    for (int q = 0; q < 3; ++q) {
-        double *b = f.b[q];
-        const double R = q == 2 ? 10.0 : 1.0;
-        const double p = b[0], v = b[1], a = b[2], pv = b[3], d = b[4];
-        const double y = z[q] - p;
-        const double S = a + R;
-        const double k0 = a / S, k1 = pv / S;
-        const double c = 1.0 - k0;
-        const double m = pv - mul(k1, a);
-        const double n = d - mul(k1, pv);
-        const double rk0 = mul(R, k0);
-        b[0] = p + mul(k0, y);
-        b[1] = v + mul(k1, y);
-        b[2] = mul(mul(c, a), c) + mul(rk0, k0);
-        b[3] = mul(c, m) + mul(rk0, k1);
-        b[4] = (n - mul(k1, m)) + mul(mul(R, k1), k1);
-    }
-    const double S = f.r[1] + 10.0;
-    const double k = f.r[1] / S;
-    const double c = 1.0 - k;
-    f.r[0] = f.r[0] + mul(k, z[3] - f.r[0]);
-    f.r[1] = mul(mul(c, f.r[1]), c) + mul(mul(10.0, k), k);
-}
-
+// -- the filter: SORT's (tracker.cuh), fed OC-SORT's z ----------------------------------------------------------------
 __device__ void to_z(const double *b, double *z) {
     const double w = b[2] - b[0], h = b[3] - b[1];
     z[0] = b[0] + w / 2.0;
@@ -192,30 +132,7 @@ __device__ void to_z(const double *b, double *z) {
     z[3] = w / (h + 1e-6);
 }
 
-__device__ void state_box(const Filt &f, double *o) {
-    const double cx = f.b[0][0], cy = f.b[1][0], s = f.b[2][0];
-    const double w = sqrt(mul(s, f.r[0]));
-    const double h = s / w;
-    o[0] = cx - w / 2.0;
-    o[1] = cy - h / 2.0;
-    o[2] = cx + w / 2.0;
-    o[3] = cy + h / 2.0;
-}
-
 // -- boxes -----------------------------------------------------------------------------------------------------------------
-// numpy's maximum / minimum: NaN propagates
-__device__ __forceinline__ double mx(double a, double b) { return (a >= b || a != a) ? a : b; }
-__device__ __forceinline__ double mn(double a, double b) { return (a <= b || a != a) ? a : b; }
-
-// SORT's iou_batch for one pair (oracle/sort_ref.py ``iou``), 0 where the union is not > 0
-__device__ double iou(const double *d, const double *t) {
-    const double w = mx(0.0, mn(d[2], t[2]) - mx(d[0], t[0]));
-    const double h = mx(0.0, mn(d[3], t[3]) - mx(d[1], t[1]));
-    const double wh = mul(w, h);
-    const double uni = (mul(d[2] - d[0], d[3] - d[1]) + mul(t[2] - t[0], t[3] - t[1])) - wh;
-    return uni > 0 ? wh / uni : 0.0;
-}
-
 __device__ __forceinline__ double sum5(const double *o) { return (((o[0] + o[1]) + o[2]) + o[3]) + o[4]; }
 
 // the unit (dy, dx) from centre (cx1, cy1) to (cx2, cy2)
@@ -235,15 +152,7 @@ struct Setting {
 __device__ void birth(OTrk &t, const ODet &d, int b) {
     double z[4];
     to_z(d.b, z);
-    for (int q = 0; q < 3; ++q) {
-        t.kf.b[q][0] = z[q];
-        t.kf.b[q][1] = 0.0;
-        t.kf.b[q][2] = P0;
-        t.kf.b[q][3] = 0.0;
-        t.kf.b[q][4] = V0;
-    }
-    t.kf.r[0] = z[3];
-    t.kf.r[1] = P0;
+    filt_init(t.kf, z);
     for (int q = 0; q < 5; ++q) t.last_obs[q] = -1.0;
     for (int q = 0; q < DT_MAX; ++q) t.ring_age[q] = -1;
     t.vel[0] = t.vel[1] = 0.0;
@@ -253,14 +162,9 @@ __device__ void birth(OTrk &t, const ODet &d, int b) {
     t.last_i = -1;
 }
 
-// The tracker's predict: SORT's vs quirk, the filter's predict, the counters; leaves the predicted box in t.pb.
+// SORT's tracker predict; leaves the predicted box in t.pb.
 __device__ void predict(OTrk &t) {
-    double *sb = t.kf.b[2];
-    if (sb[1] + sb[0] <= 0) sb[1] = mul(sb[1], 0.0);
-    filt_predict(t.kf);
-    t.age += 1;
-    if (t.tsu > 0) t.hit_streak = 0;
-    t.tsu += 1;
+    sort_predict(t);
     state_box(t.kf, t.pb);
 }
 
@@ -344,49 +248,6 @@ __device__ int load_det(const int32_t *rec, int k, const Setting &st, ODet &d) {
     return kind;
 }
 
-// One class's view of the state.
-struct ClassView {
-    int *n, *ord, *ord2, *colc, *rowp, *match, *dflag, *tflag, *ud, *ut, *owner, *born, *freel;
-    OTrk *trk;
-    ODet *high, *low;
-    double *pbox, *prev, *cost;
-    LsapWork w;
-};
-
-__device__ ClassView class_view(unsigned char *state, const OcLayout &L, int c, int K, int cap) {
-    ClassView s;
-    const size_t n = cap, k = K;
-    s.n = reinterpret_cast<int *>(state + L.n) + c;
-    s.ord = reinterpret_cast<int *>(state + L.ord) + c * n;
-    s.ord2 = reinterpret_cast<int *>(state + L.ord2) + c * n;
-    s.trk = reinterpret_cast<OTrk *>(state + L.trk) + c * n;
-    s.high = reinterpret_cast<ODet *>(state + L.high) + c * k;
-    s.low = reinterpret_cast<ODet *>(state + L.low) + c * k;
-    s.pbox = reinterpret_cast<double *>(state + L.pbox) + c * 4 * n;
-    s.prev = reinterpret_cast<double *>(state + L.prev) + c * 5 * n;
-    s.cost = reinterpret_cast<double *>(state + L.cost) + c * k * n;
-    s.colc = reinterpret_cast<int *>(state + L.colc) + c * n;
-    s.rowp = reinterpret_cast<int *>(state + L.rowp) + c * k;
-    s.match = reinterpret_cast<int *>(state + L.match) + c * n;
-    s.dflag = reinterpret_cast<int *>(state + L.dflag) + c * k;
-    s.tflag = reinterpret_cast<int *>(state + L.tflag) + c * n;
-    s.ud = reinterpret_cast<int *>(state + L.ud) + c * k;
-    s.ut = reinterpret_cast<int *>(state + L.ut) + c * n;
-    s.owner = reinterpret_cast<int *>(state + L.owner) + c * k;
-    s.born = reinterpret_cast<int *>(state + L.born) + c * k;
-    s.freel = reinterpret_cast<int *>(state + L.freel) + c * n;
-    s.w.u = reinterpret_cast<double *>(state + L.u) + c * n;
-    s.w.v = reinterpret_cast<double *>(state + L.v) + c * n;
-    s.w.spc = reinterpret_cast<double *>(state + L.spc) + c * n;
-    s.w.path = reinterpret_cast<int *>(state + L.path) + c * n;
-    s.w.col4row = reinterpret_cast<int *>(state + L.col4row) + c * n;
-    s.w.row4col = reinterpret_cast<int *>(state + L.row4col) + c * n;
-    s.w.remaining = reinterpret_cast<int *>(state + L.remaining) + c * n;
-    s.w.SR = state + L.sr + c * n;
-    s.w.SC = state + L.sc + c * n;
-    return s;
-}
-
 __device__ double warp_max(double v) {
     for (int o = 16; o > 0; o >>= 1) {
         const double x = __shfl_xor_sync(0xffffffffu, v, o);
@@ -465,7 +326,7 @@ __device__ int class_step(const ClassView &s, const int32_t *rec, int cnt, int K
             double *crow = s.cost + (size_t)d * cap;
             int cntd = 0, pick = -1;
             for (int j = lane; j < T; j += 32) {
-                const double v = iou(db, s.pbox + 4 * j);
+                const double v = sort_iou(db, s.pbox + 4 * j);
                 crow[j] = v;
                 if (v > st.iou_thresh) {
                     ++cntd;
@@ -511,7 +372,7 @@ __device__ int class_step(const ClassView &s, const int32_t *rec, int cnt, int K
             const int j = s.match[d];
             if (j >= 0) {
                 s.tflag[j] = 1;
-                s.dflag[d] = iou(s.high[d].b, s.pbox + 4 * j) < st.iou_thresh ? 2 : 1;
+                s.dflag[d] = sort_iou(s.high[d].b, s.pbox + 4 * j) < st.iou_thresh ? 2 : 1;
             }
         }
         __syncwarp();
@@ -530,8 +391,8 @@ __device__ int class_step(const ClassView &s, const int32_t *rec, int cnt, int K
     nut += compact(D, [&](int d) { return s.dflag[d] == 2; }, [&](int d, int at) { s.ut[nut + at] = s.match[d]; });
     // round 2 (BYTE): low detections x the unmatched tracks' predicted boxes
     if (NL > 0 && nut > 0) {
-        const bool ran = rematch(NL, nut, [&](int i, int j) { return iou(s.low[i].b, s.pbox + 4 * s.ut[j]); }, st.iou_thresh,
-                                 s.w, s.match);
+        const bool ran = rematch(NL, nut, [&](int i, int j) { return sort_iou(s.low[i].b, s.pbox + 4 * s.ut[j]); },
+                                 st.iou_thresh, s.w, s.match);
         if (ran) {
             for (int j = lane; j < T; j += 32) s.tflag[j] = 0;          // 1 unmatched, 2 taken here
             __syncwarp();
@@ -552,8 +413,8 @@ __device__ int class_step(const ClassView &s, const int32_t *rec, int cnt, int K
     }
     // round 3 (OCR): the unmatched high detections x the unmatched tracks' last observations
     if (nud > 0 && nut > 0) {
-        const bool ran = rematch(nud, nut, [&](int i, int j) { return iou(s.high[s.ud[i]].b, trk[ord[s.ut[j]]].last_obs); },
-                                 st.iou_thresh, s.w, s.match);
+        const auto io = [&](int i, int j) { return sort_iou(s.high[s.ud[i]].b, trk[ord[s.ut[j]]].last_obs); };
+        const bool ran = rematch(nud, nut, io, st.iou_thresh, s.w, s.match);
         if (ran) {
             for (int j = lane; j < T; j += 32) s.tflag[j] = 0;
             for (int d = lane; d < D; d += 32) s.dflag[d] = 0;
@@ -602,67 +463,36 @@ __device__ int class_step(const ClassView &s, const int32_t *rec, int cnt, int K
     return nud;
 }
 
-__global__ void __launch_bounds__(OC_THREADS, 1) ocsort_update_kernel(
-    unsigned char *state, const int32_t *dets, const int32_t *counts, long long row_stride, const int32_t *rows,
-    const long long *positions, int n_frames, int C, int K, Setting st, int32_t *ids_out, float *boxes_out) {
-    __shared__ int s_births[1024];
-    __shared__ int s_base[1024];
-    __shared__ int s_total;
+// The batch and the setting are read in place from the parameters (__grid_constant__), as the callbacks take them by
+// reference.
+__global__ void __launch_bounds__(OC_THREADS, 1) ocsort_update_kernel(unsigned char *state, const __grid_constant__ Batch bt,
+                                                                      const __grid_constant__ Setting st) {
     __shared__ ClassView s_view[OC_WARPS];      // the warp's class, in shared memory to keep its pointers out of registers
-    const int warp = threadIdx.x >> 5, n_warps = blockDim.x >> 5, lane = threadIdx.x & 31;
-    const OcLayout L = oc_layout(C, K, st.cap);
-    OcHeader *hdr = reinterpret_cast<OcHeader *>(state);
-    long long fc = hdr->frame_count, last = hdr->last_pos;
-    int taken = hdr->ids_taken, started = hdr->started;
-    for (int f = 0; f < n_frames; ++f) {
-        const long long pos = positions[f];
-        // a jump of g positions is g - 1 updates without detections; after max_age + 1 of them no track is left
-        const long long gap = started && pos > last + 1 ? pos - last - 1 : 0;
-        const long long empty = gap < (long long)st.max_age + 1 ? gap : (long long)st.max_age + 1;
-        for (int c = warp; c < C; c += n_warps) {
-            ClassView &s = s_view[warp];
-            __syncwarp();
-            if (lane == 0) s = class_view(state, L, c, K, st.cap);
-            __syncwarp();
-            for (long long e = 0; e < empty; ++e) class_step(s, nullptr, 0, K, st);
-        }
-        fc += gap + 1;
-        last = pos;
-        started = 1;
-        for (int c = warp; c < C; c += n_warps) {
-            ClassView &s = s_view[warp];
-            __syncwarp();
-            if (lane == 0) s = class_view(state, L, c, K, st.cap);
-            __syncwarp();
-            const int32_t *rec = dets + rows[f] * row_stride + (long long)c * K * 6;
-            int cnt = counts[rows[f] * row_stride + c];
-            cnt = cnt < 0 ? 0 : (cnt > K ? K : cnt);
+    const int lane = threadIdx.x & 31, K = bt.K;
+    ClassView &s = s_view[threadIdx.x >> 5];
+    auto view = [&](int c) { return class_view(state, bt.C, c, K, st.cap); };
+    auto empty = [&](long long n, long long) {
+        for_each_class(bt.C, s, view, [&](int) {
+            for (long long e = 0; e < n; ++e) class_step(s, nullptr, 0, K, st);
+        });
+    };
+    auto frame = [&](int f, long long, int *births) {
+        for_each_class(bt.C, s, view, [&](int c) {
+            const int32_t *rec;
+            const int cnt = bt.records(f, c, rec);
             const int nb = class_step(s, rec, cnt, K, st);
-            if (lane == 0) s_births[c] = nb;
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            int acc = 0;
-            for (int q = 0; q < C; ++q) {
-                s_base[q] = acc;
-                acc += s_births[q];
-            }
-            s_total = acc;
-        }
-        __syncthreads();
-        for (int c = warp; c < C; c += n_warps) {
-            ClassView &s = s_view[warp];
-            __syncwarp();
-            if (lane == 0) s = class_view(state, L, c, K, st.cap);
-            __syncwarp();
-            const int base = taken + s_base[c];
-            for (int b = lane; b < s_births[c]; b += 32) {
+            if (lane == 0) births[c] = nb;
+        });
+    };
+    auto emit = [&](int f, long long fc, const int *births, const int *base) {
+        for_each_class(bt.C, s, view, [&](int c) {
+            for (int b = lane; b < births[c]; b += 32) {
                 OTrk &t = s.trk[s.born[b]];
-                t.id = base - t.id;
+                t.id = base[c] - t.id;
             }
             __syncwarp();
-            int32_t *ids = ids_out + ((long long)f * C + c) * K;
-            float *obox = boxes_out + (((long long)f * C + c) * K) * 4;
+            int32_t *ids = bt.ids(f, c);
+            float *obox = bt.boxes(f, c);
             for (int k = lane; k < K; k += 32) {
                 int id = -1;
                 double b[4] = {0.0, 0.0, 0.0, 0.0};
@@ -679,22 +509,12 @@ __global__ void __launch_bounds__(OC_THREADS, 1) ocsort_update_kernel(
                     }
                 }
                 ids[k] = id;
-                obox[4 * k] = (float)b[1];
-                obox[4 * k + 1] = (float)b[0];
-                obox[4 * k + 2] = (float)b[3];
-                obox[4 * k + 3] = (float)b[2];
+                write_box(obox + 4 * k, b);
             }
             __syncwarp();
-        }
-        taken += s_total;
-        __syncthreads();        // s_births / s_base / s_total are rewritten by the next frame
-    }
-    if (threadIdx.x == 0) {
-        hdr->frame_count = fc;
-        hdr->last_pos = last;
-        hdr->ids_taken = taken;
-        hdr->started = started;
-    }
+        });
+    };
+    frame_loop(state, bt, (long long)st.max_age + 1, empty, frame, emit);
 }
 
 bool oc_args_ok(const char *fn, int C, int K, int max_age, int delta_t) {
@@ -718,7 +538,7 @@ extern "C" int k2y_ocsort_state_bytes(int class_num, int max_per_class, int max_
         return K2Y_ERR_INVALID;
     }
     if (!oc_args_ok("k2y_ocsort_state_bytes", class_num, max_per_class, max_age, delta_t)) return K2Y_ERR_INVALID;
-    *bytes = oc_layout(class_num, max_per_class, oc_cap(max_per_class, max_age)).total;
+    *bytes = state_bytes(class_num, max_per_class, oc_cap(max_per_class, max_age));
     return K2Y_OK;
 }
 
@@ -727,15 +547,12 @@ extern "C" int k2y_ocsort_update(void *state_dev, const k2y_det *dets_dev, const
                                  int max_per_class, double det_thresh, int max_age, int min_hits, double iou_thresh, int delta_t,
                                  double inertia, int use_byte, int32_t *ids_out_dev, float *boxes_out_dev, void *stream) {
     const char *fn = "k2y_ocsort_update";
-    if (!oc_args_ok(fn, class_num, max_per_class, max_age, delta_t)) return K2Y_ERR_INVALID;
-    if (!state_dev || !dets_dev || !counts_dev || !rows_dev || !positions_dev || !ids_out_dev || !boxes_out_dev || n_frames < 0 ||
-        min_hits < 0 || !(det_thresh >= 0.0 && det_thresh <= 1.0) || !(iou_thresh >= 0.0 && iou_thresh <= 1.0) ||
+    const Batch bt{(const int32_t *)dets_dev, counts_dev, rows_dev, positions_dev, row_stride_words, n_frames, class_num,
+                   max_per_class, ids_out_dev, boxes_out_dev};
+    if (!oc_args_ok(fn, class_num, max_per_class, max_age, delta_t) || !batch_ok(fn, state_dev, bt)) return K2Y_ERR_INVALID;
+    if (min_hits < 0 || !(det_thresh >= 0.0 && det_thresh <= 1.0) || !(iou_thresh >= 0.0 && iou_thresh <= 1.0) ||
         !(inertia >= 0.0 && inertia <= 1.0)) {
-        set_error("%s: null pointer, n_frames < 0, min_hits < 0, or det_thresh, iou_thresh or inertia outside [0, 1]", fn);
-        return K2Y_ERR_INVALID;
-    }
-    if (row_stride_words < (long long)class_num * max_per_class * 6) {
-        set_error("%s: row stride %lld words is smaller than one row's records", fn, row_stride_words);
+        set_error("%s: min_hits < 0, or det_thresh, iou_thresh or inertia outside [0, 1]", fn);
         return K2Y_ERR_INVALID;
     }
     if (n_frames == 0) return K2Y_OK;
@@ -749,9 +566,7 @@ extern "C" int k2y_ocsort_update(void *state_dev, const k2y_det *dets_dev, const
     st.use_byte = use_byte != 0;
     st.cap = oc_cap(max_per_class, max_age);
     const int threads = (class_num < OC_WARPS ? class_num : OC_WARPS) * 32;
-    ocsort_update_kernel<<<1, threads, 0, (cudaStream_t)stream>>>(
-        (unsigned char *)state_dev, (const int32_t *)dets_dev, counts_dev, row_stride_words, rows_dev, positions_dev, n_frames,
-        class_num, max_per_class, st, ids_out_dev, boxes_out_dev);
+    ocsort_update_kernel<<<1, threads, 0, (cudaStream_t)stream>>>((unsigned char *)state_dev, bt, st);
     K2Y_CUDA_CHECK(cudaGetLastError());
     return K2Y_OK;
 }

@@ -1,8 +1,9 @@
-"""``warp_lsap`` (csrc/lsap_warp.cuh), the assignment solver of ByteTrack, OC-SORT and the MOT evaluator, against
+"""``warp_lsap`` (csrc/lsap_warp.cuh), the assignment solver of SORT, ByteTrack, OC-SORT and the MOT evaluator, against
 scipy.optimize.linear_sum_assignment: every pair equal, ties included.  The matrices are chosen for what a warp-wide
 solver can get wrong: the tie key across lanes, column counts on either side of a multiple of 32, the transposed case, -0.0
-beside +0.0, 512 x 512 in shared memory and a large problem in global memory.  tests/lsap_harness.cu runs one warp per
-problem; it is compiled here with the library's nvcc flags and is not part of the library."""
+beside +0.0, 512 x 512 in shared memory and a large problem in global memory.  tests/lsap_harness.cu runs the warp form,
+one warp per problem, and the one-thread form SORT uses, 32 problems to a warp; it is compiled here with the library's nvcc
+flags and is not part of the library."""
 import ctypes
 import os
 import subprocess
@@ -16,6 +17,8 @@ from conftest import ROOT
 CSRC = os.path.join(ROOT, "k210_yolo_framework_b200", "csrc")
 HARNESS = os.path.join(ROOT, "tests", "lsap_harness.cu")
 SHARED_CAP = 512        # K2Y_MOT_MAX_ROWS: the shared kernel's entries per array
+GLOBAL, SHARED, THREAD = 0, 1, 2        # the harness's kernels: a warp per problem, state in global or shared memory; a
+                                        # thread per problem, state in global memory
 
 
 def _nvcc_cmd(out):
@@ -91,8 +94,8 @@ def _scipy(c):
     return m
 
 
-def _solve(lib, mats, shared):
-    """warp_lsap's match of every matrix, one warp each, in one launch."""
+def _solve(lib, mats, mode):
+    """warp_lsap's match of every matrix, one warp (or one thread) each, in one launch."""
     import torch
     dev = torch.device("cuda", 0)
     nr = np.array([m.shape[0] for m in mats], np.int32)
@@ -102,7 +105,7 @@ def _solve(lib, mats, shared):
     ent = np.maximum(nr, nc).astype(np.int64)
     woff = np.concatenate([[0], np.cumsum(ent)])
     wn = int(woff[-1])
-    if shared:
+    if mode == SHARED:
         assert ent.max() <= SHARED_CAP
     cost = torch.from_numpy(np.concatenate([m.ravel() for m in mats] + [np.zeros(1)])).to(dev)
     t = {k: torch.from_numpy(v).to(dev) for k, v in dict(coff=coff, moff=moff, woff=woff, nr=nr, nc=nc).items()}
@@ -111,7 +114,7 @@ def _solve(lib, mats, shared):
     wi = torch.empty(4 * wn + 1, dtype=torch.int32, device=dev)
     wb = torch.empty(2 * wn + 1, dtype=torch.uint8, device=dev)
     st = torch.cuda.current_stream(dev)
-    err = lib.lsap_harness_run(len(mats), int(shared), cost.data_ptr(), t["coff"].data_ptr(), t["nr"].data_ptr(),
+    err = lib.lsap_harness_run(len(mats), mode, cost.data_ptr(), t["coff"].data_ptr(), t["nr"].data_ptr(),
                                t["nc"].data_ptr(), t["woff"].data_ptr(), wd.data_ptr(), wi.data_ptr(), wb.data_ptr(), wn,
                                match.data_ptr(), t["moff"].data_ptr(), ctypes.c_void_p(st.cuda_stream))
     assert err == 0
@@ -120,8 +123,8 @@ def _solve(lib, mats, shared):
     return [out[moff[p]:moff[p + 1]] for p in range(len(mats))]
 
 
-def _check(lib, mats, shared, what, kinds=None):
-    got = _solve(lib, mats, shared)
+def _check(lib, mats, mode, what, kinds=None):
+    got = _solve(lib, mats, mode)
     bad = [p for p, (m, g) in enumerate(zip(mats, got)) if not np.array_equal(g, _scipy(m))]
     assert not bad, (what, len(bad), [(mats[p].shape, kinds[p] if kinds else None) for p in bad[:8]])
 
@@ -134,17 +137,17 @@ def _problems(seed, shapes, per):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("shared", [1, 0], ids=["shared", "global"])
-def test_small_shapes_equal_scipy(harness, shared):
-    mats, kinds = _problems(10 + shared, SHAPES, 14)
+@pytest.mark.parametrize("mode", [SHARED, GLOBAL, THREAD], ids=["shared", "global", "thread"])
+def test_small_shapes_equal_scipy(harness, mode):
+    mats, kinds = _problems(10 + mode, SHAPES, 14)
     assert len(mats) > 2000
-    _check(harness, mats, shared, "small", kinds)
+    _check(harness, mats, mode, "small", kinds)
 
 
 @pytest.mark.gpu
 def test_512_in_shared_memory_equals_scipy(harness):
     mats, kinds = _problems(20, LARGE, 1)
-    _check(harness, mats, 1, "512 shared", kinds)
+    _check(harness, mats, SHARED, "512 shared", kinds)
 
 
 @pytest.mark.gpu
@@ -159,8 +162,9 @@ def test_signed_zero_ties_equal_scipy(harness):
                 k = rng.integers(0, nr * nc, 3)
                 c.ravel()[k] = -0.5
             mats.append(c)
-    _check(harness, mats, 1, "signed zeros")
-    _check(harness, mats, 0, "signed zeros, global")
+    _check(harness, mats, SHARED, "signed zeros")
+    _check(harness, mats, GLOBAL, "signed zeros, global")
+    _check(harness, mats, THREAD, "signed zeros, one thread")
 
 
 @pytest.mark.gpu
@@ -170,4 +174,5 @@ def test_large_problem_in_global_memory_equals_scipy(harness):
     # IDTP's costs are negated counts of frames two ids were matched in: mostly -0.0, a few ids overlapping a lot
     c = -np.where(rng.random((1500, 1400)) < 0.004, rng.integers(1, 60, (1500, 1400)), 0).astype(np.float64)
     d = -rng.integers(0, 6, (1400, 1500)).astype(np.float64)
-    _check(harness, [c, d], 0, "large global")
+    _check(harness, [c, d], GLOBAL, "large global")
+    _check(harness, [c, d], THREAD, "large, one thread")
