@@ -11,6 +11,19 @@ with the tracking (SORT, ByteTrack with --tracker bytetrack or OC-SORT with --tr
                                       --track_use_byte --obj_thresh 0.1 ...]
     python -m torch.distributed.run --nproc-per-node 8 evaluate_mot.py ...   # one rank per GPU; rank 0 evaluates
 
+--streams N tracks up to N sequences at once, their frames interleaved in the same batches (serve.interleave; each in its
+own tracking stream, DetectionPipeline.enable_tracking(streams=N)); the default 1 tracks them one after another.  The
+tables, --out and --results are the same for every N.  N is a memory choice: each stream holds the tracker's state,
+k2y_*_state_bytes() on the device, at the default settings per stream
+
+                      VOC (C 20, K 30)    COCO (C 80, K 100)
+    SORT                    0.3 MB                4.0 MB
+    ByteTrack              10.4 MB              138.5 MB
+    OC-SORT                21.8 MB              429.0 MB
+
+(MB of 10^6 bytes; OC-SORT's K x cap scratch of round 1's costs per class makes it the largest, and --track_max_age or
+--max_per_class shrink it).
+
 SEQ is a MOTChallenge sequence directory (seqinfo.ini, imDir/%06d<imExt>, gt/gt.txt); a directory without seqinfo.ini
 stands for its subdirectories that have one, sorted by name (such as MOT17/train).  Each sequence is one stream of frame
 positions 0..seqLength-1, tracked from a fresh start.  A missing frame file, or one whose size differs from seqinfo.ini's,
@@ -25,6 +38,7 @@ TrackEval's summary shows it, and HOTA(0), LocA(0) and HOTALocA(0).  --out write
 repr so that reading a file back gives the evaluated values.  Sequences without gt/gt.txt are tracked and written with
 --results but left out of the metrics.
 """
+import argparse
 import json
 import os
 import sys
@@ -34,7 +48,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 from evaluate_map import load_checked  # noqa: E402
-from serve import ModelArgParser, add_model_args, add_track_args, detect_files, enable_tracking, open_pipeline  # noqa: E402
+from serve import ModelArgParser, add_model_args, add_track_args, detect_files, enable_tracking, interleave, open_pipeline  # noqa: E402
 from k210_yolo_framework_b200.evaluate import MOT_BENCHMARKS, MotEval, load_mot_gt, read_seqinfo  # noqa: E402
 
 HOTA_COLUMNS = ("HOTA", "DetA", "AssA", "DetRe", "DetPr", "AssRe", "AssPr", "LocA", "OWTA", "HOTA(0)", "LocA(0)",
@@ -95,29 +109,35 @@ def evaluate(args):
     pipe, world, rank = open_pipeline(args, args.max_per_class)
     if not 0 <= args.person_class < args.class_num:
         raise ValueError(f"--person_class {args.person_class} is outside [0, {args.class_num})")
-    enable_tracking(pipe, args)
+    enable_tracking(pipe, args, streams=args.streams)
     ev = MotEval(args.benchmark, device=pipe.device_index) if rank == 0 and any(s[2] for s in seqs) else None
     if args.results and rank == 0:
         os.makedirs(args.results, exist_ok=True)
+    if ev is not None:
+        for info, _, gt_path in seqs:
+            if gt_path:
+                ev.add_sequence(info["name"], load_mot_gt(gt_path, args.benchmark), info["seqLength"])
     gpu_png, gpu_progressive = getattr(args, "gpu_png", False), getattr(args, "gpu_progressive", False)
-    for info, files, gt_path in seqs:
-        name, L, hw = info["name"], info["seqLength"], (info["imHeight"], info["imWidth"])
-        if ev is not None and gt_path:
-            ev.add_sequence(name, load_mot_gt(gt_path, args.benchmark), L)
-        pipe.reset_tracks()
-        rows = []
-        for chunk, dets, counts, (ids, boxes) in detect_files(
-                pipe, list(range(L)), args.decode_threads, lambda k: load_checked(files[k], hw, gpu_png, gpu_progressive),
-                positions=list(range(L))):
-            if rank != 0:
-                continue
-            n = len(chunk)
+    lengths = [info["seqLength"] for info, _, _ in seqs]
+    schedule = interleave(lengths, args.streams, pipe.world * pipe.images_per_batch)
+    rows = [[] for _ in seqs]
+    loads = [(lambda k, f=files, hw=(info["imHeight"], info["imWidth"]): load_checked(f[k], hw, gpu_png, gpu_progressive))
+             for info, files, _ in seqs]
+    for chunk, dets, counts, (ids, boxes) in detect_files(pipe, None, args.decode_threads, lambda key: loads[key[0]](key[1]),
+                                                          positions=[list(range(L)) for L in lengths], schedule=schedule):
+        if rank != 0:
+            continue
+        for i in sorted({i for i, _ in chunk}):       # the batch's rows split by sequence, each in frame order
+            (info, _, gt_path), js = seqs[i], [j for j, (q, _) in enumerate(chunk) if q == i]
+            pos = [chunk[j][1] for j in js]
+            part = [t[js] for t in (ids, boxes, dets, counts)]
             if ev is not None and gt_path:
-                ev.update(name, chunk, ids[:n], boxes[:n], dets[:n], counts[:n], args.person_class)
+                ev.update(info["name"], pos, *part, args.person_class)
             if args.results:
-                rows.append(tracker_rows(chunk, ids[:n], boxes[:n], dets[:n], counts[:n], args.person_class))
-        if args.results and rank == 0:
-            write_results(os.path.join(args.results, name + ".txt"), np.concatenate(rows + [np.zeros((0, 7))]))
+                rows[i].append(tracker_rows(pos, *part, args.person_class))
+    if args.results and rank == 0:
+        for (info, _, _), r in zip(seqs, rows):
+            write_results(os.path.join(args.results, info["name"] + ".txt"), np.concatenate(r + [np.zeros((0, 7))]))
     if world > 1:
         dist.barrier()
     return ev.result() if ev is not None else None
@@ -152,6 +172,13 @@ def to_json(res):
     return {"sequences": res["sequences"], "combined": res["combined"], "hota": res["hota"]}
 
 
+def streams_arg(v):
+    n = int(v)
+    if n < 1:
+        raise argparse.ArgumentTypeError(f"--streams {v}: at least 1")
+    return n
+
+
 def build_parser():
     ap = ModelArgParser()
     add_model_args(ap)
@@ -163,6 +190,9 @@ def build_parser():
     ap.add_argument("--iou_thresh", type=float, default=0.5, help="NMS IoU threshold")
     ap.add_argument("--max_per_class", type=int, default=100)
     add_track_args(ap)
+    ap.add_argument("--streams", type=streams_arg, default=1, metavar="N",
+                    help="track up to N sequences at once, in the same batches, each its own stream (the results do not "
+                         "depend on N; each stream holds the tracker's state on the device)")
     ap.add_argument("--results", default=None, metavar="DIR", help="write DIR/<name>.txt in MOTChallenge tracker format")
     ap.add_argument("--out", default=None, help="write the table as JSON")
     return ap

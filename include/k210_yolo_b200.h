@@ -286,6 +286,36 @@ int k2y_ocsort_update(void *state_dev, const k2y_det *dets_dev, const int32_t *c
                       double det_thresh, int max_age, int min_hits, double iou_thresh, int delta_t, double inertia, int use_byte,
                       int32_t *ids_out_dev, float *boxes_out_dev, void *stream);
 
+/* Many streams in one launch: k2y_track_update, k2y_bytetrack_update and k2y_ocsort_update over n_streams independent
+ * streams, with one CTA per stream.
+ *   state_dev       n_streams consecutive states, state_stride bytes apart: the tracker's k2y_*_state_bytes(), a multiple of
+ *                   256 (any stride >= it that is a multiple of 256 is taken).  Each is zeroed to start its stream.
+ *   streams_dev     int32 [n_frames]: each frame's stream, or null when every frame is stream 0.  A batch may mix the streams'
+ *                   frames in any order and lack any of them.  Each stream runs its own frames in batch order, with its own
+ *                   frame count, gaps and ids from 1, exactly as the single-stream call runs them.  A stream with no frame
+ *                   in the batch keeps its state as it is, so its next position counts the frames between as a gap.
+ *                   Frames whose stream lies outside [0, n_streams) get cleared outputs (id -1, box 0) and touch no state;
+ *                   callers should refuse them first.
+ * Positions must increase along each stream; the streams are independent of one another.  The other arguments are as for
+ * the single-stream calls, which are these calls with n_streams 1 and a null streams_dev.  One launch of n_streams CTAs per
+ * call, asynchronous on `stream`.  K2Y_ERR_INVALID (nothing launched) also for n_streams < 1, or, with several streams, a
+ * state_stride below one stream's state bytes or not a multiple of 256. */
+int k2y_track_update_streams(void *state_dev, int n_streams, size_t state_stride, const k2y_det *dets_dev,
+                             const int32_t *counts_dev, long long row_stride_words, const int32_t *rows_dev,
+                             const long long *positions_dev, const int32_t *streams_dev, int n_frames, int class_num,
+                             int max_per_class, int max_age, int min_hits, double iou_thresh, int32_t *ids_out_dev,
+                             float *boxes_out_dev, void *stream);
+int k2y_bytetrack_update_streams(void *state_dev, int n_streams, size_t state_stride, const k2y_det *dets_dev,
+                                 const int32_t *counts_dev, long long row_stride_words, const int32_t *rows_dev,
+                                 const long long *positions_dev, const int32_t *streams_dev, int n_frames, int class_num,
+                                 int max_per_class, double track_thresh, double match_thresh, int track_buffer, int fuse_score,
+                                 int32_t *ids_out_dev, float *boxes_out_dev, void *stream);
+int k2y_ocsort_update_streams(void *state_dev, int n_streams, size_t state_stride, const k2y_det *dets_dev,
+                              const int32_t *counts_dev, long long row_stride_words, const int32_t *rows_dev,
+                              const long long *positions_dev, const int32_t *streams_dev, int n_frames, int class_num,
+                              int max_per_class, double det_thresh, int max_age, int min_hits, double iou_thresh, int delta_t,
+                              double inertia, int use_byte, int32_t *ids_out_dev, float *boxes_out_dev, void *stream);
+
 /* ------------------------------------------------------------------------------------------
  * Multi-GPU collation: images shard across ranks (one process per GPU), and the one exchange on the path
  * is ONE ncclAllGather of the fixed-size record blocks.  The reference is single-process (keras_inference.py:12-17), so

@@ -122,6 +122,14 @@ _SIGNATURES = {
     "k2y_ocsort_update": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_longlong, c_void_p, c_void_p, c_int, c_int, c_int,
                                   ctypes.c_double, c_int, c_int, ctypes.c_double, c_int, ctypes.c_double, c_int, c_void_p, c_void_p,
                                   c_void_p]),
+    "k2y_track_update_streams": (c_int, [c_void_p, c_int, c_size_t, c_void_p, c_void_p, ctypes.c_longlong, c_void_p, c_void_p, c_void_p,
+                                         c_int, c_int, c_int, c_int, c_int, ctypes.c_double, c_void_p, c_void_p, c_void_p]),
+    "k2y_bytetrack_update_streams": (c_int, [c_void_p, c_int, c_size_t, c_void_p, c_void_p, ctypes.c_longlong, c_void_p, c_void_p,
+                                             c_void_p, c_int, c_int, c_int, ctypes.c_double, ctypes.c_double, c_int, c_int, c_void_p,
+                                             c_void_p, c_void_p]),
+    "k2y_ocsort_update_streams": (c_int, [c_void_p, c_int, c_size_t, c_void_p, c_void_p, ctypes.c_longlong, c_void_p, c_void_p, c_void_p,
+                                          c_int, c_int, c_int, ctypes.c_double, c_int, c_int, ctypes.c_double, c_int, ctypes.c_double,
+                                          c_int, c_void_p, c_void_p, c_void_p]),
     "k2y_comm_unique_id": (c_int, [c_void_p]),
     "k2y_comm_create": (c_int, [c_void_p, c_int, c_int, c_int, POINTER(c_void_p)]),
     "k2y_comm_destroy": (c_int, [c_void_p]),

@@ -316,6 +316,8 @@ __device__ int class_step(const ClassView &s, int f, const int32_t *rec, int cnt
 __global__ void __launch_bounds__(BT_THREADS, 1) bytetrack_update_kernel(unsigned char *state, const __grid_constant__ Batch bt,
                                                                          const __grid_constant__ Setting st) {
     __shared__ ClassView s_view[BT_WARPS];      // the warp's class, in shared memory to keep its pointers out of registers
+    if (!stream_has_frames(bt)) return;
+    state += (size_t)blockIdx.x * bt.stride;
     const int lane = threadIdx.x & 31;
     ClassView &s = s_view[threadIdx.x >> 5];
     auto view = [&](int c) { return class_view(state, bt.C, c, bt.K, st.cap); };
@@ -379,14 +381,18 @@ extern "C" int k2y_bytetrack_state_bytes(int class_num, int max_per_class, int t
     return K2Y_OK;
 }
 
-extern "C" int k2y_bytetrack_update(void *state_dev, const k2y_det *dets_dev, const int32_t *counts_dev, long long row_stride_words,
-                                    const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num,
-                                    int max_per_class, double track_thresh, double match_thresh, int track_buffer, int fuse_score,
-                                    int32_t *ids_out_dev, float *boxes_out_dev, void *stream) {
+extern "C" int k2y_bytetrack_update_streams(void *state_dev, int n_streams, size_t state_stride, const k2y_det *dets_dev,
+                                            const int32_t *counts_dev, long long row_stride_words, const int32_t *rows_dev,
+                                            const long long *positions_dev, const int32_t *streams_dev, int n_frames,
+                                            int class_num, int max_per_class, double track_thresh, double match_thresh,
+                                            int track_buffer, int fuse_score, int32_t *ids_out_dev, float *boxes_out_dev,
+                                            void *stream) {
     const char *fn = "k2y_bytetrack_update";
     const Batch bt{(const int32_t *)dets_dev, counts_dev, rows_dev, positions_dev, row_stride_words, n_frames, class_num,
-                   max_per_class, ids_out_dev, boxes_out_dev};
-    if (!bt_args_ok(fn, class_num, max_per_class, track_buffer) || !batch_ok(fn, state_dev, bt)) return K2Y_ERR_INVALID;
+                   max_per_class, ids_out_dev, boxes_out_dev, streams_dev, n_streams, state_stride};
+    if (!bt_args_ok(fn, class_num, max_per_class, track_buffer) ||
+        !batch_ok(fn, state_dev, bt, state_bytes(class_num, max_per_class, bt_cap(max_per_class, track_buffer))))
+        return K2Y_ERR_INVALID;
     if (!(track_thresh >= 0.0 && track_thresh <= 1.0) || !(match_thresh >= 0.0 && match_thresh <= 1.0)) {
         set_error("%s: track_thresh or match_thresh outside [0, 1]", fn);
         return K2Y_ERR_INVALID;
@@ -400,7 +406,16 @@ extern "C" int k2y_bytetrack_update(void *state_dev, const k2y_det *dets_dev, co
     st.cap = bt_cap(max_per_class, track_buffer);
     st.fuse = fuse_score != 0;
     const int threads = (class_num < BT_WARPS ? class_num : BT_WARPS) * 32;
-    bytetrack_update_kernel<<<1, threads, 0, (cudaStream_t)stream>>>((unsigned char *)state_dev, bt, st);
+    bytetrack_update_kernel<<<n_streams, threads, 0, (cudaStream_t)stream>>>((unsigned char *)state_dev, bt, st);
     K2Y_CUDA_CHECK(cudaGetLastError());
     return K2Y_OK;
+}
+
+extern "C" int k2y_bytetrack_update(void *state_dev, const k2y_det *dets_dev, const int32_t *counts_dev, long long row_stride_words,
+                                    const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num,
+                                    int max_per_class, double track_thresh, double match_thresh, int track_buffer, int fuse_score,
+                                    int32_t *ids_out_dev, float *boxes_out_dev, void *stream) {
+    return k2y_bytetrack_update_streams(state_dev, 1, 0, dets_dev, counts_dev, row_stride_words, rows_dev, positions_dev, nullptr,
+                                        n_frames, class_num, max_per_class, track_thresh, match_thresh, track_buffer, fuse_score,
+                                        ids_out_dev, boxes_out_dev, stream);
 }

@@ -468,6 +468,8 @@ __device__ int class_step(const ClassView &s, const int32_t *rec, int cnt, int K
 __global__ void __launch_bounds__(OC_THREADS, 1) ocsort_update_kernel(unsigned char *state, const __grid_constant__ Batch bt,
                                                                       const __grid_constant__ Setting st) {
     __shared__ ClassView s_view[OC_WARPS];      // the warp's class, in shared memory to keep its pointers out of registers
+    if (!stream_has_frames(bt)) return;
+    state += (size_t)blockIdx.x * bt.stride;
     const int lane = threadIdx.x & 31, K = bt.K;
     ClassView &s = s_view[threadIdx.x >> 5];
     auto view = [&](int c) { return class_view(state, bt.C, c, K, st.cap); };
@@ -542,14 +544,18 @@ extern "C" int k2y_ocsort_state_bytes(int class_num, int max_per_class, int max_
     return K2Y_OK;
 }
 
-extern "C" int k2y_ocsort_update(void *state_dev, const k2y_det *dets_dev, const int32_t *counts_dev, long long row_stride_words,
-                                 const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num,
-                                 int max_per_class, double det_thresh, int max_age, int min_hits, double iou_thresh, int delta_t,
-                                 double inertia, int use_byte, int32_t *ids_out_dev, float *boxes_out_dev, void *stream) {
+extern "C" int k2y_ocsort_update_streams(void *state_dev, int n_streams, size_t state_stride, const k2y_det *dets_dev,
+                                         const int32_t *counts_dev, long long row_stride_words, const int32_t *rows_dev,
+                                         const long long *positions_dev, const int32_t *streams_dev, int n_frames, int class_num,
+                                         int max_per_class, double det_thresh, int max_age, int min_hits, double iou_thresh,
+                                         int delta_t, double inertia, int use_byte, int32_t *ids_out_dev, float *boxes_out_dev,
+                                         void *stream) {
     const char *fn = "k2y_ocsort_update";
     const Batch bt{(const int32_t *)dets_dev, counts_dev, rows_dev, positions_dev, row_stride_words, n_frames, class_num,
-                   max_per_class, ids_out_dev, boxes_out_dev};
-    if (!oc_args_ok(fn, class_num, max_per_class, max_age, delta_t) || !batch_ok(fn, state_dev, bt)) return K2Y_ERR_INVALID;
+                   max_per_class, ids_out_dev, boxes_out_dev, streams_dev, n_streams, state_stride};
+    if (!oc_args_ok(fn, class_num, max_per_class, max_age, delta_t) ||
+        !batch_ok(fn, state_dev, bt, state_bytes(class_num, max_per_class, oc_cap(max_per_class, max_age))))
+        return K2Y_ERR_INVALID;
     if (min_hits < 0 || !(det_thresh >= 0.0 && det_thresh <= 1.0) || !(iou_thresh >= 0.0 && iou_thresh <= 1.0) ||
         !(inertia >= 0.0 && inertia <= 1.0)) {
         set_error("%s: min_hits < 0, or det_thresh, iou_thresh or inertia outside [0, 1]", fn);
@@ -566,7 +572,16 @@ extern "C" int k2y_ocsort_update(void *state_dev, const k2y_det *dets_dev, const
     st.use_byte = use_byte != 0;
     st.cap = oc_cap(max_per_class, max_age);
     const int threads = (class_num < OC_WARPS ? class_num : OC_WARPS) * 32;
-    ocsort_update_kernel<<<1, threads, 0, (cudaStream_t)stream>>>((unsigned char *)state_dev, bt, st);
+    ocsort_update_kernel<<<n_streams, threads, 0, (cudaStream_t)stream>>>((unsigned char *)state_dev, bt, st);
     K2Y_CUDA_CHECK(cudaGetLastError());
     return K2Y_OK;
+}
+
+extern "C" int k2y_ocsort_update(void *state_dev, const k2y_det *dets_dev, const int32_t *counts_dev, long long row_stride_words,
+                                 const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num,
+                                 int max_per_class, double det_thresh, int max_age, int min_hits, double iou_thresh, int delta_t,
+                                 double inertia, int use_byte, int32_t *ids_out_dev, float *boxes_out_dev, void *stream) {
+    return k2y_ocsort_update_streams(state_dev, 1, 0, dets_dev, counts_dev, row_stride_words, rows_dev, positions_dev, nullptr,
+                                     n_frames, class_num, max_per_class, det_thresh, max_age, min_hits, iou_thresh, delta_t,
+                                     inertia, use_byte, ids_out_dev, boxes_out_dev, stream);
 }

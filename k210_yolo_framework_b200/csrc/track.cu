@@ -4,7 +4,7 @@
 // association is the one-thread form of warp_lsap (lsap_warp.cuh, scipy's assignment, ties included), as the threads of a
 // warp serve different classes.  The classes meet once per frame in frame_loop (tracker.cuh), where the frame's births
 // take their ids from one counter in (class, birth) order.  The launch walks the batch's frames in order, so one launch
-// serves a batch of any length.
+// serves a batch of any length; with several streams, each CTA walks its own stream's frames on its own state.
 //
 // The state lives in global memory between launches (SORT_ARRAYS): the stream's header, every class's track list in
 // SORT's order, and per-class scratch (the frame's detections, the tracks' predicted boxes and the assignment's work
@@ -119,6 +119,8 @@ __device__ void emit_box(const Trk &t, float *out) {
 // The batch is read in place from the parameters (__grid_constant__), as the callbacks take it by reference.
 __global__ void __launch_bounds__(1024) track_update_kernel(unsigned char *state, const __grid_constant__ Batch bt, int cap,
                                                             int max_age, int min_hits, double iou_thresh) {
+    if (!stream_has_frames(bt)) return;
+    state += (size_t)blockIdx.x * bt.stride;
     const int c = threadIdx.x, C = bt.C, K = bt.K;
     const bool active = c < C;
     const ClassView s = class_view(state, C, active ? c : 0, K, cap);
@@ -234,22 +236,35 @@ extern "C" int k2y_track_state_bytes(int class_num, int max_per_class, int max_a
     return K2Y_OK;
 }
 
-extern "C" int k2y_track_update(void *state_dev, const k2y_det *dets_dev, const int32_t *counts_dev, long long row_stride_words,
-                                const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num,
-                                int max_per_class, int max_age, int min_hits, double iou_thresh, int32_t *ids_out_dev,
-                                float *boxes_out_dev, void *stream) {
+extern "C" int k2y_track_update_streams(void *state_dev, int n_streams, size_t state_stride, const k2y_det *dets_dev,
+                                        const int32_t *counts_dev, long long row_stride_words, const int32_t *rows_dev,
+                                        const long long *positions_dev, const int32_t *streams_dev, int n_frames, int class_num,
+                                        int max_per_class, int max_age, int min_hits, double iou_thresh, int32_t *ids_out_dev,
+                                        float *boxes_out_dev, void *stream) {
     const char *fn = "k2y_track_update";
     const Batch bt{(const int32_t *)dets_dev, counts_dev, rows_dev, positions_dev, row_stride_words, n_frames, class_num,
-                   max_per_class, ids_out_dev, boxes_out_dev};
-    if (!track_args_ok(fn, class_num, max_per_class, max_age) || !batch_ok(fn, state_dev, bt)) return K2Y_ERR_INVALID;
+                   max_per_class, ids_out_dev, boxes_out_dev, streams_dev, n_streams, state_stride};
+    if (!track_args_ok(fn, class_num, max_per_class, max_age) ||
+        !batch_ok(fn, state_dev, bt, state_bytes(class_num, max_per_class, track_cap(max_per_class, max_age))))
+        return K2Y_ERR_INVALID;
     if (min_hits < 0 || !(iou_thresh >= 0.0 && iou_thresh <= 1.0)) {
         set_error("%s: min_hits < 0 or iou_thresh outside [0, 1]", fn);
         return K2Y_ERR_INVALID;
     }
     if (n_frames == 0) return K2Y_OK;
     const int threads = (class_num + 31) / 32 * 32;
-    track_update_kernel<<<1, threads, 0, (cudaStream_t)stream>>>((unsigned char *)state_dev, bt,
-                                                                 track_cap(max_per_class, max_age), max_age, min_hits, iou_thresh);
+    track_update_kernel<<<n_streams, threads, 0, (cudaStream_t)stream>>>((unsigned char *)state_dev, bt,
+                                                                         track_cap(max_per_class, max_age), max_age, min_hits,
+                                                                         iou_thresh);
     K2Y_CUDA_CHECK(cudaGetLastError());
     return K2Y_OK;
+}
+
+extern "C" int k2y_track_update(void *state_dev, const k2y_det *dets_dev, const int32_t *counts_dev, long long row_stride_words,
+                                const int32_t *rows_dev, const long long *positions_dev, int n_frames, int class_num,
+                                int max_per_class, int max_age, int min_hits, double iou_thresh, int32_t *ids_out_dev,
+                                float *boxes_out_dev, void *stream) {
+    return k2y_track_update_streams(state_dev, 1, 0, dets_dev, counts_dev, row_stride_words, rows_dev, positions_dev, nullptr,
+                                    n_frames, class_num, max_per_class, max_age, min_hits, iou_thresh, ids_out_dev, boxes_out_dev,
+                                    stream);
 }

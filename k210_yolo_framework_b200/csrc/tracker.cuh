@@ -169,7 +169,8 @@ __device__ void sort_predict(Track &t) {
 
 // -- the stream ------------------------------------------------------------------------------------------------------------
 // A batch of frames in a gathered record block (dets [.., C, K, 6] and counts [.., C], row_stride words a row), and the
-// outputs ids [n_frames, C, K] and boxes [n_frames, C, K, 4].
+// outputs ids [n_frames, C, K] and boxes [n_frames, C, K, 4].  The frames may belong to n_streams streams, whose states lie
+// `stride` bytes apart: frame f is stream streams[f] (every frame is stream 0 when streams is null).
 struct Batch {
     const int32_t *dets, *counts, *rows;
     const long long *positions;
@@ -177,6 +178,16 @@ struct Batch {
     int n_frames, C, K;
     int32_t *ids_out;
     float *boxes_out;
+    const int32_t *streams;
+    int n_streams;
+    size_t stride;
+
+    __device__ int stream(int f) const { return streams ? streams[f] : 0; }
+    // the first frame from f on of the CTA's stream, blockIdx.x; n_frames when there is none
+    __device__ int next_frame(int f) const {
+        while (f < n_frames && stream(f) != (int)blockIdx.x) ++f;
+        return f;
+    }
 
     // class c's records in frame f and their count, clamped to [0, K]
     __device__ int records(int f, int c, const int32_t *&rec) const {
@@ -206,9 +217,10 @@ __device__ inline void write_box(float *o, const double *b) {
     o[3] = (float)b[2];
 }
 
-// The checks every tracker's update makes of its batch; false, with the error set, for a null pointer, n_frames < 0 or a
-// row stride below one row's records.
-inline bool batch_ok(const char *fn, const void *state, const Batch &b) {
+// The checks every tracker's update makes of its batch; false, with the error set, for a null pointer, n_frames < 0, a
+// row stride below one row's records, n_streams < 1, or (with several streams) a state stride below one stream's
+// state_bytes or not a multiple of 256.
+inline bool batch_ok(const char *fn, const void *state, const Batch &b, size_t state_bytes) {
     if (!state || !b.dets || !b.counts || !b.rows || !b.positions || !b.ids_out || !b.boxes_out || b.n_frames < 0) {
         set_error("%s: null pointer or n_frames < 0", fn);
         return false;
@@ -217,12 +229,34 @@ inline bool batch_ok(const char *fn, const void *state, const Batch &b) {
         set_error("%s: row stride %lld words is smaller than one row's records", fn, b.row_stride);
         return false;
     }
+    if (b.n_streams < 1 || (b.n_streams > 1 && (b.stride < state_bytes || b.stride % 256 != 0))) {
+        set_error("%s: n_streams %d (>= 1) and, with several, a state stride of %zu bytes (a multiple of 256, >= the %zu "
+                  "bytes of one stream's state)", fn, b.n_streams, b.stride, state_bytes);
+        return false;
+    }
     return true;
 }
 
-// The stream's frame loop, run by the whole CTA over the batch's frames in order.  A jump of g positions is g - 1 updates
-// without detections, and after max_empty of them no track is left; then the frame runs, and its births take their ids
-// from the stream's one counter in (class, birth) order.  The tracker's callbacks:
+// Whether the batch has a frame of the CTA's stream, blockIdx.x; a kernel returns at once when it has none, leaving that
+// stream's state as it is, and else works on the state at blockIdx.x * stride.  CTA 0 first clears the outputs of the
+// frames whose stream lies outside [0, n_streams).  Block-wide.  Not inlined: inlined, it costs SORT's kernel (held to 64
+// registers) spills in its frame loop.
+__device__ __noinline__ inline bool stream_has_frames(const Batch &bt) {
+    if (blockIdx.x == 0 && bt.streams) {
+        for (long long i = threadIdx.x; i < (long long)bt.n_frames * bt.C; i += blockDim.x) {
+            const int f = (int)(i / bt.C), s = bt.streams[f];
+            if (s < 0 || s >= bt.n_streams) bt.clear(f, (int)(i % bt.C), 0, 1);
+        }
+    }
+    int mine = 0;
+    for (int f = threadIdx.x; f < bt.n_frames && !mine; f += blockDim.x) mine = bt.stream(f) == (int)blockIdx.x;
+    return __syncthreads_or(mine);
+}
+
+// The stream's frame loop, run by the whole CTA over the batch's frames of its stream, blockIdx.x, in batch order; `state`
+// is that stream's.  A jump of g positions is g - 1 updates without detections, and after max_empty of
+// them no track is left; then the frame runs, and its births take their ids from the stream's one counter in (class,
+// birth) order.  The tracker's callbacks:
 //  - empty(n, fc): n updates without detections, the first at frame count fc + 1;
 //  - frame(f, fc, births): frame f at frame count fc, storing class c's births in births[c];
 //  - emit(f, fc, births, base): frame f's outputs; class c's births are ids base[c] + 1, base[c] + 2, ...
@@ -231,38 +265,33 @@ __device__ void frame_loop(unsigned char *state, const Batch &bt, long long max_
                            const Emit &emit) {
     __shared__ int s_births[1024];
     __shared__ int s_base[1024];
-    __shared__ int s_total;
+    __shared__ StreamHeader s_hdr;      // the header as the frames advance it, in shared memory to keep it out of registers
     StreamHeader *hdr = reinterpret_cast<StreamHeader *>(state);
-    long long fc = hdr->frame_count, last = hdr->last_pos;
-    int taken = hdr->ids_taken, started = hdr->started;
-    for (int f = 0; f < bt.n_frames; ++f) {
-        const long long pos = bt.positions[f];
-        const long long gap = started && pos > last + 1 ? pos - last - 1 : 0;
-        empty(gap < max_empty ? gap : max_empty, fc);
-        fc += gap + 1;
-        last = pos;
-        started = 1;
+    if (threadIdx.x == 0) s_hdr = *hdr;
+    __syncthreads();
+    for (int f = bt.next_frame(0); f < bt.n_frames; f = bt.next_frame(f + 1)) {
+        const long long pos = bt.positions[f], last = s_hdr.last_pos;
+        const long long gap = s_hdr.started && pos > last + 1 ? pos - last - 1 : 0;
+        empty(gap < max_empty ? gap : max_empty, s_hdr.frame_count);
+        const long long fc = s_hdr.frame_count + gap + 1;
         frame(f, fc, s_births);
         __syncthreads();
         if (threadIdx.x == 0) {
-            int acc = taken;
+            int acc = s_hdr.ids_taken;
             for (int q = 0; q < bt.C; ++q) {
                 s_base[q] = acc;
                 acc += s_births[q];
             }
-            s_total = acc;
+            s_hdr.frame_count = fc;
+            s_hdr.last_pos = pos;
+            s_hdr.ids_taken = acc;
+            s_hdr.started = 1;
         }
         __syncthreads();
         emit(f, fc, s_births, s_base);
-        taken = s_total;
-        __syncthreads();        // s_births / s_base / s_total are rewritten by the next frame
+        __syncthreads();        // s_births / s_base / s_hdr are rewritten by the next frame
     }
-    if (threadIdx.x == 0) {
-        hdr->frame_count = fc;
-        hdr->last_pos = last;
-        hdr->ids_taken = taken;
-        hdr->started = started;
-    }
+    if (threadIdx.x == 0) *hdr = s_hdr;
 }
 
 }  // namespace k2y

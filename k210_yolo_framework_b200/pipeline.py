@@ -39,10 +39,11 @@ the image while it loads them, then merges all views as above.  It combines with
 
 ``enable_tracking`` tracks objects across the frames of a stream, SORT-style (``track.Tracker``, oracle/sort_ref.py), with
 ByteTrack (``track.ByteTracker``, oracle/bytetrack_ref.py) or with OC-SORT (``track.OcSortTracker``, oracle/ocsort_ref.py):
-``submit_images(frames=...)`` gives each image's position in the stream, one ``k2y_track_update`` (``k2y_bytetrack_update``,
-``k2y_ocsort_update``) launch per batch runs behind the
-NMS / all-gather on the stream that holds the gathered block, before its D2H, and ``tracks(ticket)`` returns each record's track
-id and box.  The records are unchanged.
+``submit_images(frames=...)`` gives each image's position in the stream, one ``k2y_track_update_streams``
+(``k2y_bytetrack_update_streams``, ``k2y_ocsort_update_streams``) launch per batch runs behind the NMS / all-gather on the
+stream that holds the gathered block, before its D2H, and ``tracks(ticket)`` returns each record's track id and box.  The
+records are unchanged.  ``enable_tracking(streams=S)`` tracks S independent streams at once, one CTA each:
+``submit_images(streams=...)`` names each frame's stream, and a batch may mix them.
 
 ``enable_png_decode`` makes ``submit_images`` decode the PNG files the GPU takes there too (``preprocess.png_gpu_decodable``),
 in the same staging range and H2D copy as the batch's JPEGs; their status words travel beside the JPEGs'.
@@ -62,6 +63,7 @@ from ._lib import check, lib
 from .detect import DET_WORDS, KerasDetector
 from .dist import DetectionGather
 from .preprocess import BatchLayout, Staging, check_jpeg_status, check_png_status, check_progressive_status, letterbox_packed
+from .track import check_positions
 
 SLOTS = 2
 
@@ -245,13 +247,17 @@ class DetectionPipeline:
     def enable_tracking(self, max_age: Optional[int] = None, min_hits: Optional[int] = None, iou_thresh: Optional[float] = None, *,
                         method: str = "sort", track_thresh: float = 0.5, match_thresh: float = 0.8, track_buffer: int = 30,
                         fuse_score: bool = True, det_thresh: float = 0.6, delta_t: int = 3, inertia: float = 0.2,
-                        use_byte: bool = False) -> None:
+                        use_byte: bool = False, streams: int = 1) -> None:
         """From now on ``submit_images`` takes `frames`, each image's position in a stream of frames, and tracks the objects of
         the stream as SORT does (oracle/sort_ref.py states every rule): per class, a Kalman filter per track, IoU association
         by optimal assignment, a track born for each unmatched detection and removed once it missed more than `max_age`
         frames (1 when left out), and reported once it was matched in `min_hits` frames in a row (3; or in the stream's first
         `min_hits` frames), matching at IoU `iou_thresh` (0.3).
         ``tracks(ticket)`` returns each record's id and track box.  A new call starts a new stream, as ``reset_tracks`` does.
+        With `streams` S > 1 the pipeline tracks S independent streams (camera feeds, videos) in the same batches:
+        ``submit_images`` then takes each frame's stream too, and each stream has its own tracks, frame count and ids from 1,
+        exactly as if it were tracked alone, so a track is identified by (stream, id).  Each stream's state takes the
+        tracker's ``k2y_*_state_bytes()`` on the device.
         Raises ``ValueError``, leaving the pipeline as it was, for a bad setting or when max_per_class * (max_age + 1)
         exceeds the 1024 tracks one class holds (max_age <= 33 at max_per_class 30, <= 9 at 100).
 
@@ -282,7 +288,7 @@ class DetectionPipeline:
                 raise ValueError("track_thresh, match_thresh, track_buffer and fuse_score set ByteTrack: use method='bytetrack'")
             if oc_args:
                 raise ValueError("det_thresh, delta_t, inertia and use_byte set OC-SORT: use method='ocsort'")
-            tracker = Tracker(self.gather.C, self.gather.K, *sort_setting, self.device_index)
+            tracker = Tracker(self.gather.C, self.gather.K, *sort_setting, self.device_index, streams)
         elif method == "bytetrack":
             if sort_args:
                 raise ValueError("max_age, min_hits and iou_thresh set SORT: ByteTrack takes track_thresh, match_thresh, "
@@ -290,20 +296,22 @@ class DetectionPipeline:
             if oc_args:
                 raise ValueError("det_thresh, delta_t, inertia and use_byte set OC-SORT: use method='ocsort'")
             tracker = ByteTracker(self.gather.C, self.gather.K, track_thresh, match_thresh, track_buffer, fuse_score,
-                                  self.device_index)
+                                  self.device_index, streams)
         elif method == "ocsort":
             if byte_args:
                 raise ValueError("track_thresh, match_thresh, track_buffer and fuse_score set ByteTrack: OC-SORT takes max_age, "
                                  "min_hits, iou_thresh, det_thresh, delta_t, inertia and use_byte")
             tracker = OcSortTracker(self.gather.C, self.gather.K, det_thresh, 30 if max_age is None else max_age,
                                     3 if min_hits is None else min_hits, 0.3 if iou_thresh is None else iou_thresh, delta_t,
-                                    inertia, use_byte, self.device_index)
+                                    inertia, use_byte, self.device_index, streams)
         else:
             raise ValueError(f"tracking method {method!r}: 'sort', 'bytetrack' or 'ocsort'")
         dev = torch.device("cuda", self.device_index)
         n, C, K = self.world * self.batch, self.gather.C, self.gather.K
         self._track = dict(
             tracker=tracker, rows=torch.empty(n, dtype=torch.int32, device=dev), pos=torch.empty(n, dtype=torch.int64, device=dev),
+            streams=torch.empty(n, dtype=torch.int32, device=dev),
+            streams_host=[torch.empty(n, dtype=torch.int32).pin_memory() for _ in range(SLOTS)],
             ids=torch.empty((n, C, K), dtype=torch.int32, device=dev), boxes=torch.empty((n, C, K, 4), dtype=torch.float32, device=dev),
             rows_host=[torch.empty(n, dtype=torch.int32).pin_memory() for _ in range(SLOTS)],
             pos_host=[torch.empty(n, dtype=torch.int64).pin_memory() for _ in range(SLOTS)],
@@ -311,28 +319,31 @@ class DetectionPipeline:
             boxes_host=[torch.empty((n, C, K, 4), dtype=torch.float32).pin_memory() for _ in range(SLOTS)])
         self._track_n = [None] * SLOTS
 
-    def reset_tracks(self) -> None:
-        """Starts a new stream: no tracks, frame count 0, ids from 1, any first position.  Ordered after the batches already
-        submitted."""
+    def reset_tracks(self, stream: Optional[int] = None) -> None:
+        """Starts every stream (`stream` None), or stream `stream` alone, anew: no tracks, frame count 0, ids from 1, any
+        first position.  Ordered after the batches already submitted; the other streams are unaffected."""
         if self._track is None:
             raise RuntimeError("reset_tracks() needs enable_tracking()")
-        self._track["tracker"].reset(self._side if self.world > 1 else self._det_stream)
+        self._track["tracker"].reset(stream, self._side if self.world > 1 else self._det_stream)
 
     def tracks(self, ticket: int):
         """(ids int32 [F, C, K], boxes float32 [F, C, K, 4]) of the F frames of the ``submit_images`` batch behind `ticket`, in
         the order of its `frames`: each record's track id (-1: no track, or one not reported in this frame) and, where it
         has an id, its track's state box (ymin, xmin, ymax, xmax) after the frame; pinned host views, valid after
         ``collect(ticket)`` until the ticket's slot is reused.  Frame q is global image q: with several ranks, rank q //
-        images_per_batch's image q % images_per_batch."""
+        images_per_batch's image q % images_per_batch.  Ids count from 1 in each stream: with several streams a track is
+        identified by (stream, id)."""
         if self._track is None or self._track_n[ticket] is None:
             raise RuntimeError("no tracks for this ticket: call enable_tracking() and give submit_images() its frames")
         self._d2h_done[ticket].synchronize()
         m = self._track_n[ticket]
         return self._track["ids_host"][ticket][:m], self._track["boxes_host"][ticket][:m]
 
-    def _track_slot(self, s: int, st: torch.cuda.Stream, frames: list) -> None:
-        """Enqueues the tracking of gather slot s's frames on `st`, behind its gathered block: rows and positions H2D, one
-        launch of the tracker's kernel (k2y_track_update, k2y_bytetrack_update or k2y_ocsort_update), ids and boxes D2H."""
+    def _track_slot(self, s: int, st: torch.cuda.Stream, frames: list, streams: Optional[list], last: dict) -> None:
+        """Enqueues the tracking of gather slot s's frames (of `streams`; None: all stream 0) on `st`, behind its gathered
+        block: rows, positions and streams H2D, one launch of the tracker's kernel (k2y_track_update_streams,
+        k2y_bytetrack_update_streams or k2y_ocsort_update_streams), ids and boxes D2H.  `last`: each stream's last position
+        in the batch."""
         tk, m, B = self._track, len(frames), self._ipb
         self._track_n[s] = m
         if m == 0:
@@ -342,8 +353,12 @@ class DetectionPipeline:
         tk["pos_host"][s].numpy()[:m] = frames
         tk["rows"][:m].copy_(tk["rows_host"][s][:m], non_blocking=True)
         tk["pos"][:m].copy_(tk["pos_host"][s][:m], non_blocking=True)
+        if streams is not None:
+            tk["streams_host"][s].numpy()[:m] = streams
+            tk["streams"][:m].copy_(tk["streams_host"][s][:m], non_blocking=True)
         dets, counts = self.gather.views(s)
-        tk["tracker"].update(dets, counts, tk["rows"], tk["pos"], m, tk["ids"], tk["boxes"], st, frames[-1])
+        tk["tracker"].update(dets, counts, tk["rows"], tk["pos"], m, tk["ids"], tk["boxes"], st, last,
+                             None if streams is None else tk["streams"])
         tk["ids_host"][s][:m].copy_(tk["ids"][:m], non_blocking=True)
         tk["boxes_host"][s][:m].copy_(tk["boxes"][:m], non_blocking=True)
 
@@ -512,7 +527,8 @@ class DetectionPipeline:
         self._render_done[s].record(det)
         self._render_free[slot].record(det)
 
-    def submit_images(self, images: Sequence[np.ndarray], frames: Optional[Sequence[int]] = None) -> int:
+    def submit_images(self, images: Sequence[np.ndarray], frames: Optional[Sequence[int]] = None,
+                      streams: Optional[Sequence[int]] = None) -> int:
         """Streaming form for raw images: `images` is a list of n <= ``images_per_batch`` host numpy uint8 [h, w, 3] RGB arrays of any sizes, or
         image files (``bytes``, ``bytearray``, ``memoryview``): baseline JPEGs are decoded on the GPU on the copy stream in front
         of the letterbox, other files on the host inside this call (``preprocess.BatchLayout``).
@@ -526,7 +542,9 @@ class DetectionPipeline:
 
         With ``enable_tracking`` `frames` is required: the stream positions of the global batch's frames in gathered-row order
         (global image q is rank q // images_per_batch's image q % images_per_batch; images past len(frames) are not frames),
-        increasing along the stream.  Every rank gives the same list."""
+        increasing along the stream.  Every rank gives the same list.  With ``enable_tracking(streams=S)``, S > 1, `streams`
+        is required too: each frame's stream in 0..S-1, in the same order as `frames` (left out, every frame is stream 0);
+        positions increase along each stream, and the streams are independent of one another."""
         viewed = self._tiling is not None or self._flip
         if viewed and isinstance(images, (list, tuple)) and len(images) > self.images_per_batch:
             raise ValueError(f"{len(images)} images of {self._views} views do not fit a batch of {self.batch}")
@@ -537,10 +555,17 @@ class DetectionPipeline:
             raise ValueError(f"{n} images do not fit a batch of {self.batch}")
         if (frames is None) != (self._track is None):
             raise ValueError("submit_images takes frames= exactly when tracking is on (enable_tracking)")
+        last = None
         if frames is not None:
-            frames = self._track["tracker"].check_positions(frames)
+            tracker = self._track["tracker"]
+            if streams is None and tracker.streams > 1:
+                raise ValueError(f"submit_images takes streams= when tracking {tracker.streams} streams")
+            frames, stream_list, last = check_positions(frames, streams, tracker.last_positions)
+            streams = None if streams is None else stream_list
             if len(frames) > self.world * self._ipb or (self.world == 1 and len(frames) > n):
                 raise ValueError(f"{len(frames)} frame positions for {n} images per rank of {self.world} ranks")
+        elif streams is not None:
+            raise ValueError("submit_images takes streams= only with frames= (enable_tracking)")
         if self._render is not None:
             from .render import JPEG_MAX_DIMENSION
             for i, (h, w) in enumerate(layout.hw.tolist()):
@@ -581,7 +606,7 @@ class DetectionPipeline:
             at = self._staging[slot].dev.data_ptr() + layout.merge_table_at
             table = (at, at + 4 * (n + 1), at + 4 * (n + 1 + nv) if self._flip else None, n)
         t = self._run_slot(slot, buf, nv, self._slot_hw[slot][:nv], n if self.world == 1 else None,
-                           self._slot_yx[slot][:nv] if viewed else None, table, frames)
+                           self._slot_yx[slot][:nv] if viewed else None, table, frames, streams, last)
         self._rendered_slot[t] = self._render is not None
         if self._render is not None:
             with torch.cuda.device(dev):
@@ -589,7 +614,8 @@ class DetectionPipeline:
         return t
 
     def _run_slot(self, slot: int, buf: torch.Tensor, n: int, image_hw: Optional[torch.Tensor], rows: Optional[int],
-                  view_yx: Optional[torch.Tensor] = None, table=None, frames: Optional[list] = None) -> int:
+                  view_yx: Optional[torch.Tensor] = None, table=None, frames: Optional[list] = None,
+                  streams: Optional[list] = None, last: Optional[dict] = None) -> int:
         """Network + decode (+ all-gather) of input slot `slot` once its H2D is done, then (with `frames`) the tracking, then
         the D2H of the records."""
         compute = torch.cuda.current_stream(self.device_index)
@@ -603,7 +629,7 @@ class DetectionPipeline:
         st = self._side if self.world > 1 else self._det_stream
         with torch.cuda.stream(st):
             if frames is not None:
-                self._track_slot(s, st, frames)
+                self._track_slot(s, st, frames, streams, last)
             self._host[s].copy_(self.gather.bufs[s], non_blocking=True)
             self._d2h_done[s].record(st)
             self._slot_free[s].record(st)

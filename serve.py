@@ -40,7 +40,15 @@ are read by index (k210_yolo_framework_b200.video) and routed as JPEG files are;
 OpenCV's FFmpeg backend on the decode threads of every rank, each rank keeping its own frames.  --draw DIR then writes
 DIR/<stem>.avi, a Motion-JPEG AVI of the drawn frames at the source frame rate, on rank 0.
 
-With --track (a video only) the objects are tracked across the frames on the GPU, SORT-style (DetectionPipeline.enable_tracking,
+Several video files may be given at once (and only video files, each once): they are all served at the same time, their
+frames interleaved in the same batches (``interleave``, one frame of each video in turn), so N camera recordings share one
+pipeline and its batches instead of taking N runs.  Each video keeps its own lines, "video" naming it; the lines of
+different videos interleave in batch order, and each video's lines stay in frame order.  --draw DIR writes one
+DIR/<stem>.avi per video (two videos with one stem are refused before any work), and under --track each video is its own
+stream (DetectionPipeline.enable_tracking(streams=...)), with its own ids from 1: every video's lines are those it gives
+served alone.  One input behaves as it always has.
+
+With --track (videos only) the objects are tracked across the frames on the GPU, SORT-style (DetectionPipeline.enable_tracking,
 --track_max_age, --track_min_hits, --track_iou), or with --tracker bytetrack by ByteTrack (--track_thresh, --track_match,
 --track_buffer, --track_no_fuse_score; its low-score association sees only the records above --obj_thresh, so it wants
 --obj_thresh 0.1), or with --tracker ocsort by OC-SORT (--track_max_age, default 30, --track_min_hits, --track_iou,
@@ -129,19 +137,54 @@ def open_pipeline(args, max_per_class=30):
     return pipe, world, rank
 
 
-def draw_paths(files, out_dir):
-    """``out_dir/<stem>.jpg`` for every input file; raises ValueError when two files share a stem (their drawn results would
-    overwrite each other)."""
+def draw_paths(files, out_dir, ext=".jpg"):
+    """``out_dir/<stem><ext>`` for every input file (.avi for videos); raises ValueError when two files share a stem (their
+    drawn results would overwrite each other)."""
     seen = {}
     for p in files:
         stem = os.path.splitext(os.path.basename(p))[0]
         if stem in seen:
-            raise ValueError(f"--draw: {seen[stem]} and {p} would both be written to {stem}.jpg")
+            raise ValueError(f"--draw: {seen[stem]} and {p} would both be written to {stem}{ext}")
         seen[stem] = p
-    return [os.path.join(out_dir, os.path.splitext(os.path.basename(p))[0] + ".jpg") for p in files]
+    return [os.path.join(out_dir, os.path.splitext(os.path.basename(p))[0] + ext) for p in files]
 
 
-def detect_files(pipe, files, decode_threads=4, load=None, rendered=False, positions=None):
+def interleave(lengths, slots, G):
+    """The schedule of sequences of `lengths` frames served through `slots` stream slots, G frames a global batch: a list with
+    per global batch (frames, resets), `frames` the batch's (sequence, frame, slot) in row order and `resets` the slots to
+    reset before it.  Round-robin: one frame per active sequence a turn, in slot order (the turns carry on from one batch
+    to the next), until the batch holds G frames or no active sequence has frames left.  When a batch starts, each free
+    slot, lowest first, takes the next sequence in the given order; a slot freed in a batch is taken again from the next
+    batch only, after its reset, so two sequences never share a slot within a batch.  Sequences of no frames are skipped.
+    So one slot runs the sequences one after another, each in batches of G frames with a short last one, and slots >=
+    len(lengths) runs them all at once in full batches but the last."""
+    slots, G = int(slots), int(G)
+    if slots < 1 or G < 1:
+        raise ValueError(f"{slots} slots and {G} frames a batch: both must be >= 1")
+    todo = deque(i for i, n in enumerate(lengths) if n > 0)
+    active, used = [None] * slots, [False] * slots      # per slot: [sequence, its next frame]; whether it ever held one
+    left = lambda a: a is not None and a[1] < lengths[a[0]]
+    out, turn = [], 0
+    while todo or any(a is not None for a in active):
+        resets = []
+        for slot in range(slots):
+            if active[slot] is None and todo:
+                if used[slot]:
+                    resets.append(slot)
+                active[slot], used[slot] = [todo.popleft(), 0], True
+        frames = []
+        while len(frames) < G and any(left(a) for a in active):
+            a = active[turn]
+            if left(a):
+                frames.append((a[0], a[1], turn))
+                a[1] += 1
+            turn = (turn + 1) % slots
+        active = [a if left(a) else None for a in active]
+        out.append((frames, resets))
+    return out
+
+
+def detect_files(pipe, files, decode_threads=4, load=None, rendered=False, positions=None, schedule=None):
     """Yields ``(paths, dets, counts)`` per global batch of world * images_per_batch files, in file order: the batch's gathered
     record blocks as ``collect`` returns them (pinned host views, valid until the generator resumes twice; with tiling on
     several ranks, copies of the rows that hold images, so that row j is file j here too).  Every rank reads ITS
@@ -152,13 +195,27 @@ def detect_files(pipe, files, decode_threads=4, load=None, rendered=False, posit
     (default: load_image).  With `rendered` (the pipeline's rendering enabled) each tuple also carries this rank's drawn
     JPEG files of the batch, its padding images' files left out.  With `positions` (the pipeline's tracking enabled; each
     file's position in the stream) the batch's positions go to submit_images and each tuple ends with ``pipe.tracks``: the
-    (ids, boxes) of the batch's files, row j being file j."""
+    (ids, boxes) of the batch's files, row j being file j.
+
+    With `schedule` (``interleave``'s batches for G = world * images_per_batch) the frames of several sequences share the
+    batches instead: `files` is not used, the keys (what `load` takes and the tuples list) are (sequence, frame) pairs,
+    `positions[sequence][frame]` gives each frame's position, and with `positions` each frame's slot is its stream
+    (submit_images' `streams`) and the batch's resets run before it is submitted (``reset_tracks(slot)``)."""
     load = load or load_image
     B, G, rank = pipe.images_per_batch, pipe.world * pipe.images_per_batch, pipe.rank
     rows = None
     if pipe.world > 1 and B != pipe.batch:      # rank r's B images lie from row r * batch of the gathered block
         rows = [r * pipe.batch + j for r in range(pipe.world) for j in range(B)]
-    chunks = [files[g0:g0 + G] for g0 in range(0, len(files), G)]
+    if schedule is None:
+        chunks = [files[g0:g0 + G] for g0 in range(0, len(files), G)]
+        plan = [(chunk, None if positions is None else {"frames": [positions[g * G + q] for q in range(len(chunk))]}, [])
+                for g, chunk in enumerate(chunks)]
+    else:
+        plan = [([(i, k) for i, k, _ in frames], None if positions is None else
+                 {"frames": [positions[i][k] for i, k, _ in frames], "streams": [slot for _, _, slot in frames]}, resets)
+                for frames, resets in schedule]
+        if any(len(chunk) > G for chunk, _, _ in plan):
+            raise ValueError(f"a schedule batch holds more than the {G} frames of a global batch")
     filler = np.full(pipe.in_hw + (3,), 128, np.uint8)
     with ThreadPoolExecutor(max(1, int(decode_threads))) as pool:
         def decode(chunk):      # this rank's images of a global batch, decoding in the pool
@@ -171,12 +228,14 @@ def detect_files(pipe, files, decode_threads=4, load=None, rendered=False, posit
             return out + (pipe.tracks(ticket),) if positions is not None else out
 
         pending = deque()
-        nxt = decode(chunks[0]) if chunks else []
-        for g, chunk in enumerate(chunks):
+        nxt = decode(plan[0][0]) if plan else []
+        for g, (chunk, kw, resets) in enumerate(plan):
             imgs = [f.result() for f in nxt]
-            nxt = decode(chunks[g + 1]) if g + 1 < len(chunks) else []
-            kw = {} if positions is None else {"frames": [positions[g * G + q] for q in range(len(chunk))]}
-            pending.append((chunk, pipe.submit_images(imgs + [filler] * (B - len(imgs)), **kw), len(imgs)))
+            nxt = decode(plan[g + 1][0]) if g + 1 < len(plan) else []
+            if kw is not None:
+                for slot in resets:
+                    pipe.reset_tracks(slot)
+            pending.append((chunk, pipe.submit_images(imgs + [filler] * (B - len(imgs)), **(kw or {})), len(imgs)))
             if len(pending) == 2:
                 yield result(*pending.popleft())
         while pending:
@@ -199,11 +258,17 @@ def detections(recs, track=None):
     return out
 
 
+def input_paths(args):
+    """The input positional as a list (a single path given as a string is one input)."""
+    return [args.images] if isinstance(args.images, str) else list(args.images)
+
+
 def serve(args, out_fh=None):
     import torch.distributed as dist
-    if is_video(args.images):
+    paths = input_paths(args)
+    if is_video(paths[0]):
         return serve_video(args, out_fh)
-    files = list_images(args.images)
+    files = list_images(paths[0])
     draw_dir = getattr(args, "draw", None)
     targets = draw_paths(files, draw_dir) if draw_dir else None     # refuses duplicate stems before any work
     pipe, world, rank = open_pipeline(args)
@@ -235,30 +300,36 @@ def serve(args, out_fh=None):
 
 
 def serve_video(args, out_fh=None):
-    """``serve`` for a video file: one JSON line per frame, {"video", "frame" (its position in the stream), "time" (seconds),
-    "detections"}, in frame order.  Frames are batched and sharded over the ranks as files are (``detect_files``); Motion-JPEG
-    AVI frames are read by index and routed as image files are, other videos are decoded in order by OpenCV's FFmpeg backend on
-    every rank, each keeping its own frames.  With --draw DIR rank 0 writes DIR/<stem>.avi at the source frame rate from the
-    GPU-drawn JPEG frames, which the other ranks send it once per global batch."""
+    """``serve`` for one or more video files: one JSON line per frame, {"video", "frame" (its position in the stream), "time"
+    (seconds), "detections"}, each video's lines in frame order.  Several videos share the batches (``interleave``, one slot
+    and, under --track, one tracking stream per video), and the lines of different videos interleave in batch order.
+    Frames are batched and sharded over the ranks as files are (``detect_files``); Motion-JPEG AVI frames are read by index
+    and routed as image files are, other videos are decoded in order by OpenCV's FFmpeg backend on every rank, each keeping
+    its own frames.  With --draw DIR rank 0 writes DIR/<stem>.avi per video at its source frame rate from the GPU-drawn JPEG
+    frames, which the other ranks send it once per global batch."""
     import torch.distributed as dist
-    src = open_video(args.images)
+    paths = input_paths(args)
     draw_dir = getattr(args, "draw", None)
+    targets = draw_paths(paths, draw_dir, ".avi") if draw_dir else None      # refuses duplicate stems before any work
+    srcs = [open_video(p) for p in paths]
     pipe, world, rank = open_pipeline(args)
     if draw_dir:
         os.makedirs(draw_dir, exist_ok=True)
         pipe.enable_rendering(quality=args.draw_quality)
     track = getattr(args, "track", False)
     if track:
-        enable_tracking(pipe, args)
+        enable_tracking(pipe, args, streams=len(srcs))
     B, G = pipe.images_per_batch, pipe.world * pipe.images_per_batch
+    schedule = interleave([src.n_frames for src in srcs], len(srcs), G)
+    mine = {(i, k) for frames, _ in schedule for q, (i, k, _) in enumerate(frames) if q // B == rank}   # this rank's frames
     gpu_png, gpu_progressive = getattr(args, "gpu_png", False), getattr(args, "gpu_progressive", False)
-    load = src.loader(keep=lambda k: (k % G) // B == rank, route=lambda data: route_image(data, gpu_png, gpu_progressive))
-    target = os.path.join(draw_dir, os.path.splitext(os.path.basename(args.images))[0] + ".avi") if draw_dir else None
-    writer, n_out = None, 0
+    loads = [src.loader(keep=lambda k, i=i: (i, k) in mine, route=lambda data: route_image(data, gpu_png, gpu_progressive))
+             for i, src in enumerate(srcs)]
+    writers, n_out = [None] * len(srcs), 0
     try:
-        positions = [src.position(k) for k in range(src.n_frames)] if track else None
-        for item in detect_files(pipe, list(range(src.n_frames)), getattr(args, "decode_threads", 4), load, rendered=bool(draw_dir),
-                                 positions=positions):
+        positions = [[src.position(k) for k in range(src.n_frames)] for src in srcs] if track else None
+        for item in detect_files(pipe, None, getattr(args, "decode_threads", 4), lambda key: loads[key[0]](key[1]),
+                                 rendered=bool(draw_dir), positions=positions, schedule=schedule):
             chunk, dets, counts = item[:3]
             if draw_dir:
                 drawn = item[3]
@@ -266,22 +337,23 @@ def serve_video(args, out_fh=None):
                     parts = [None] * world if rank == 0 else None
                     dist.gather_object(drawn, parts, dst=0)
                     drawn = [d for part in parts for d in part] if rank == 0 else []
-                for data in drawn:
-                    if writer is None:
-                        writer = AviWriter(target, src.fps, jpeg_hw(data))
-                    writer.write(data)
+                for (i, _), data in zip(chunk, drawn):
+                    if writers[i] is None:
+                        writers[i] = AviWriter(targets[i], srcs[i].fps, jpeg_hw(data))
+                    writers[i].write(data)
             if rank != 0:
                 continue
             recs = DetectionPipeline.records(dets, counts)
-            for j, k in enumerate(chunk):
+            for j, (i, k) in enumerate(chunk):
                 tr = (item[-1][0][j], item[-1][1][j], counts[j]) if track else None
-                line = {"video": args.images, "frame": src.position(k), "time": src.time(k), "detections": detections(recs[j], tr)}
+                line = {"video": paths[i], "frame": srcs[i].position(k), "time": srcs[i].time(k), "detections": detections(recs[j], tr)}
                 if out_fh is not None:
                     out_fh.write(json.dumps(line) + "\n")
                 n_out += 1
     finally:
-        if writer is not None:
-            writer.close()
+        for w in writers:
+            if w is not None:
+                w.close()
     if world > 1:
         dist.barrier()
     return n_out
@@ -349,20 +421,34 @@ def quality_arg(v):
 
 
 class ServeArgParser(ModelArgParser):
-    """serve.py's parser: also refuses --track for anything but a video file."""
+    """serve.py's parser: also refuses --track for anything but video files, several inputs unless all are video files, the
+    same input twice, and with --draw two videos of one stem."""
 
     def parse_known_args(self, args=None, namespace=None):
         ns, rest = super().parse_known_args(args, namespace)
-        if getattr(ns, "track", False) and not is_video(ns.images):
-            self.error(f"--track tracks the frames of a video; {ns.images} is not a video file")
+        paths = input_paths(ns)
+        if len(paths) > 1:
+            if len({os.path.realpath(p) for p in paths}) < len(paths):
+                self.error("the same input is given twice")
+            others = [p for p in paths if not is_video(p)]
+            if others:
+                self.error(f"several inputs must all be video files; {others[0]} is not")
+            if getattr(ns, "draw", None):
+                try:
+                    draw_paths(paths, ns.draw, ".avi")
+                except ValueError as e:
+                    self.error(str(e))
+        if getattr(ns, "track", False) and not is_video(paths[0]):
+            self.error(f"--track tracks the frames of a video; {paths[0]} is not a video file")
         return ns, rest
 
 
 def build_parser():
     ap = ServeArgParser()
     add_model_args(ap)
-    ap.add_argument("images", help="directory of images, a text file with one path per line, or a video file (recognised by its "
-                                    "content: AVI, MP4 / MOV or Matroska / WebM)")
+    ap.add_argument("images", nargs="+", metavar="IMAGES",
+                    help="directory of images, a text file with one path per line, or one or more video files (recognised by "
+                         "their content: AVI, MP4 / MOV or Matroska / WebM), served together")
     ap.add_argument("--obj_thresh", type=float, default=0.7)
     ap.add_argument("--iou_thresh", type=float, default=0.5)
     ap.add_argument("--out", default="-")
@@ -431,12 +517,12 @@ def track_args_error(ns):
     return None
 
 
-def enable_tracking(pipe, args):
-    """DetectionPipeline.enable_tracking with the add_track_args flags."""
+def enable_tracking(pipe, args, streams=1):
+    """DetectionPipeline.enable_tracking with the add_track_args flags, for `streams` streams."""
     pipe.enable_tracking(args.track_max_age, args.track_min_hits, args.track_iou, method=args.tracker,
                          track_thresh=args.track_thresh, match_thresh=args.track_match, track_buffer=args.track_buffer,
                          fuse_score=not args.track_no_fuse_score, det_thresh=args.track_det_thresh,
-                         delta_t=args.track_delta_t, inertia=args.track_inertia, use_byte=args.track_use_byte)
+                         delta_t=args.track_delta_t, inertia=args.track_inertia, use_byte=args.track_use_byte, streams=streams)
 
 
 def main():
@@ -446,7 +532,7 @@ def main():
     n = serve(args, fh)
     if rank == 0 and fh is not sys.stdout:
         fh.close()
-        print(f"{n} {'frames' if is_video(args.images) else 'images'} -> {args.out}", file=sys.stderr)
+        print(f"{n} {'frames' if is_video(input_paths(args)[0]) else 'images'} -> {args.out}", file=sys.stderr)
 
 
 if __name__ == "__main__":
