@@ -585,6 +585,20 @@ int k2y_render_detections(unsigned char *images_dev, int n, const long long *off
                           int max_per_class, const unsigned char *colors_dev, void *stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Track rendering in place, pixel for pixel draw.draw_tracks (the same deliberate differences as k2y_render_detections).
+ * Images as k2y_render_detections.  atlas_dev[i]: the device track atlas of image i's font (render.TrackLabelAtlas: int32
+ * header [8] with [0] = 12 glyphs, int32 entries [12][10] of "0".."9", " ", "#", then the glyph masks).  ids_dev / boxes_dev
+ * / counts_dev: the tracker's ids int32 [n][class_num][max_per_class], track boxes float32 (ymin, xmin, ymax, xmax)
+ * [n][class_num][max_per_class][4] and the record counts [n][class_num], with the given per-image strides in elements;
+ * records with id < 0 are not drawn.  Each track is drawn in colors_dev[id % color_num] (uint8 [color_num][3]) and labelled
+ * "{class:2d} #{id}", class_num 1..80.  Asynchronous on `stream`, one launch per 128 images.
+ * ---------------------------------------------------------------------------------------- */
+int k2y_render_tracks(unsigned char *images_dev, int n, const long long *offsets_host, const int *hw_host,
+                      const int32_t *const *atlas_dev, const int32_t *ids_dev, const float *boxes_dev, const int32_t *counts_dev,
+                      long long id_image_stride, long long box_image_stride_words, long long count_image_stride, int class_num,
+                      int max_per_class, const unsigned char *colors_dev, int color_num, void *stream);
+
+/* ------------------------------------------------------------------------------------------
  * Evaluation: the counters behind the reference's Yolo_Precision / Yolo_Recall metrics (tools/custom.py:13-75) on device
  * tensors.  y_true_dev / y_pred_dev: n_boxes records of entry_floats = 5 + classes floats (any [..., A, 5+C] head or label
  * tensor, flattened); element 4 is the confidence.  counts_dev[3] (uint64, caller-zeroed, accumulated into): tp, fp, fn with

@@ -174,6 +174,9 @@ _SIGNATURES = {
     "k2y_jpeg_encode": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "k2y_render_detections": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong), POINTER(c_int), POINTER(c_void_p), c_void_p, c_void_p,
                                       ctypes.c_longlong, ctypes.c_longlong, c_int, c_int, c_void_p, c_void_p]),
+    "k2y_render_tracks": (c_int, [c_void_p, c_int, POINTER(ctypes.c_longlong), POINTER(c_int), POINTER(c_void_p), c_void_p, c_void_p,
+                                  c_void_p, ctypes.c_longlong, ctypes.c_longlong, ctypes.c_longlong, c_int, c_int, c_void_p, c_int,
+                                  c_void_p]),
     "k2y_ap_create": (c_int, [c_int, c_int, POINTER(c_float), c_int, c_int, POINTER(c_void_p)]),
     "k2y_ap_destroy": (c_int, [c_void_p]),
     "k2y_ap_match": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_longlong, ctypes.c_longlong, c_int, c_void_p, c_void_p, c_int,

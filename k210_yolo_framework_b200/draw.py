@@ -36,23 +36,45 @@ def label_font_size(image_h: int) -> int:
     return int(np.floor(3e-2 * image_h + 0.5))
 
 
-def draw_detections(orig_img: np.ndarray, found: List[Tuple], colormap, font_path: str = "asset/FiraMono-Medium.otf"):
-    """found: (class, flat_index, score, top, left, bottom, right) tuples.  Returns the annotated PIL image."""
+def _draw_labelled(orig_img: np.ndarray, items, font_path: str):
+    """Draws (box, label, colour) items onto a copy of `orig_img` as keras_inference.py:150-172 draws one detection, a later
+    item over an earlier one.  Returns the PIL image."""
     from PIL import Image, ImageDraw
     image_shape = orig_img.shape[0:2]
     pil_img = Image.fromarray(orig_img)
     font = label_font(image_shape[0], font_path)
     thickness = (image_shape[0] + image_shape[1]) // 300
-    for c, _idx, score, top, left, bottom, right in found:
-        label = "{:2d} {:.2f}".format(int(c), score)
+    for box, label, colour in items:
         draw = ImageDraw.Draw(pil_img)
         tb = draw.textbbox((0, 0), label, font=font)
         label_size = (tb[2] - tb[0], tb[3] - tb[1])
-        top, left, bottom, right, origin = box_geometry(image_shape, (top, left, bottom, right), label_size)
-        colour = tuple(int(v) for v in colormap[int(c)])
+        top, left, bottom, right, origin = box_geometry(image_shape, box, label_size)
+        colour = tuple(int(v) for v in colour)
         for j in range(thickness):
             draw.rectangle([left + j, top + j, right - j, bottom - j], outline=colour)
         draw.rectangle([origin, (origin[0] + label_size[0], origin[1] + label_size[1])], fill=colour)
         draw.text(origin, label, fill=(0, 0, 0), font=font)
         del draw
     return pil_img
+
+
+def draw_detections(orig_img: np.ndarray, found: List[Tuple], colormap, font_path: str = "asset/FiraMono-Medium.otf"):
+    """found: (class, flat_index, score, top, left, bottom, right) tuples.  Returns the annotated PIL image."""
+    return _draw_labelled(orig_img, (((top, left, bottom, right), "{:2d} {:.2f}".format(int(c), score), colormap[int(c)])
+                                     for c, _idx, score, top, left, bottom, right in found), font_path)
+
+
+def track_label(cls: int, track_id: int) -> str:
+    """The label of a drawn track: ``"{class:2d} #{track_id}"``."""
+    return "{:2d} #{}".format(int(cls), int(track_id))
+
+
+def draw_tracks(orig_img: np.ndarray, tracks: List[Tuple], colormap, font_path: str = "asset/FiraMono-Medium.otf"):
+    """tracks: (class, track_id, top, left, bottom, right) tuples, the track boxes of one frame in the order
+    ``DetectionPipeline.tracks`` lays them out (class ascending, then record order).  Draws each as ``draw_detections`` draws
+    a record (font, ring thickness, geometry, label origin, a later track over an earlier one), with three differences: the
+    box is the track's, the colour is ``colormap[track_id % len(colormap)]``, so it follows the track and an id switch shows as
+    a colour change, and the label is ``"{class:2d} #{track_id}"``.  Tracks with id -1 (none) are not drawn.  Returns the
+    annotated PIL image."""
+    return _draw_labelled(orig_img, (((top, left, bottom, right), track_label(c, tid), colormap[int(tid) % len(colormap)])
+                                     for c, tid, top, left, bottom, right in tracks if int(tid) >= 0), font_path)

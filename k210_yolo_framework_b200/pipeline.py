@@ -23,7 +23,8 @@ slot's ``image_hw``, so two batches in flight each carry their own original size
 ``enable_rendering`` adds the drawn result to ``submit_images``: behind the NMS, on the decode stream, the batch's local records
 are drawn onto its original images where they lie in the slot's device staging buffer and encoded as JPEG files;
 ``rendered(ticket)`` brings them back after ``collect`` with one exact-size copy.  The next ``submit_images`` into that input
-slot waits for the render before it overwrites the originals.
+slot waits for the render before it overwrites the originals.  ``enable_rendering(tracks=True)`` draws the batch's tracks
+instead (``k2y_render_tracks``): behind the tracking launch, on the stream that runs it.
 
 ``enable_tiling`` makes ``submit_images`` detect on overlapping tiles of each image as well as on the whole image: a batch of
 n <= batch // V images is letterboxed as n * V views, the network and the decode run on those, and one more per-class NMS
@@ -484,23 +485,35 @@ class DetectionPipeline:
         self._track_n[t] = None
         return t
 
-    def enable_rendering(self, quality: int = 75, font_path: str = "asset/FiraMono-Medium.otf", colormap=None) -> None:
+    def enable_rendering(self, quality: int = 75, font_path: str = "asset/FiraMono-Medium.otf", colormap=None, *,
+                         tracks: bool = False) -> None:
         """From now on every ``submit_images`` batch also has its local records drawn onto its original images (as
         ``draw.draw_detections`` draws them, ``render.render_detections_device``) and encoded as JPEG files (as PIL saves them at
         `quality`, ``render.JpegEncoder``), on the decode stream behind the NMS; ``rendered(ticket)`` returns them after
         ``collect``.  `colormap`: RGB triples per class (default ``Helper.colormap``, 80 classes).  Records and ``collect``
         are unchanged.  ``submit_images`` then refuses an image with more than ``render.JPEG_MAX_DIMENSION`` (65500) rows or
-        columns, which no JPEG file can hold."""
+        columns, which no JPEG file can hold.
+
+        With `tracks` each image is drawn with its tracks instead, as ``draw.draw_tracks`` draws the frame's rows of
+        ``tracks(ticket)`` (``render.render_tracks_device``): every record with a track id, its track box in colour
+        ``colormap[id % len(colormap)]``, labelled ``"{class:2d} #{id}"``.  An image that is not one of the batch's frames is
+        encoded undrawn.  ``submit_images`` then needs tracking on (``enable_tracking``)."""
         from .helper import _COLORMAP
-        from .render import JpegEncoder, LabelAtlas, color_table
+        from .render import MAX_CLASSES, JpegEncoder, LabelAtlas, TrackLabelAtlas, color_table, track_color_table
         colormap = _COLORMAP if colormap is None else colormap
         C = self.gather.C
-        if C > len(colormap):
+        if C > len(colormap) and not tracks:
             raise ValueError(f"class_num {C} exceeds the colormap's {len(colormap)} classes")
         if not 1 <= int(quality) <= 100:
             raise ValueError(f"quality {quality} is outside 1..100")
         dev = torch.device("cuda", self.device_index)
-        self._render = dict(quality=int(quality), atlas=LabelAtlas(C, font_path), colors=color_table(colormap, C, dev),
+        if tracks:
+            if C > MAX_CLASSES:
+                raise ValueError(f"class_num {C}: tracks are drawn for at most {MAX_CLASSES} classes")
+            atlas, colors = TrackLabelAtlas(font_path), track_color_table(colormap, dev)
+        else:
+            atlas, colors = LabelAtlas(C, font_path), color_table(colormap, C, dev)
+        self._render = dict(quality=int(quality), atlas=atlas, colors=colors, tracks=bool(tracks),
                             encoders=[JpegEncoder(dev) for _ in range(SLOTS)])
 
     def rendered(self, ticket: int) -> List[bytes]:
@@ -526,6 +539,27 @@ class DetectionPipeline:
             r["encoders"][s].enqueue(staging.dev.data_ptr(), layout.offsets, layout.hw, r["quality"], det)
         self._render_done[s].record(det)
         self._render_free[slot].record(det)
+
+    def _render_tracks_slot(self, slot: int, s: int, layout: BatchLayout, st: torch.cuda.Stream) -> None:
+        """Draws the tracks of this rank's frames of gather slot s onto input slot `slot`'s originals and encodes them, on
+        `st`, the stream that ran the slot's tracking, right behind it.  The device ids and boxes hold one batch's tracks:
+        the next batch's tracking, enqueued on `st` by a later ``submit_images``, overwrites them only after this render."""
+        from .render import render_tracks_packed
+        r, tk = self._render, self._track
+        st.wait_event(self._h2d_done[slot])      # the originals are in place (already implied by the network's wait)
+        staging = self._staging[slot]
+        n = len(layout)
+        q0, row0 = self.rank * self._ipb, self.rank * self.batch    # this rank's first frame and its gathered row
+        drawn = min(n, max(0, (self._track_n[s] or 0) - q0))        # images past the batch's frames are encoded undrawn
+        with torch.cuda.device(staging.dev.device):
+            if drawn:
+                _, counts = self.gather.views(s)
+                render_tracks_packed(staging.dev.data_ptr(), layout.offsets[:drawn], layout.hw[:drawn], counts[row0:row0 + drawn],
+                                     tk["ids"][q0:q0 + drawn], tk["boxes"][q0:q0 + drawn], r["atlas"], r["colors"],
+                                     staging.dev.device, st)
+            r["encoders"][s].enqueue(staging.dev.data_ptr(), layout.offsets, layout.hw, r["quality"], st)
+        self._render_done[s].record(st)
+        self._render_free[slot].record(st)
 
     def submit_images(self, images: Sequence[np.ndarray], frames: Optional[Sequence[int]] = None,
                       streams: Optional[Sequence[int]] = None) -> int:
@@ -566,6 +600,11 @@ class DetectionPipeline:
                 raise ValueError(f"{len(frames)} frame positions for {n} images per rank of {self.world} ranks")
         elif streams is not None:
             raise ValueError("submit_images takes streams= only with frames= (enable_tracking)")
+        if self._render is not None and self._render["tracks"]:
+            if self._track is None:
+                raise ValueError("enable_rendering(tracks=True) draws the tracks: call enable_tracking() too")
+            for h in sorted({h for h, _ in layout.hw.tolist()}):
+                self._render["atlas"].host(h)   # builds the glyphs of each new font size here: a refused font raises now
         if self._render is not None:
             from .render import JPEG_MAX_DIMENSION
             for i, (h, w) in enumerate(layout.hw.tolist()):
@@ -605,19 +644,21 @@ class DetectionPipeline:
         if layout.merge_table_at is not None:     # the view offsets, sides and mirror flags, where the H2D copy put them
             at = self._staging[slot].dev.data_ptr() + layout.merge_table_at
             table = (at, at + 4 * (n + 1), at + 4 * (n + 1 + nv) if self._flip else None, n)
+        draw_tracks = self._render is not None and self._render["tracks"]
         t = self._run_slot(slot, buf, nv, self._slot_hw[slot][:nv], n if self.world == 1 else None,
-                           self._slot_yx[slot][:nv] if viewed else None, table, frames, streams, last)
+                           self._slot_yx[slot][:nv] if viewed else None, table, frames, streams, last,
+                           (lambda s, st: self._render_tracks_slot(slot, s, layout, st)) if draw_tracks else None)
         self._rendered_slot[t] = self._render is not None
-        if self._render is not None:
+        if self._render is not None and not draw_tracks:
             with torch.cuda.device(dev):
                 self._render_slot(slot, t, layout)
         return t
 
     def _run_slot(self, slot: int, buf: torch.Tensor, n: int, image_hw: Optional[torch.Tensor], rows: Optional[int],
                   view_yx: Optional[torch.Tensor] = None, table=None, frames: Optional[list] = None,
-                  streams: Optional[list] = None, last: Optional[dict] = None) -> int:
+                  streams: Optional[list] = None, last: Optional[dict] = None, after_track=None) -> int:
         """Network + decode (+ all-gather) of input slot `slot` once its H2D is done, then (with `frames`) the tracking, then
-        the D2H of the records."""
+        the D2H of the records, then ``after_track(gather slot, stream)`` on the same stream (the track drawing)."""
         compute = torch.cuda.current_stream(self.device_index)
         compute.wait_event(self._h2d_done[slot])
         self.engine.bind_input(buf)
@@ -632,6 +673,8 @@ class DetectionPipeline:
                 self._track_slot(s, st, frames, streams, last)
             self._host[s].copy_(self.gather.bufs[s], non_blocking=True)
             self._d2h_done[s].record(st)
+            if after_track is not None:
+                after_track(s, st)
             self._slot_free[s].record(st)
         return s
 
@@ -762,8 +805,12 @@ class LanedPipeline:
         k, t = ticket
         return self.lanes[k].collect(t)
 
-    def enable_rendering(self, quality: int = 75, font_path: str = "asset/FiraMono-Medium.otf", colormap=None) -> None:
-        """``DetectionPipeline.enable_rendering`` on every lane."""
+    def enable_rendering(self, quality: int = 75, font_path: str = "asset/FiraMono-Medium.otf", colormap=None, *,
+                         tracks: bool = False) -> None:
+        """``DetectionPipeline.enable_rendering`` on every lane.  Not with `tracks`: the lanes do not track."""
+        if tracks:
+            raise NotImplementedError("track drawing needs tracking, which runs on a DetectionPipeline; a LanedPipeline's lanes "
+                                      "cannot order one stream's frames")
         for ln in self.lanes:
             ln.enable_rendering(quality, font_path, colormap)
 

@@ -7,6 +7,10 @@ pixel for pixel what ``draw.draw_detections`` draws.  The label glyphs come from
 mask offset and ``textbbox`` size of every ``(class, hundredths)`` label, taken from Pillow on the host exactly as
 ``ImageDraw.text`` / ``textbbox`` get them, cached per font size and uploaded once.
 
+``render_tracks_device`` draws a tracker's output the same way (``k2y_render_tracks``), as ``draw.draw_tracks`` draws it:
+each record's track box in its id's colour, labelled ``"{class:2d} #{id}"``.  Ids are unbounded, so its ``TrackLabelAtlas``
+holds the label's 12 glyphs per font size and the kernel composes each label from them.
+
 ``encode_jpeg_batch`` encodes CUDA uint8 [h, w, 3] images as baseline JPEG files byte-identical to
 ``PIL.Image.fromarray(x).save(f, "JPEG", quality=q)`` (``k2y_jpeg_encode``, csrc/jpeg_encode.cu): the headers are built on the
 host, colour conversion, downsampling, FDCT, quantisation, Huffman coding and byte stuffing run on the device, one launch per
@@ -27,6 +31,8 @@ LABELS_PER_CLASS = 101      # hundredths 0..100
 HEADER_WORDS = 8            # atlas header: [0] classes
 ENTRY_WORDS = 8             # mask byte offset, mask w, mask h, mask x, mask y, label w, label h, 0
 MAX_CLASSES = 80            # the colour table's classes (Helper.colormap)
+TRACK_GLYPHS = "0123456789 #"   # the glyphs of a track label, in track atlas order
+TRACK_ENTRY_WORDS = 10      # mask byte offset, mask w, mask h, mask x, mask y, textbbox left, top, right, bottom, advance
 JPEG_MAX_DIMENSION = 65500  # libjpeg-turbo's limit: PIL neither writes nor reads a JPEG with more rows or columns
 _LL = ctypes.POINTER(ctypes.c_longlong)
 _INT = ctypes.POINTER(ctypes.c_int)
@@ -73,14 +79,12 @@ def build_atlas(font, class_num: int) -> np.ndarray:
     return np.concatenate([header, entries.reshape(-1), blob.view(np.int32)])
 
 
-class LabelAtlas:
-    """The label glyphs of every ``(class, hundredths)`` for the font ``draw.label_font`` picks per image height, built on the
-    host once per font size (about 0.3 s per 2020 labels) and uploaded once per device."""
+class _FontAtlas:
+    """Atlas words per font size of the font ``draw.label_font`` picks per image height, built on the host once per size
+    (``_build(font)``) and uploaded once per device."""
 
-    def __init__(self, class_num: int, font_path: str = "asset/FiraMono-Medium.otf"):
-        if not 1 <= int(class_num) <= MAX_CLASSES:
-            raise ValueError(f"class_num {class_num} is outside 1..{MAX_CLASSES}")
-        self.class_num, self.font_path = int(class_num), font_path
+    def __init__(self, font_path: str):
+        self.font_path = font_path
         self._key_of_size: Dict[int, object] = {}
         self._host: Dict[object, np.ndarray] = {}
         self._dev: Dict[tuple, torch.Tensor] = {}
@@ -97,7 +101,7 @@ class LabelAtlas:
                 font = ImageFont.load_default()
                 key = ("default",)
             if key not in self._host:
-                self._host[key] = build_atlas(font, self.class_num)
+                self._host[key] = self._build(font)
             self._key_of_size[size] = key
         return key
 
@@ -112,6 +116,73 @@ class LabelAtlas:
             torch.cuda.synchronize(device)      # visible to every stream before first use
             self._dev[key] = t
         return t
+
+
+class LabelAtlas(_FontAtlas):
+    """The label glyphs of every ``(class, hundredths)`` for the font ``draw.label_font`` picks per image height, built on the
+    host once per font size (about 0.3 s per 2020 labels) and uploaded once per device."""
+
+    def __init__(self, class_num: int, font_path: str = "asset/FiraMono-Medium.otf"):
+        if not 1 <= int(class_num) <= MAX_CLASSES:
+            raise ValueError(f"class_num {class_num} is outside 1..{MAX_CLASSES}")
+        super().__init__(font_path)
+        self.class_num = int(class_num)
+
+    def _build(self, font) -> np.ndarray:
+        return build_atlas(font, self.class_num)
+
+
+def check_track_font(font) -> None:
+    """Raises ``ValueError`` unless the advances of the track label's glyphs are whole pixels that add up without kerning,
+    over every pair: then glyph i of a label starts at the integer pen position sum(advance[c_j] for j < i), which is what
+    ``k2y_render_tracks`` composes the label from."""
+    adv = {}
+    for ch in TRACK_GLYPHS:
+        a = font.getlength(ch)
+        if a != int(a):
+            raise ValueError(f"the advance of {ch!r} is {a} pixels, not a whole number: track labels cannot be composed per glyph")
+        adv[ch] = int(a)
+    for a in TRACK_GLYPHS:
+        for b in TRACK_GLYPHS:
+            if font.getlength(a + b) != adv[a] + adv[b]:
+                raise ValueError(f"{a + b!r} advances {font.getlength(a + b)} pixels, not {adv[a]} + {adv[b]} (kerning): track "
+                                 "labels cannot be composed per glyph")
+
+
+def build_track_atlas(font) -> np.ndarray:
+    """The track atlas words of `font`: int32 header [8] ([0] glyphs), entries [12][10] of the glyphs of ``TRACK_GLYPHS``
+    (mask byte offset, mask w, mask h, mask x, mask y, textbbox left, top, right, bottom, advance), then the masks.  Raises
+    ``ValueError`` for a font ``check_track_font`` refuses."""
+    from PIL import Image, ImageDraw
+    check_track_font(font)
+    draw = ImageDraw.Draw(Image.new("RGB", (1, 1)))
+    entries = np.zeros((len(TRACK_GLYPHS), TRACK_ENTRY_WORDS), np.int32)
+    masks, off = [], 0
+    for g, ch in enumerate(TRACK_GLYPHS):
+        m, (mx, my), _ = glyphs(font, ch)
+        tb = draw.textbbox((0, 0), ch, font=font)
+        entries[g] = (off, m.shape[1], m.shape[0], mx, my, tb[0], tb[1], tb[2], tb[3], int(font.getlength(ch)))
+        masks.append(m.reshape(-1))
+        off += m.size
+    blob = np.concatenate(masks + [np.zeros((-off) % 4, np.uint8)])
+    header = np.zeros(HEADER_WORDS, np.int32)
+    header[0] = len(TRACK_GLYPHS)
+    return np.concatenate([header, entries.reshape(-1), blob.view(np.int32)])
+
+
+class TrackLabelAtlas(_FontAtlas):
+    """The 12 glyphs of the track labels ``"{class:2d} #{track_id}"`` (``TRACK_GLYPHS``: digits, space and ``#``) for the
+    font ``draw.label_font`` picks per image height: per glyph the mask and mask offset ``ImageDraw.text`` draws it with, its
+    ``textbbox`` and its advance, built on the host once per font size and uploaded once per device.  ``k2y_render_tracks``
+    composes any label from them, ids being unbounded.  Raises ``ValueError`` (when a font size is first used) for a font
+    whose advances of these glyphs are fractional or kern."""
+
+    def __init__(self, font_path: str = "asset/FiraMono-Medium.otf"):
+        super().__init__(font_path)
+
+    @staticmethod
+    def _build(font) -> np.ndarray:
+        return build_track_atlas(font)
 
 
 def color_table(colormap, class_num: int, device: torch.device) -> torch.Tensor:
@@ -168,6 +239,56 @@ def render_detections_device(images: Sequence[torch.Tensor], dets: torch.Tensor,
     colors = color_table(_COLORMAP if colormap is None else colormap, atlas.class_num, dev)
     with torch.cuda.device(dev):
         render_packed(base, offsets, hw, dets, counts, atlas, colors, dev, st)
+    colors.record_stream(st)
+
+
+def track_color_table(colormap, device: torch.device) -> torch.Tensor:
+    """Every colormap entry on the device: a track's colour is ``colormap[id % len(colormap)]``."""
+    if len(colormap) < 1:
+        raise ValueError("the colormap has no colours")
+    t = torch.tensor(np.asarray(colormap, np.uint8).reshape(len(colormap), 3)).to(device)
+    torch.cuda.synchronize(device)
+    return t
+
+
+def render_tracks_packed(base_ptr: int, offsets: np.ndarray, hw: np.ndarray, counts: torch.Tensor, ids: torch.Tensor,
+                         boxes: torch.Tensor, atlas: TrackLabelAtlas, colors: torch.Tensor, device: torch.device,
+                         stream: torch.cuda.Stream) -> None:
+    """``k2y_render_tracks`` over images packed at `offsets` from `base_ptr` (device), asynchronous on `stream`."""
+    n = len(offsets)
+    if ids.dim() != 3 or counts.dim() != 2:
+        raise ValueError("ids must be CUDA int32 [n, C, K], boxes CUDA float32 [n, C, K, 4], counts CUDA int32 [n, C]")
+    C, K = ids.shape[1], ids.shape[2]
+    if (ids.dtype != torch.int32 or boxes.dtype != torch.float32 or counts.dtype != torch.int32 or
+            tuple(ids.stride()[1:]) != (K, 1) or boxes.dim() != 4 or tuple(boxes.shape[1:]) != (C, K, 4) or
+            tuple(boxes.stride()[1:]) != (K * 4, 4, 1) or counts.shape[1] != C or counts.stride(1) != 1 or
+            min(ids.shape[0], boxes.shape[0], counts.shape[0]) < n or not (ids.is_cuda and boxes.is_cuda and counts.is_cuda)):
+        raise ValueError(f"ids must be CUDA int32 [n, C, K], boxes CUDA float32 [n, C, K, 4], counts CUDA int32 [n, C], dense per "
+                         f"image (got {tuple(ids.shape)}, {tuple(boxes.shape)}, {tuple(counts.shape)})")
+    if not 1 <= C <= MAX_CLASSES:
+        raise ValueError(f"class_num {C} is outside 1..{MAX_CLASSES}")
+    tables = [atlas.device(int(h), device) for h, _ in hw]
+    ptrs = (ctypes.c_void_p * n)(*[t.data_ptr() for t in tables])
+    offsets = np.ascontiguousarray(offsets, np.int64)
+    hw = np.ascontiguousarray(hw, np.int32)
+    check(lib.k2y_render_tracks(ctypes.c_void_p(base_ptr), n, offsets.ctypes.data_as(_LL), hw.ctypes.data_as(_INT), ptrs,
+                                ids.data_ptr(), boxes.data_ptr(), counts.data_ptr(), ids.stride(0), boxes.stride(0), counts.stride(0),
+                                C, K, colors.data_ptr(), colors.shape[0], ctypes.c_void_p(stream.cuda_stream)))
+
+
+def render_tracks_device(images: Sequence[torch.Tensor], counts: torch.Tensor, ids: torch.Tensor, boxes: torch.Tensor,
+                         atlas: TrackLabelAtlas, colormap=None, stream: Optional[torch.cuda.Stream] = None) -> None:
+    """Draws image i's tracks onto ``images[i]`` (contiguous CUDA uint8 [h, w, 3]) in place, as ``draw.draw_tracks`` would:
+    record k of class c (k < ``counts[i, c]``, int32 [n, C]) with ``ids[i, c, k]`` >= 0 (int32 [n, C, K]) is drawn with its
+    track box ``boxes[i, c, k]`` (float32 [n, C, K, 4], ymin, xmin, ymax, xmax), labelled ``"{c:2d} #{id}"``, in colour
+    ``colormap[id % len(colormap)]`` (default ``Helper.colormap``): the layout ``DetectionPipeline.tracks`` returns, as device
+    tensors.  Asynchronous on `stream` (default: the current stream)."""
+    from .helper import _COLORMAP
+    dev, base, offsets, hw = _check_views(images)
+    st = stream if stream is not None else torch.cuda.current_stream(dev)
+    colors = track_color_table(_COLORMAP if colormap is None else colormap, dev)
+    with torch.cuda.device(dev):
+        render_tracks_packed(base, offsets, hw, counts, ids, boxes, atlas, colors, dev, st)
     colors.record_stream(st)
 
 

@@ -40,13 +40,22 @@ scored dense_voc stream and at "coco_bound", 80 classes of 100 with max_age 39, 
 that it holds its bound of 4,000 tracks) and ocsort_ref (oracle/ocsort_ref.py on the host).  The GPU's ids and boxes on the
 route's records and on the first batch of dense_voc must equal ocsort_ref's; the run fails otherwise.
 
+With --draw_tracks, also the track drawing (DetectionPipeline.enable_rendering(tracks=True), SORT, default setting):
+  draw_plain /   the GPU route with --track --draw on two fresh pipelines, one drawing the records and one the tracks
+  draw_tracks:   (--draw_tracks), windows alternating; every frame of the tracks' AVI must equal draw.draw_tracks of the
+                 frame with its tracks + PIL's save, byte for byte, and the records of both must equal the gpu route's;
+  render_kernel: CUDA-event time of k2y_render_tracks and of k2y_render_detections on the same 32 decoded frames, drawing
+                 that batch's tracks and records: windows of 50 launches enqueued back to back on one stream through the
+                 packed entry points (colour tables and atlases built once, no synchronise between launches), the two
+                 kernels' windows alternating, median of the windows.
+
 The video: the bench_ingest photos resized to 1280x720 with the golden dog photo pasted in (so that there are records to
 compare), written as a Motion-JPEG AVI at 4:2:2, quality 90, without DHT segments, as cameras write them.  Every route runs
 once to warm up and then `--windows` timed passes (median).  All Motion-JPEG routes must give the same records, and the mp4v
 route the records of its own decoded pixels; the run fails otherwise.  The card's name, power limit and SM clock are read in
 the same run.  Prints one JSON line.
 
-    python scripts/bench_video.py [--frames 256 --batch 32 --windows 3 --track [bytetrack | ocsort]]
+    python scripts/bench_video.py [--frames 256 --batch 32 --windows 3 --track [bytetrack | ocsort] --draw_tracks]
 """
 import argparse
 import io
@@ -131,6 +140,7 @@ def main():
     ap.add_argument("--track", nargs="?", const="sort", default=None, choices=["sort", "bytetrack", "ocsort"],
                     help="also measure SORT tracking on the GPU and on the host; `--track bytetrack` measures ByteTrack too, "
                          "`--track ocsort` OC-SORT")
+    ap.add_argument("--draw_tracks", action="store_true", help="also measure drawing the tracks (route and kernel)")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_video measures on a GPU"
     import cv2
@@ -192,6 +202,8 @@ def main():
         make_pipe = lambda obj_thresh=0.3: new_pipeline(anchors, args.batch, obj_thresh)     # noqa: E731
         track = bench_track(make_pipe, n, gpu_load, recs["gpu"], args.batch, args.windows) if args.track else None
         scored = bench_scored(make_pipe, n, gpu_load, args.batch, args.windows, args.track) if args.track in SCORED else None
+        drawing = bench_draw_tracks(make_pipe, n, src, gpu_load, decoded, recs["gpu"], args.batch, args.windows, tmp) \
+            if args.draw_tracks else None
         gpu = gpu_info()
     mjpeg = [recs[k] for k in ("gpu", "pil_1", "pil_4", "pil_16", "pixels", "draw")]
     same = all(r is not None and r == mjpeg[0] for r in mjpeg) and recs["ffmpeg_mp4v"] == mp4_ref and drawn_frames == n
@@ -201,13 +213,98 @@ def main():
         "video": f"MJPEG AVI {W720}x{H720} 4:2:2 q90 without DHT", "avi_bytes": avi_bytes, "mp4v_bytes": mp4_bytes,
         "gpu_decoded_frames": int(gpu_frames), "records": int(sum(len(r) for r in mjpeg[0] or [])), "frames_per_s": rate,
         "windows_s": {k: [round(t, 4) for t in v] for k, v in times.items()}, "records_equal": same,
-        **({"track": track} if track else {}), **({args.track: scored} if scored else {}), "gpu": gpu}))
+        **({"track": track} if track else {}), **({args.track: scored} if scored else {}),
+        **({"draw_tracks": drawing} if drawing else {}), "gpu": gpu}))
     if not same:
         sys.exit("the routes' records differ")
     if track and not track["ids_equal"]:
         sys.exit("the GPU tracker's ids and boxes differ from oracle/sort_ref.py's")
     if scored and not scored["ids_equal"]:
         sys.exit(f"the GPU {SCORED[args.track]}'s ids and boxes differ from oracle/{args.track}_ref.py's")
+    if drawing and not (drawing["frames_equal_pil"] and drawing["records_equal"]):
+        sys.exit("the drawn tracks differ from draw.draw_tracks + PIL's save, or the records from the gpu route's")
+
+
+def draw_tracks_of(img, k, tracks, recs, batch, colormap):
+    """Frame k drawn by draw.draw_tracks with its tracks (the route's per-batch (ids, boxes) and per-frame records), saved as
+    PIL saves it at quality 75."""
+    from k210_yolo_framework_b200.draw import draw_tracks
+    ids, boxes = (x[k % batch].numpy() for x in tracks[k // batch])
+    seen, found = {}, []
+    for c, *_ in recs[k]:
+        j = seen[c] = seen.get(c, -1) + 1
+        found.append((c, int(ids[c, j]), *(float(v) for v in boxes[c, j])))
+    b = io.BytesIO()
+    draw_tracks(img, found, colormap).save(b, "JPEG", quality=75)
+    return b.getvalue()
+
+
+def bench_draw_tracks(make_pipe, n, src, load, decoded, gpu_recs, batch, windows, tmp):
+    """The --draw_tracks arms: --track --draw against --track --draw --draw_tracks on the route, and k2y_render_tracks
+    against k2y_render_detections on one batch of decoded frames."""
+    from k210_yolo_framework_b200.helper import _COLORMAP
+    from k210_yolo_framework_b200.render import (LabelAtlas, TrackLabelAtlas, color_table, render_packed, render_tracks_packed,
+                                                 track_color_table)
+    pipes, paths, tracks, recs = {}, {}, {}, {}
+    for name, on in (("draw_plain", False), ("draw_tracks", True)):
+        pipes[name] = make_pipe()
+        pipes[name].enable_tracking()
+        pipes[name].enable_rendering(quality=75, tracks=on)
+        paths[name] = os.path.join(tmp, f"{name}.avi")
+    times = {name: [] for name in pipes}
+    for w in range(windows + 1):          # window 0 warms up; the order alternates
+        for name in (list(pipes) if w % 2 == 0 else list(pipes)[::-1]):
+            pipes[name].reset_tracks()
+            tracks[name] = []
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            recs[name] = run(pipes[name], n, load, 4, paths[name], tracks=tracks[name])
+            torch.cuda.synchronize()
+            if w:
+                times[name].append(time.perf_counter() - t0)
+    drawn = open_video(paths["draw_tracks"])
+    frames_equal = drawn.n_frames == n and all(
+        drawn.frame_bytes(k) == draw_tracks_of(decoded[k], k, tracks["draw_tracks"], recs["draw_tracks"], batch, _COLORMAP)
+        for k in range(n))
+    # the kernels: the first batch's frames, records and tracks on the device
+    m = min(batch, n)
+    pipe = make_pipe()
+    pipe.enable_tracking()
+    t = pipe.submit_images([src.frame_bytes(k) for k in range(m)], frames=list(range(m)))
+    dets, counts = (x[:m].cuda() for x in pipe.collect(t))
+    ids, boxes = (x[:m].cuda() for x in pipe.tracks(t))
+    buf = torch.empty((m, H720, W720, 3), dtype=torch.uint8, device="cuda")
+    buf.copy_(torch.from_numpy(np.stack(decoded[:m])))
+    # the packed entry points with colour tables built once and atlases uploaded by the warm-up: nothing but the launch's host
+    # setup between two launches, no synchronise
+    dev, st = buf.device, torch.cuda.current_stream()
+    offsets = np.arange(m, dtype=np.int64) * (H720 * W720 * 3)
+    hw = np.array([[H720, W720]] * m, np.int32)
+    det_atlas, track_atlas = LabelAtlas(20), TrackLabelAtlas()
+    det_colors, track_colors = color_table(_COLORMAP, 20, dev), track_color_table(_COLORMAP, dev)
+    calls = {"render_detections": lambda: render_packed(buf.data_ptr(), offsets, hw, dets, counts, det_atlas, det_colors, dev, st),
+             "render_tracks": lambda: render_tracks_packed(buf.data_ptr(), offsets, hw, counts, ids, boxes, track_atlas,
+                                                           track_colors, dev, st)}
+    for fn in calls.values():
+        fn()
+    kernel = {name: [] for name in calls}
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
+    for w in range(max(windows, 5)):
+        for name in (list(calls) if w % 2 == 0 else list(calls)[::-1]):
+            ev[0].record()
+            for _ in range(50):
+                calls[name]()
+            ev[1].record()
+            ev[1].synchronize()
+            kernel[name].append(ev[0].elapsed_time(ev[1]) / 50)
+    return {"frames_per_s": {k: round(n / statistics.median(v), 1) for k, v in times.items()},
+            "windows_s": {k: [round(x, 4) for x in v] for k, v in times.items()},
+            "render_kernel_ms_per_batch": {k: round(statistics.median(v), 4) for k, v in kernel.items()},
+            "kernel_batch": f"{m} frames {W720}x{H720}, {int(counts.clamp(min=0).sum())} records, "
+                            f"{int((ids >= 0).sum())} with a track",
+            "tracks_drawn": int(sum(int((i >= 0).sum()) for i, _ in tracks["draw_tracks"])),
+            "records_equal": recs["draw_plain"] == gpu_recs and recs["draw_tracks"] == gpu_recs,
+            "frames_equal_pil": bool(frames_equal)}
 
 
 def frame_blocks(recs, C, K, scores=False):

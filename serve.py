@@ -54,7 +54,9 @@ With --track (videos only) the objects are tracked across the frames on the GPU,
 --obj_thresh 0.1), or with --tracker ocsort by OC-SORT (--track_max_age, default 30, --track_min_hits, --track_iou,
 --track_det_thresh, --track_delta_t, --track_inertia, --track_use_byte): every detection of a line gains "track", its track id
 or null, and "track_box_tlbr", the track's box, when it has an id (under OC-SORT the record's own box).  Dropped frames count
-as frames without detections.
+as frames without detections.  With --track --draw DIR --draw_tracks each DIR/<stem>.avi shows the tracks instead of the
+records (DetectionPipeline.enable_rendering(tracks=True), draw.draw_tracks): every track box in the colour of its id, labelled
+"{class:2d} #{id}", so an id switch shows as a change of colour and label.  The JSON lines do not change.
 """
 import argparse
 import io
@@ -315,7 +317,7 @@ def serve_video(args, out_fh=None):
     pipe, world, rank = open_pipeline(args)
     if draw_dir:
         os.makedirs(draw_dir, exist_ok=True)
-        pipe.enable_rendering(quality=args.draw_quality)
+        pipe.enable_rendering(quality=args.draw_quality, tracks=getattr(args, "draw_tracks", False))
     track = getattr(args, "track", False)
     if track:
         enable_tracking(pipe, args, streams=len(srcs))
@@ -422,7 +424,7 @@ def quality_arg(v):
 
 class ServeArgParser(ModelArgParser):
     """serve.py's parser: also refuses --track for anything but video files, several inputs unless all are video files, the
-    same input twice, and with --draw two videos of one stem."""
+    same input twice, with --draw two videos of one stem, and --draw_tracks without --track and --draw."""
 
     def parse_known_args(self, args=None, namespace=None):
         ns, rest = super().parse_known_args(args, namespace)
@@ -440,6 +442,8 @@ class ServeArgParser(ModelArgParser):
                     self.error(str(e))
         if getattr(ns, "track", False) and not is_video(paths[0]):
             self.error(f"--track tracks the frames of a video; {paths[0]} is not a video file")
+        if getattr(ns, "draw_tracks", False) and not (getattr(ns, "track", False) and getattr(ns, "draw", None)):
+            self.error("--draw_tracks draws the tracks into the --draw videos: it needs --track and --draw")
         return ns, rest
 
 
@@ -460,6 +464,9 @@ def build_parser():
                     help="track objects across a video's frames on the GPU (SORT, or --tracker bytetrack or ocsort): each "
                          "detection gains its track id and box")
     add_track_args(ap, " (--track)")
+    ap.add_argument("--draw_tracks", action="store_true",
+                    help="draw the tracks into the --draw videos instead of the detections: each track box in its id's colour, "
+                         "labelled with class and id (needs --track and --draw)")
     return ap
 
 
